@@ -1,7 +1,7 @@
-# Build of libape_b200.so (sm_100a only) and the oracle's C restatement.
+# Build of libape_b200.so (sm_90a only) and the oracle's C restatement.
 # `python -c "import __graft_entry__ as g; g.build()"` runs the same commands.
 NVCC      ?= nvcc
-NVCCFLAGS ?= -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 \
+NVCCFLAGS ?= -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
              -Xcompiler -fPIC -Iinclude
 CSRC      := $(wildcard ape_b200/csrc/*.cu)
 OBJS      := $(patsubst ape_b200/csrc/%.cu,build/%.o,$(CSRC))
@@ -14,7 +14,7 @@ build/%.o: ape_b200/csrc/%.cu $(wildcard ape_b200/csrc/*.cuh) include/ape_b200.h
 	$(NVCC) $(NVCCFLAGS) -Xptxas -v -c $< -o $@ 2> build/$*.ptxas.log || (cat build/$*.ptxas.log; false)
 
 $(LIB): $(OBJS)
-	$(NVCC) -gencode arch=compute_100a,code=sm_100a -shared -o $@ $(OBJS)
+	$(NVCC) -gencode arch=compute_90a,code=sm_90a -shared -o $@ $(OBJS)
 
 oracle:
 	$(MAKE) -C oracle

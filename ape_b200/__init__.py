@@ -1,4 +1,4 @@
-"""ape_b200 — B200 (sm_100a) kernels and host modules for APE's detection forward pass.
+"""ape_b200 — H100 (sm_90a) kernels and host modules for APE's detection forward pass.
 
 Importing the package loads libape_b200.so (raises if it is not built: there is no CPU or
 PyTorch fallback) and registers the reference's operator names under `torch.ops.ape`."""

@@ -1,571 +1,16 @@
 // attn_fwd.cu — softmax attention core of the EVA-02 ViT blocks (Attention.forward, ape/modeling/backbone/
 // vit_eva_clip.py:218-319: q·k^T·scale -> softmax -> ·v, 16 heads x 64, window (N=1024) and global (N=4096) blocks)
-// on the 5th-gen tensor cores: flash-attention forward with tcgen05.mma, S and P·V accumulators in tensor memory,
-// Q/K/V tiles staged by TMA straight out of the fused [M, 3C] qkv buffer the qkv GEMM wrote (no head split copies).
-//
-// One CTA = 128 queries of one (sequence, head); it walks the keys in blocks of 64.  Roles (192 threads):
-//   warp 0      TMA producer : Q once, then K_j and V_j (64 x 64 each, 128-byte swizzle), each in its own single buffer
-//   warp 1      MMA issuer   : S_j = Q K_j^T (4 x tcgen05.mma 128x64x16, K-major operands) into TMEM columns 0..63;
-//                              O += P_j V_j (4 x tcgen05.mma 128x64x16, A = P from shared memory, B = V_j in its natural
-//                              [key][channel] layout = MN-major operand) accumulating in TMEM columns 64..127
-//   warps 2..5  softmax      : thread = query row (TMEM lane): tcgen05.ld S_j, exponentials in the exp2 domain relative
-//                              to a per-row reference maximum, P_j -> 16 bit -> 128B-swizzled shared memory.
-// O stays in tensor memory for the whole key loop.  The reference maximum is only moved when a row's maximum grows
-// by more than 2^8 (then the warp rescales its 32 rows of O in place with tcgen05.ld / tcgen05.st): P <= 256 fits the
-// 16-bit formats, and the common iteration touches S only.  That keeps the softmax threads under 85 registers, so
-// FOUR CTAs share an SM (49 KB shared memory, 128 TMEM columns each; the 512 CTAs of a ViT layer are one wave): while one CTA's rows are in the exponential
-// unit, the others' MMAs and loads proceed.  S_{j+1} is issued as soon as S_j has been read into registers.
-// Bound: for head dim 64 the 16 ex2/clk/SM of the SFU cap attention near half of the tensor peak (4 x 64 flops per
-// exponential); see DESIGN.md.
+// and of the EVA02-CLIP text tower (causal, 77-token prompts packed at a row stride): flash-attention forward with wgmma
+// (attn.cuh), Q/K/V tiles staged by TMA straight out of the fused [M, 3C] qkv buffer the qkv GEMM wrote (no head split
+// copies).  One CTA = 128 queries (two consumer warpgroups) of one (sequence, head).
 #include <stdlib.h>
-#include <type_traits>
 
-#include "common.cuh"
-#include "tc.cuh"
+#include "attn.cuh"
 
 namespace ape {
 namespace {
-
-constexpr int QM = 128, KN = 64, HD = 64;
-constexpr int kAttnThreads = 192;
-constexpr float kRescaleThreshold = 8.f;  // log2 units
-constexpr int kDefaultAttnVariant = 0;
-
-struct alignas(1024) AttnSmem {
-  uint8_t q[QM * HD * 2];   // 16 KB
-  uint8_t k[KN * HD * 2];   // 8 KB   (K and V are single buffers with their own barriers: K_{j+1} is fetched while
-  uint8_t v[KN * HD * 2];   // 8 KB    the softmax of block j runs, V_{j+1} while S_{j+1} is computed)
-  uint8_t p[QM * KN * 2];   // 16 KB
-  uint64_t q_full, k_full, k_empty, v_full, v_empty;
-  uint64_t s_full, s_empty, p_full, pv_done;
-  uint32_t tmem_base;
-};
-
-struct AttnParams {
-  void *out;
-  long long ldo;     // elements
-  int n;             // tokens per sequence (multiple of 128)
-  int n_valid;       // keys >= n_valid of every sequence are masked out (rows padded up to n; n_valid <= n)
-  int seq_stride;    // rows between the starts of consecutive sequences (n unless sequences are packed tighter than the tile)
-  int causal;        // key t attends only to keys <= t (text tower, eva02_clip/transformer.py:714-720)
-  int heads, C;      // C = heads * 64
-  float *stats_out;  // [rows, heads, 2] (sum, sum of squares) of each row's 64 stored output values per head, or nullptr
-  float scale_log2;  // softmax scale * log2(e)
-  uint32_t idesc_qk, idesc_pv;
-};
-
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// Packed fp32 pairs (sm_100: fma / add .f32x2 process two lanes of a 64-bit register pair per instruction).  ncu's source view of
-// the softmax loop (profiles/r02_attn_global_ncu_raw.csv): 411 instructions per warp and key block, 64 of them the scale FFMAs
-// and 64 the row-sum FADDs, with the exponential unit and the issue slots saturating together at ~53 % — halving those two
-// groups takes 15 % of the instructions out of the loop.
-__device__ __forceinline__ uint64_t pk2(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void up2(uint64_t v, float &a, float &b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ void sts_v4(uint32_t addr, const uint4 &v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kAttnThreads, 4)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  AttnSmem &s = *reinterpret_cast<AttnSmem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qblk = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
-  const int row0 = seq * p.seq_stride;   // first token row of this sequence in the qkv buffer
-  // key blocks that hold at least one key some row of this tile attends to
-  const int nkv = ((p.causal ? min(p.n_valid, (qblk + 1) * QM) : p.n_valid) + KN - 1) / KN;
-  constexpr uint32_t TMEM_COLS = 128;    // S (64 fp32 columns) | O (64)
-
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tensormap(&map_qkv);
-    tc::mbar_init(&s.q_full, 1);
-    tc::mbar_init(&s.k_full, 1);
-    tc::mbar_init(&s.k_empty, 1);
-    tc::mbar_init(&s.v_full, 1);
-    tc::mbar_init(&s.v_empty, 1);
-    tc::mbar_init(&s.s_full, 1);
-    tc::mbar_init(&s.s_empty, 4);   // one arrival per softmax warp
-    tc::mbar_init(&s.p_full, 4);
-    tc::mbar_init(&s.pv_done, 1);
-    tc::fence_mbar_init();
-  }
-  if (warp == 1) {
-    tc::tmem_alloc(&s.tmem_base, TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = s.tmem_base;
-  pdl_wait();  // barriers and tensor memory are set up; the previous kernel's output (qkv) may be read from here on
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      tc::mbar_expect_tx(&s.q_full, QM * HD * 2);
-      tc::tma_load_2d(s.q, &map_qkv, &s.q_full, head * HD, row0 + qblk * QM);                       // the box is 64 rows:
-      tc::tma_load_2d(s.q + KN * HD * 2, &map_qkv, &s.q_full, head * HD, row0 + qblk * QM + KN);    // two boxes per Q tile
-      for (int j = 0; j < nkv; ++j) {
-        tc::mbar_wait(&s.k_empty, (j & 1) ^ 1);  // S_{j-1} has been computed
-        tc::mbar_expect_tx(&s.k_full, KN * HD * 2);
-        tc::tma_load_2d(s.k, &map_qkv, &s.k_full, p.C + head * HD, row0 + j * KN);
-        tc::mbar_wait(&s.v_empty, (j & 1) ^ 1);  // O += P_{j-1} V_{j-1} has completed
-        tc::mbar_expect_tx(&s.v_full, KN * HD * 2);
-        tc::tma_load_2d(s.v, &map_qkv, &s.v_full, 2 * p.C + head * HD, row0 + j * KN);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      tc::mbar_wait(&s.q_full, 0);
-      tc::fence_after_sync();
-      const uint64_t dq = tc::make_smem_desc_sw128(tc::smem_u32(s.q));
-      const uint64_t dk = tc::make_smem_desc_sw128(tc::smem_u32(s.k));
-      const uint64_t dv = tc::make_smem_desc_sw128(tc::smem_u32(s.v));
-      const uint64_t dp = tc::make_smem_desc_sw128(tc::smem_u32(s.p));
-      auto issue_qk = [&](int j) {
-        tc::mbar_wait(&s.k_full, j & 1);
-        tc::fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < HD / 16; ++k) tc::mma_f16(tmem, dq + 2 * k, dk + 2 * k, p.idesc_qk, k != 0);
-        tc::mma_commit(&s.s_full);
-        tc::mma_commit(&s.k_empty);  // K_j may be replaced by K_{j+1}
-      };
-      issue_qk(0);
-      for (int j = 0; j < nkv; ++j) {
-        if (j + 1 < nkv) {  // S_{j+1} as soon as the softmax warps hold S_j in registers
-          tc::mbar_wait(&s.s_empty, j & 1);
-          issue_qk(j + 1);
-        }
-        tc::mbar_wait(&s.v_full, j & 1);
-        tc::mbar_wait(&s.p_full, j & 1);  // P_j is in shared memory (and O was rescaled if it had to be)
-        tc::fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < KN / 16; ++k)  // A: +32 B per 16 keys inside the swizzle row; B (MN-major): +16 key rows = 2 KB
-          tc::mma_f16(tmem + 64, dp + 2 * k, dv + 128 * k, p.idesc_pv, (j | k) != 0);
-        tc::mma_commit(&s.pv_done);
-        tc::mma_commit(&s.v_empty);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== softmax (warps 2..5; thread = query row) =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16);
-    float m_ref = -INFINITY, l = 0.f;
-    const uint32_t prow = tc::smem_u32(s.p) + row * 128;
-    const uint64_t sc2 = pk2(p.scale_log2, p.scale_log2);
-    // Per key block the scores are read from tensor memory ONCE: exponentials are formed against the reference maximum
-    // carried over from the previous blocks while the block's own maximum is tracked on the side; only when some row of
-    // the warp outgrows the reference by more than 2^8 (P would leave the 16-bit range) is the block redone against the new
-    // reference (and O rescaled) — rare after the first block, which takes its reference from its own scores up front.
-    auto load_half = [&](int hh, int kvalid, uint32_t *r) {
-      tc::tmem_ld_32x32b_x32(trow + 32 * hh, r);
-      tc::tmem_ld_wait();
-      if (kvalid < KN) {  // padded / future keys score -inf: ex2(-inf) = 0
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (32 * hh + i >= kvalid) r[i] = 0xff800000u;
-      }
-    };
-    auto exp_half = [&](int hh, const uint32_t *r, uint64_t *s4) {  // s4: four packed pairs of partial row sums
-      const uint64_t nm2 = pk2(-m_ref, -m_ref);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float e[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint64_t x2 = fma2(pk2(__uint_as_float(r[8 * c + 2 * i]), __uint_as_float(r[8 * c + 2 * i + 1])), sc2, nm2);
-          float x0, x1;
-          up2(x2, x0, x1);
-          e[2 * i] = ex2(x0);
-          e[2 * i + 1] = ex2(x1);
-          s4[i] = add2(s4[i], pk2(e[2 * i], e[2 * i + 1]));
-        }
-        sts_v4(prow + (((4 * hh + c) ^ (row & 7)) << 4), Elem<T>::pack(e));
-      }
-    };
-    auto release_s = [&]() {  // S_j is in registers: the tensor core may compute S_{j+1}
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.s_empty);
-    };
-    for (int j = 0; j < nkv; ++j) {
-      tc::mbar_wait(&s.s_full, j & 1);
-      tc::fence_after_sync();
-      // real keys of this block the row may attend to: padding beyond n_valid, and (causal) keys after the query's own position
-      const int kvalid = p.causal ? min(p.n_valid, qblk * QM + row + 1) - j * KN : p.n_valid - j * KN;
-      uint32_t r[32];
-      if (j == 0) {  // first block: the reference is this block's own row maximum (every row sees key 0)
-        float m = -INFINITY;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          load_half(hh, kvalid, r);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) m = fmaxf(m, __uint_as_float(r[i]));
-        }
-        m_ref = p.scale_log2 * m;
-      }
-      uint64_t s8[4];
-      float m4[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) s8[i] = 0ull;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) m4[i] = -INFINITY;
-      load_half(0, kvalid, r);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(r[i]));
-      if (j > 0) {  // before the first write of P_j: P_{j-1} has been consumed (and O holds blocks 0..j-1)
-        tc::mbar_wait(&s.pv_done, (j - 1) & 1);
-        tc::fence_after_sync();
-      }
-      exp_half(0, r, s8);
-      load_half(1, kvalid, r);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(r[i]));
-      const float mx = p.scale_log2 * fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-      const bool moved = __any_sync(0xffffffffu, mx > m_ref + kRescaleThreshold);
-      if (!moved) {
-        release_s();
-        exp_half(1, r, s8);
-      } else {  // warp-uniform, rare: new reference, rescale this warp's rows of O in place, redo the block's exponentials
-        const float m_new = fmaxf(m_ref, mx);
-        const float alpha = ex2(m_ref - m_new);
-        m_ref = m_new;
-        l *= alpha;
-        if (j > 0) {
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t o[32];
-            tc::tmem_ld_32x32b_x32(trow + 64 + 32 * hh, o);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tc::tmem_st_32x32b_x32(trow + 64 + 32 * hh, o);
-          }
-          tc::tmem_st_wait();
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) s8[i] = 0ull;
-        load_half(0, kvalid, r);
-        exp_half(0, r, s8);
-        load_half(1, kvalid, r);
-        release_s();
-        exp_half(1, r, s8);
-      }
-      {
-        float a0, a1, b0, b1;
-        up2(add2(s8[0], s8[1]), a0, a1);
-        up2(add2(s8[2], s8[3]), b0, b1);
-        l += (a0 + a1) + (b0 + b1);
-      }
-      tc::fence_proxy_async();  // P visible to the tensor core's (async proxy) reads
-      tc::fence_before_sync();  // ... and the O rescale ordered before the MMA that accumulates into it
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.p_full);
-    }
-    tc::mbar_wait(&s.pv_done, (nkv - 1) & 1);
-    tc::fence_after_sync();
-    const float inv = 1.f / l;
-    T *dst = reinterpret_cast<T *>(p.out) + (size_t)(row0 + qblk * QM + row) * p.ldo + head * HD;
-    float st_sum = 0.f, st_sq = 0.f;
-    // packed sequences (seq_stride < n): rows past the sequence belong to the next one and must not be written
-    const bool store_row = p.seq_stride >= p.n || qblk * QM + row < p.n_valid;
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      uint32_t o[32];
-      tc::tmem_ld_32x32b_x32(trow + 64 + 32 * hh, o);
-      tc::tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float f[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(o[8 * c + i]) * inv;
-        const uint4 pk = Elem<T>::pack(f);
-        if (store_row) *reinterpret_cast<uint4 *>(dst + 32 * hh + 8 * c) = pk;
-        if (p.stats_out != nullptr) {  // statistics of the values as stored, for the LayerNorm folded into the next GEMM
-          float g[8];
-          Elem<T>::unpack(pk, g);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { st_sum += g[i]; st_sq += g[i] * g[i]; }
-        }
-      }
-    }
-    if (p.stats_out != nullptr && store_row)
-      *reinterpret_cast<float2 *>(p.stats_out + ((size_t)(row0 + qblk * QM + row) * p.heads + head) * 2) = make_float2(st_sum, st_sq);
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem, TMEM_COLS);
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------------
-// attn_fwd5_kernel — second structure for the same op.  ncu on the kernel above shows neither the tensor pipe nor the
-// exponential unit saturated; the accounting of its SHARED-MEMORY traffic explains why: per key block a CTA moves 16 KB of
-// Q + 8 KB of K + 16 KB of P + 8 KB of V through the MMA operand path, writes 16 KB of P and receives 16 KB of K / V from TMA
-// = 80 KB; four resident CTAs per SM need 2 560 clocks of the 128 B/clk port per round of blocks, more than the 2 048 clocks
-// the exponentials take.  This variant takes P out of shared memory altogether:
-//   * P_j is written with tcgen05.st into TENSOR memory (16-bit pairs, lane = query row) and consumed by P.V as the A operand
-//     of tcgen05.mma (the `[a_tmem]` form); per block 48 KB cross the shared-memory port instead of 80;
-//   * 256 tensor-memory columns per CTA: S0 | S1 (double-buffered scores) | P0 | P1 | O — two CTAs per SM; S_{j+1} is computed
-//     while the softmax of block j runs, P.V of block j while the softmax of block j+1 runs: the softmax warps never wait for
-//     the tensor core in the steady state (only the rare O rescale needs the previous P.V to have landed);
-//   * with two CTAs per SM a softmax thread may hold its whole score row (64 fp32) in registers: exact row maximum first, then
-//     the exponentials — one tensor-memory read per block, no redo path;
-//   * K and V are double-buffered in shared memory (48 KB per CTA).
-struct alignas(1024) AttnSmem5 {
-  uint8_t q[QM * HD * 2];
-  uint8_t k[2][KN * HD * 2];
-  uint8_t v[2][KN * HD * 2];
-  uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
-  uint64_t s_full[2], s_empty[2], p_full[2], p_empty[2];
-  uint32_t tmem_base;
-};
-
-template <typename T>
-__global__ void __launch_bounds__(kAttnThreads, 2)
-attn_fwd5_kernel(const __grid_constant__ CUtensorMap map_qkv, const AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  AttnSmem5 &s = *reinterpret_cast<AttnSmem5 *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qblk = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
-  const int row0 = seq * p.seq_stride;
-  const int nkv = ((p.causal ? min(p.n_valid, (qblk + 1) * QM) : p.n_valid) + KN - 1) / KN;
-  constexpr uint32_t TMEM_COLS = 256;  // S0 [0,64) | S1 [64,128) | P0 [128,160) | P1 [160,192) | O [192,256)
-  constexpr uint32_t COL_P = 128, COL_O = 192;
-
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tensormap(&map_qkv);
-    tc::mbar_init(&s.q_full, 1);
-#pragma unroll
-    for (int b = 0; b < 2; ++b) {
-      tc::mbar_init(&s.k_full[b], 1);
-      tc::mbar_init(&s.k_empty[b], 1);
-      tc::mbar_init(&s.v_full[b], 1);
-      tc::mbar_init(&s.v_empty[b], 1);
-      tc::mbar_init(&s.s_full[b], 1);
-      tc::mbar_init(&s.s_empty[b], 4);  // one arrival per softmax warp
-      tc::mbar_init(&s.p_full[b], 4);
-      tc::mbar_init(&s.p_empty[b], 1);
-    }
-    tc::fence_mbar_init();
-  }
-  if (warp == 1) {
-    tc::tmem_alloc(&s.tmem_base, TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = s.tmem_base;
-  pdl_wait();
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      tc::mbar_expect_tx(&s.q_full, QM * HD * 2);
-      tc::tma_load_2d(s.q, &map_qkv, &s.q_full, head * HD, row0 + qblk * QM);
-      tc::tma_load_2d(s.q + KN * HD * 2, &map_qkv, &s.q_full, head * HD, row0 + qblk * QM + KN);
-      for (int j = 0; j < nkv; ++j) {
-        const int b = j & 1, n = j >> 1;
-        tc::mbar_wait(&s.k_empty[b], (n & 1) ^ 1);
-        tc::mbar_expect_tx(&s.k_full[b], KN * HD * 2);
-        tc::tma_load_2d(s.k[b], &map_qkv, &s.k_full[b], p.C + head * HD, row0 + j * KN);
-        tc::mbar_wait(&s.v_empty[b], (n & 1) ^ 1);
-        tc::mbar_expect_tx(&s.v_full[b], KN * HD * 2);
-        tc::tma_load_2d(s.v[b], &map_qkv, &s.v_full[b], 2 * p.C + head * HD, row0 + j * KN);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      tc::mbar_wait(&s.q_full, 0);
-      tc::fence_after_sync();
-      const uint64_t dq = tc::make_smem_desc_sw128(tc::smem_u32(s.q));
-      auto issue_qk = [&](int j) {  // S[j & 1] = Q K_j^T
-        const int b = j & 1, n = j >> 1;
-        tc::mbar_wait(&s.k_full[b], n & 1);
-        tc::mbar_wait(&s.s_empty[b], (n & 1) ^ 1);  // the softmax warps hold S_{j-2} in registers
-        tc::fence_after_sync();
-        const uint64_t dk = tc::make_smem_desc_sw128(tc::smem_u32(s.k[b]));
-#pragma unroll
-        for (int k = 0; k < HD / 16; ++k) tc::mma_f16(tmem + 64 * b, dq + 2 * k, dk + 2 * k, p.idesc_qk, k != 0);
-        tc::mma_commit(&s.s_full[b]);
-        tc::mma_commit(&s.k_empty[b]);
-      };
-      issue_qk(0);
-      for (int j = 0; j < nkv; ++j) {
-        const int b = j & 1, n = j >> 1;
-        if (j + 1 < nkv) issue_qk(j + 1);
-        tc::mbar_wait(&s.v_full[b], n & 1);
-        tc::mbar_wait(&s.p_full[b], n & 1);  // P_j is in tensor memory (and O was rescaled if it had to be)
-        tc::fence_after_sync();
-        const uint64_t dv = tc::make_smem_desc_sw128(tc::smem_u32(s.v[b]));
-#pragma unroll
-        for (int k = 0; k < KN / 16; ++k)  // A: 16 keys = 8 packed columns of P; B (MN-major): +16 key rows = 2 KB
-          tc::mma_f16_ts(tmem + COL_O, tmem + COL_P + 32 * b + 8 * k, dv + 128 * k, p.idesc_pv, (j | k) != 0);
-        tc::mma_commit(&s.p_empty[b]);  // P buffer b free again = O holds blocks 0..j
-        tc::mma_commit(&s.v_empty[b]);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== softmax (warps 2..5; thread = query row = tensor-memory lane) =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16);
-    float m_ref = -INFINITY, l = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const int b = j & 1, n = j >> 1;
-      tc::mbar_wait(&s.s_full[b], n & 1);
-      tc::fence_after_sync();
-      uint32_t r[64];
-      tc::tmem_ld_32x32b_x32(trow + 64 * b, r);
-      tc::tmem_ld_32x32b_x32(trow + 64 * b + 32, r + 32);
-      tc::tmem_ld_wait();
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.s_empty[b]);  // S_j is in registers: S_{j+2} may overwrite the buffer
-      const int kvalid = p.causal ? min(p.n_valid, qblk * QM + row + 1) - j * KN : p.n_valid - j * KN;
-      if (kvalid < KN) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (i >= kvalid) r[i] = 0xff800000u;
-      }
-      float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 64; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(r[i]));
-      const float mx = p.scale_log2 * fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-      const bool moved = __any_sync(0xffffffffu, mx > m_ref + kRescaleThreshold);
-      if (moved) {  // warp-uniform; always on the first block (m_ref = -inf), rare afterwards
-        const float m_new = fmaxf(m_ref, mx);
-        const float alpha = ex2(m_ref - m_new);
-        m_ref = m_new;
-        l *= alpha;
-        if (j > 0) {  // O must hold blocks 0..j-1 before it is rescaled in place
-          tc::mbar_wait(&s.p_empty[(j - 1) & 1], ((j - 1) >> 1) & 1);
-          tc::fence_after_sync();
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t o[32];
-            tc::tmem_ld_32x32b_x32(trow + COL_O + 32 * hh, o);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tc::tmem_st_32x32b_x32(trow + COL_O + 32 * hh, o);
-          }
-          tc::tmem_st_wait();
-        }
-      }
-      if (j >= 2) {  // P buffer b is free once P_{j-2}.V_{j-2} has completed (long ago in the steady state)
-        tc::mbar_wait(&s.p_empty[b], (n - 1) & 1);
-        tc::fence_after_sync();
-      }
-      uint32_t pk[32];
-      float s4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const float e0 = ex2(fmaf(__uint_as_float(r[2 * i]), p.scale_log2, -m_ref));
-        const float e1 = ex2(fmaf(__uint_as_float(r[2 * i + 1]), p.scale_log2, -m_ref));
-        s4[i & 1] += e0;
-        s4[2 + (i & 1)] += e1;
-        if constexpr (sizeof(T) == 2 && std::is_same<T, __half>::value) {
-          const __half2 h = __floats2half2_rn(e0, e1);
-          pk[i] = *reinterpret_cast<const uint32_t *>(&h);
-        } else {
-          const __nv_bfloat162 h = __floats2bfloat162_rn(e0, e1);
-          pk[i] = *reinterpret_cast<const uint32_t *>(&h);
-        }
-      }
-      l += (s4[0] + s4[1]) + (s4[2] + s4[3]);
-      tc::tmem_st_32x32b_x32(trow + COL_P + 32 * b, pk);  // P_j: keys 2i / 2i+1 in the halves of column i
-      tc::tmem_st_wait();
-      tc::fence_before_sync();  // P (and a rescaled O) ordered before the MMA that reads them
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.p_full[b]);
-    }
-    tc::mbar_wait(&s.p_empty[(nkv - 1) & 1], ((nkv - 1) >> 1) & 1);
-    tc::fence_after_sync();
-    const float inv = 1.f / l;
-    T *dst = reinterpret_cast<T *>(p.out) + (size_t)(row0 + qblk * QM + row) * p.ldo + head * HD;
-    float st_sum = 0.f, st_sq = 0.f;
-    const bool store_row = p.seq_stride >= p.n || qblk * QM + row < p.n_valid;
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      uint32_t o[32];
-      tc::tmem_ld_32x32b_x32(trow + COL_O + 32 * hh, o);
-      tc::tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float f[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(o[8 * c + i]) * inv;
-        const uint4 pk4 = Elem<T>::pack(f);
-        if (store_row) *reinterpret_cast<uint4 *>(dst + 32 * hh + 8 * c) = pk4;
-        if (p.stats_out != nullptr) {
-          float g[8];
-          Elem<T>::unpack(pk4, g);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { st_sum += g[i]; st_sq += g[i] * g[i]; }
-        }
-      }
-    }
-    if (p.stats_out != nullptr && store_row)
-      *reinterpret_cast<float2 *>(p.stats_out + ((size_t)(row0 + qblk * QM + row) * p.heads + head) * 2) = make_float2(st_sum, st_sq);
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem, TMEM_COLS);
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn attn_encoder() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
+constexpr int QM = 128, HD = 64;
+constexpr int kDefaultAttnVariant = 1;
 }  // namespace
 }  // namespace ape
 
@@ -575,9 +20,9 @@ extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t l
                                int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
                                void *stream);
 
-// Kernel structure used by ape_attn_fwd*: 0 = attn_fwd_kernel (P through shared memory, 4 CTAs / SM), 1 = attn_fwd5_kernel (P in
-// tensor memory, 2 CTAs / SM).  set >= 0 selects it for the process (tests / tuning); returns the value in force.  The initial
-// value comes from APE_ATTN_VARIANT or the built-in default.
+// Kernel structure used by ape_attn_fwd*: 0 = P written to shared memory and read from there by the P.V MMA, 1 = P kept in
+// registers as the MMA's A operand.  set >= 0 selects it for the process (tests / tuning); returns the value in force.  The
+// initial value comes from APE_ATTN_VARIANT or the built-in default.
 extern "C" int ape_attn_variant(int set) {
   static int current = [] {
     const char *e = getenv("APE_ATTN_VARIANT");
@@ -610,47 +55,20 @@ extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t l
   if (ld < 3 * C || ldo < C || (ld * 2) % 16 || (ldo * 2) % 16 || (reinterpret_cast<uintptr_t>(qkv) & 15) ||
       (reinterpret_cast<uintptr_t>(out) & 15))
     return fail(APE_ERR_INVALID_ARG, "attn: qkv [rows, >= 3*heads*64] / out [rows, >= heads*64] with 16-byte aligned rows");
-  EncodeTiledFn enc = attn_encoder();
-  if (!enc) return fail(APE_ERR_UNSUPPORTED, "attn: cuTensorMapEncodeTiled not available from the driver");
-  CUtensorMap map;
-  cuuint64_t dims[2] = {(cuuint64_t)(3 * C), (cuuint64_t)total_rows};  // rows past the buffer read as zeros (TMA)
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)HD, (cuuint32_t)KN};  // 64 channels x 64 rows; Q takes two boxes
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(&map, dtype == APE_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                   const_cast<void *>(qkv), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(APE_ERR_INVALID_ARG, "attn: cuTensorMapEncodeTiled failed (%d)", (int)r);
-  AttnParams p{};
-  p.out = out; p.ldo = ldo; p.n = n; p.n_valid = n_valid; p.heads = heads; p.C = C; p.stats_out = stats_out;
-  p.seq_stride = seq_stride; p.causal = causal ? 1 : 0;
+  CUtensorMap map;  // rows past the buffer read as zeros (TMA)
+  if (int rc = attn::make_map(&map, qkv, dtype, total_rows, 3 * C, ld)) return rc;
+  attn::Params p{};
+  p.out = out; p.ldo = ldo; p.heads = heads; p.stats_out = stats_out;
+  p.q_seq_rows = seq_stride; p.kv_seq_rows = seq_stride;
+  p.q_col0 = 0; p.k_col0 = C; p.v_col0 = 2 * C;
+  p.n_valid = n_valid; p.causal = causal ? 1 : 0;
+  p.q_store_rows = seq_stride >= n ? n : n_valid;
   p.scale_log2 = scale * 1.4426950408889634f;
-  const int fmt = dtype == APE_DTYPE_BF16 ? 1 : 0;
-  p.idesc_qk = tc::make_idesc_f16(QM, KN, fmt);
-  p.idesc_pv = tc::make_idesc_f16(QM, HD, fmt) | (1u << 16);  // B (= V, [key][channel]) is MN-major
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   dim3 grid((unsigned)(n / QM), (unsigned)heads, (unsigned)num_seq);
-  // kernel structure: 0 = P through shared memory, 4 CTAs / SM (attn_fwd_kernel); 1 = P in tensor memory, double-buffered
-  // S / P / K / V, 2 CTAs / SM (attn_fwd5_kernel).  APE_ATTN_VARIANT overrides the default (read once).
-  const int variant = ape_attn_variant(-1);
-#define APE_ATTN_LAUNCH(KERNEL, SMEM_T)                                                                            \
-  do {                                                                                                             \
-    const size_t smem = sizeof(SMEM_T) + 1024;                                                                     \
-    static bool set = false;                                                                                       \
-    if (!set) {                                                                                                    \
-      cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);        \
-      if (e != cudaSuccess) return fail((int)e, "attn: cudaFuncSetAttribute: %s", cudaGetErrorString(e));         \
-      set = true;                                                                                                  \
-    }                                                                                                              \
-    APE_LAUNCH((KERNEL), grid, kAttnThreads, smem, st, map, p);                                                    \
-  } while (0)
-  if (variant == 1) {
-    if (dtype == APE_DTYPE_F16) APE_ATTN_LAUNCH(attn_fwd5_kernel<__half>, AttnSmem5);
-    else APE_ATTN_LAUNCH(attn_fwd5_kernel<__nv_bfloat16>, AttnSmem5);
-  } else {
-    if (dtype == APE_DTYPE_F16) APE_ATTN_LAUNCH(attn_fwd_kernel<__half>, AttnSmem);
-    else APE_ATTN_LAUNCH(attn_fwd_kernel<__nv_bfloat16>, AttnSmem);
-  }
-#undef APE_ATTN_LAUNCH
-  return check_launch("attn_fwd_kernel");
+  const bool p_smem = ape_attn_variant(-1) == 0;
+  if (dtype == APE_DTYPE_F16)
+    return p_smem ? attn::launch<__half, 1, 2, true>(map, map, map, p, grid, st) : attn::launch<__half, 1, 2, false>(map, map, map, p, grid, st);
+  return p_smem ? attn::launch<__nv_bfloat16, 1, 2, true>(map, map, map, p, grid, st)
+                : attn::launch<__nv_bfloat16, 1, 2, false>(map, map, map, p, grid, st);
 }

@@ -1,10 +1,10 @@
-// attn_xfwd.cu — cross attention with wide heads on the tcgen05 tensor cores: the two softmax attentions of
-// VisionLanguageFusion for phrase / text prompts (BiMultiHeadAttention.forward, ape/layers/fuse_helper.py:67-166):
+// attn_xfwd.cu — cross attention with wide heads: the two softmax attentions of VisionLanguageFusion for phrase / text
+// prompts (BiMultiHeadAttention.forward, ape/layers/fuse_helper.py:67-166):
 //   vision  <- language :  out_v = softmax_t( q_s . k_t ) value_l     queries = S vision tokens, keys = N_t phrases
 //   language <- vision  :  out_l = softmax_s( k_t . q_s ) value_v     queries = N_t phrases,      keys = S vision tokens
 // 8 heads of 256 channels (embed_dim 2048), N_t up to 5 000, S up to 196 416 (BASELINE.json configs[3]); the reference
 // materialises the S x N_t score matrix per head in fp32 (31 GB at that size) and applies both softmaxes to it.  Here each
-// direction is one flash-attention pass: the scores never leave tensor / shared memory.
+// direction is one flash-attention pass (attn.cuh): the scores never leave registers.
 //
 // Equivalence with the reference's op sequence: it subtracts the GLOBAL maximum of the score matrix (a constant: both
 // softmaxes are invariant to it) and clamps scores and shifted scores to +-5e4 (fuse_helper.py:88-110).  A clamp only
@@ -12,311 +12,10 @@
 // either way; the results are identical unless a WHOLE row sits 5e4 below the global maximum, which LayerNormed inputs
 // (|q.k| is bounded by |q||k| of normalised vectors times the projection norms) cannot produce.
 //
-// Kernel shape: same warp roles and barrier protocol as attn_fwd.cu (TMA producer, single-thread MMA issuer, four softmax
-// warps = one TMEM lane quadrant each), generalised to
-//   * separate Q / K / V tensors (three tensor maps), different row counts for queries and keys, padded key rows masked;
-//   * head dim HD = 64 * NC: Q, K_j, V_j live in shared memory as NC swizzled 64-column chunks; S_j = sum_c Q_c K_j,c^T is
-//     4*NC accumulating MMAs into 64 TMEM columns; O (HD fp32 columns of TMEM) += P_j V_j,c is 4 MMAs per chunk.
-// HD = 256: 64 (S) + 256 (O) TMEM columns, 144 KB of shared memory, one CTA per SM.
-#include "common.cuh"
-#include "tc.cuh"
-
-namespace ape {
-namespace {
-
-constexpr int XQM = 128, XKN = 64;
-constexpr int kXThreads = 192;
-constexpr float kXRescale = 8.f;
-
-template <int NC>
-struct alignas(1024) XSmem {
-  uint8_t q[NC][XQM * 64 * 2];
-  uint8_t k[NC][XKN * 64 * 2];
-  uint8_t v[NC][XKN * 64 * 2];
-  uint8_t p[XQM * XKN * 2];
-  uint64_t q_full, k_full, k_empty, v_full, v_empty;
-  uint64_t s_full, s_empty, p_full, pv_done;
-  uint32_t tmem_base;
-};
-
-struct XParams {
-  void *out;
-  long long ldo;
-  int nq, nkv, n_valid;  // padded query rows (multiple of 128) / key rows (multiple of 64) per sequence, real keys
-  int heads;
-  float scale_log2;
-  uint32_t idesc_qk, idesc_pv;
-};
-
-__device__ __forceinline__ float xex2(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-template <typename T, int NC>
-__global__ void __launch_bounds__(kXThreads, 1)
-attn_xfwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                 const __grid_constant__ CUtensorMap map_v, const XParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  using Smem = XSmem<NC>;
-  Smem &s = *reinterpret_cast<Smem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int HD = 64 * NC;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qblk = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
-  const int qrow0 = seq * p.nq + qblk * XQM;
-  const int krow0 = seq * p.nkv;
-  const int nkv = (p.n_valid + XKN - 1) / XKN;
-  constexpr uint32_t TMEM_COLS = NC == 1 ? 128 : 512;  // S (64) + O (HD), power of two
-
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tensormap(&map_q);
-    tc::prefetch_tensormap(&map_k);
-    tc::prefetch_tensormap(&map_v);
-    tc::mbar_init(&s.q_full, 1);
-    tc::mbar_init(&s.k_full, 1);
-    tc::mbar_init(&s.k_empty, 1);
-    tc::mbar_init(&s.v_full, 1);
-    tc::mbar_init(&s.v_empty, 1);
-    tc::mbar_init(&s.s_full, 1);
-    tc::mbar_init(&s.s_empty, 4);
-    tc::mbar_init(&s.p_full, 4);
-    tc::mbar_init(&s.pv_done, 1);
-    tc::fence_mbar_init();
-  }
-  if (warp == 1) {
-    tc::tmem_alloc(&s.tmem_base, TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = s.tmem_base;
-  pdl_wait();
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      tc::mbar_expect_tx(&s.q_full, NC * XQM * 64 * 2);
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        tc::tma_load_2d(s.q[c], &map_q, &s.q_full, head * HD + c * 64, qrow0);
-        tc::tma_load_2d(s.q[c] + XKN * 64 * 2, &map_q, &s.q_full, head * HD + c * 64, qrow0 + XKN);
-      }
-      for (int j = 0; j < nkv; ++j) {
-        tc::mbar_wait(&s.k_empty, (j & 1) ^ 1);
-        tc::mbar_expect_tx(&s.k_full, NC * XKN * 64 * 2);
-#pragma unroll
-        for (int c = 0; c < NC; ++c) tc::tma_load_2d(s.k[c], &map_k, &s.k_full, head * HD + c * 64, krow0 + j * XKN);
-        tc::mbar_wait(&s.v_empty, (j & 1) ^ 1);
-        tc::mbar_expect_tx(&s.v_full, NC * XKN * 64 * 2);
-#pragma unroll
-        for (int c = 0; c < NC; ++c) tc::tma_load_2d(s.v[c], &map_v, &s.v_full, head * HD + c * 64, krow0 + j * XKN);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      tc::mbar_wait(&s.q_full, 0);
-      tc::fence_after_sync();
-      const uint64_t dp = tc::make_smem_desc_sw128(tc::smem_u32(s.p));
-      auto issue_qk = [&](int j) {
-        tc::mbar_wait(&s.k_full, j & 1);
-        tc::fence_after_sync();
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const uint64_t dq = tc::make_smem_desc_sw128(tc::smem_u32(s.q[c]));
-          const uint64_t dk = tc::make_smem_desc_sw128(tc::smem_u32(s.k[c]));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::mma_f16(tmem, dq + 2 * k, dk + 2 * k, p.idesc_qk, (c | k) != 0);
-        }
-        tc::mma_commit(&s.s_full);
-        tc::mma_commit(&s.k_empty);
-      };
-      issue_qk(0);
-      for (int j = 0; j < nkv; ++j) {
-        if (j + 1 < nkv) {
-          tc::mbar_wait(&s.s_empty, j & 1);
-          issue_qk(j + 1);
-        }
-        tc::mbar_wait(&s.v_full, j & 1);
-        tc::mbar_wait(&s.p_full, j & 1);
-        tc::fence_after_sync();
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const uint64_t dv = tc::make_smem_desc_sw128(tc::smem_u32(s.v[c]));
-#pragma unroll
-          for (int k = 0; k < XKN / 16; ++k)
-            tc::mma_f16(tmem + 64 + 64 * c, dp + 2 * k, dv + 128 * k, p.idesc_pv, (j | k) != 0);
-        }
-        tc::mma_commit(&s.pv_done);
-        tc::mma_commit(&s.v_empty);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== softmax (warps 2..5; thread = query row) =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16);
-    float m_ref = -INFINITY, l = 0.f;
-    uint8_t *prow = s.p + row * 128;
-    for (int j = 0; j < nkv; ++j) {
-      tc::mbar_wait(&s.s_full, j & 1);
-      tc::fence_after_sync();
-      float m8[8];
-      const int kvalid = p.n_valid - j * XKN;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t r[32];
-        tc::tmem_ld_32x32b_x32(trow + 32 * hh, r);
-        tc::tmem_ld_wait();
-        if (kvalid < XKN) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * hh + i >= kvalid) r[i] = 0xff800000u;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float x = __uint_as_float(r[i]);
-          m8[i & 7] = (hh == 0 && i < 8) ? x : fmaxf(m8[i & 7], x);
-        }
-      }
-      const float mx = p.scale_log2 *
-          fmaxf(fmaxf(fmaxf(m8[0], m8[1]), fmaxf(m8[2], m8[3])), fmaxf(fmaxf(m8[4], m8[5]), fmaxf(m8[6], m8[7])));
-      const bool moved = __any_sync(0xffffffffu, mx > m_ref + kXRescale);
-      float alpha = 1.f;
-      if (moved) {
-        const float m_new = fmaxf(m_ref, mx);
-        alpha = xex2(m_ref - m_new);
-        m_ref = m_new;
-        l *= alpha;
-      }
-      if (j > 0) {
-        tc::mbar_wait(&s.pv_done, (j - 1) & 1);
-        tc::fence_after_sync();
-        if (moved) {
-#pragma unroll 1
-          for (int cc = 0; cc < 2 * NC; ++cc) {
-            uint32_t o[32];
-            tc::tmem_ld_32x32b_x32(trow + 64 + 32 * cc, o);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tc::tmem_st_32x32b_x32(trow + 64 + 32 * cc, o);
-          }
-          tc::tmem_st_wait();
-        }
-      }
-      float s8[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s8[i] = 0.f;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t r[32];
-        tc::tmem_ld_32x32b_x32(trow + 32 * hh, r);
-        tc::tmem_ld_wait();
-        if (hh == 1) {
-          tc::fence_before_sync();
-          __syncwarp();
-          if (lane == 0) tc::mbar_arrive(&s.s_empty);
-        }
-        if (kvalid < XKN) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * hh + i >= kvalid) r[i] = 0xff800000u;
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          float e[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            e[i] = xex2(fmaf(__uint_as_float(r[8 * c + i]), p.scale_log2, -m_ref));
-            s8[i] += e[i];
-          }
-          *reinterpret_cast<uint4 *>(prow + (((4 * hh + c) ^ (row & 7)) << 4)) = Elem<T>::pack(e);
-        }
-      }
-      l += ((s8[0] + s8[1]) + (s8[2] + s8[3])) + ((s8[4] + s8[5]) + (s8[6] + s8[7]));
-      tc::fence_proxy_async();
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.p_full);
-    }
-    tc::mbar_wait(&s.pv_done, (nkv - 1) & 1);
-    tc::fence_after_sync();
-    const float inv = 1.f / l;
-    T *dst = reinterpret_cast<T *>(p.out) + (size_t)(qrow0 + row) * p.ldo + head * HD;
-#pragma unroll 1
-    for (int cc = 0; cc < 2 * NC; ++cc) {
-      uint32_t o[32];
-      tc::tmem_ld_32x32b_x32(trow + 64 + 32 * cc, o);
-      tc::tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float f[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(o[8 * c + i]) * inv;
-        *reinterpret_cast<uint4 *>(dst + 32 * cc + 8 * c) = Elem<T>::pack(f);
-      }
-    }
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem, TMEM_COLS);
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn x_encoder() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-int x_map(CUtensorMap *map, const void *base, int dtype, long long rows, long long cols, long long ld) {
-  EncodeTiledFn enc = x_encoder();
-  if (!enc) return fail(APE_ERR_UNSUPPORTED, "attn_x: cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, 64};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, dtype == APE_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                   const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(APE_ERR_INVALID_ARG, "attn_x: cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return APE_OK;
-}
-
-template <typename T, int NC>
-int launch_x(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const XParams &p, dim3 grid, cudaStream_t st) {
-  const size_t smem = sizeof(XSmem<NC>) + 1024;
-  auto k = attn_xfwd_kernel<T, NC>;
-  static bool set = false;
-  if (!set) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail((int)e, "attn_x: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
-    set = true;
-  }
-  APE_LAUNCH(k, grid, kXThreads, smem, st, mq, mk, mv, p);
-  return check_launch("attn_xfwd_kernel");
-}
-
-}  // namespace
-}  // namespace ape
+// Separate Q / K / V tensors (three tensor maps), different row counts for queries and keys, padded key rows masked.
+// HD = 64: 128 queries per CTA (two consumer warpgroups).  HD = 256: the O accumulator is 128 fp32 registers per thread,
+// so a CTA is one consumer warpgroup of 64 queries (160 KB of shared memory for Q and double-buffered K / V).
+#include "attn.cuh"
 
 using namespace ape;
 
@@ -325,7 +24,7 @@ extern "C" int ape_attn_cross_fwd(const void *q, int64_t ldq, const void *k, int
                                   int dtype, void *stream) {
   if (dtype != APE_DTYPE_F16 && dtype != APE_DTYPE_BF16) return fail(APE_ERR_INVALID_ARG, "attn_x: fp16 / bf16 only (dtype %d)", dtype);
   if (head_dim != 64 && head_dim != 256) return fail(APE_ERR_UNSUPPORTED, "attn_x: head_dim %d (64 or 256)", head_dim);
-  if (num_seq < 0 || nq <= 0 || nq % XQM || nkv <= 0 || nkv % XKN || n_valid <= 0 || n_valid > nkv || heads <= 0 || heads > 65535 ||
+  if (num_seq < 0 || nq <= 0 || nq % 128 || nkv <= 0 || nkv % 64 || n_valid <= 0 || n_valid > nkv || heads <= 0 || heads > 65535 ||
       num_seq > 65535)
     return fail(APE_ERR_UNSUPPORTED, "attn_x: num_seq=%d nq=%d nkv=%d n_valid=%d heads=%d (nq %% 128 == 0, nkv %% 64 == 0)", num_seq, nq,
                 nkv, n_valid, heads);
@@ -336,21 +35,21 @@ extern "C" int ape_attn_cross_fwd(const void *q, int64_t ldq, const void *k, int
       ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out)) & 15))
     return fail(APE_ERR_INVALID_ARG, "attn_x: operands [rows, >= heads*head_dim] with 16-byte aligned rows");
   CUtensorMap mq, mk, mv;
-  if (int rc = x_map(&mq, q, dtype, (long long)num_seq * nq, C, ldq)) return rc;
-  if (int rc = x_map(&mk, k, dtype, (long long)num_seq * nkv, C, ldk)) return rc;
-  if (int rc = x_map(&mv, v, dtype, (long long)num_seq * nkv, C, ldv)) return rc;
-  XParams p{};
-  p.out = out; p.ldo = ldo; p.nq = nq; p.nkv = nkv; p.n_valid = n_valid; p.heads = heads;
+  if (int rc = attn::make_map(&mq, q, dtype, (long long)num_seq * nq, C, ldq)) return rc;
+  if (int rc = attn::make_map(&mk, k, dtype, (long long)num_seq * nkv, C, ldk)) return rc;
+  if (int rc = attn::make_map(&mv, v, dtype, (long long)num_seq * nkv, C, ldv)) return rc;
+  attn::Params p{};
+  p.out = out; p.ldo = ldo; p.heads = heads;
+  p.q_seq_rows = nq; p.kv_seq_rows = nkv;
+  p.n_valid = n_valid; p.q_store_rows = nq;
   p.scale_log2 = scale * 1.4426950408889634f;
-  const int fmt = dtype == APE_DTYPE_BF16 ? 1 : 0;
-  p.idesc_qk = tc::make_idesc_f16(XQM, XKN, fmt);
-  p.idesc_pv = tc::make_idesc_f16(XQM, 64, fmt) | (1u << 16);  // B (= V chunk, [key][channel]) is MN-major
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  dim3 grid((unsigned)(nq / XQM), (unsigned)heads, (unsigned)num_seq);
   if (head_dim == 64) {
-    if (dtype == APE_DTYPE_F16) return launch_x<__half, 1>(mq, mk, mv, p, grid, st);
-    return launch_x<__nv_bfloat16, 1>(mq, mk, mv, p, grid, st);
+    const dim3 grid((unsigned)(nq / 128), (unsigned)heads, (unsigned)num_seq);
+    if (dtype == APE_DTYPE_F16) return attn::launch<__half, 1, 2, false>(mq, mk, mv, p, grid, st);
+    return attn::launch<__nv_bfloat16, 1, 2, false>(mq, mk, mv, p, grid, st);
   }
-  if (dtype == APE_DTYPE_F16) return launch_x<__half, 4>(mq, mk, mv, p, grid, st);
-  return launch_x<__nv_bfloat16, 4>(mq, mk, mv, p, grid, st);
+  const dim3 grid((unsigned)(nq / 64), (unsigned)heads, (unsigned)num_seq);
+  if (dtype == APE_DTYPE_F16) return attn::launch<__half, 4, 1, false>(mq, mk, mv, p, grid, st);
+  return attn::launch<__nv_bfloat16, 4, 1, false>(mq, mk, mv, p, grid, st);
 }

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libape_b200.so (sm_100a only).
+// common.cuh — shared helpers for libape_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -10,8 +10,8 @@
 
 #include "ape_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libape_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libape_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace ape {
@@ -42,7 +42,7 @@ inline int dtype_size(int dtype) { return dtype == APE_DTYPE_F32 ? 4 : 2; }
 // launched (its CTAs start as SM resources free up and run their own set-up), then waits until the PREVIOUS kernel has
 // completed and flushed its writes — before this kernel reads or writes any global memory.  Launches go through APE_LAUNCH,
 // which sets cudaLaunchAttributeProgrammaticStreamSerialization; between two kernels of the library the launch latency and
-// the prologue (barrier / tensor-memory set-up of the tcgen05 kernels) then overlap the tail of the previous kernel, in
+// the prologue (barrier set-up of the TMA / wgmma kernels) then overlap the tail of the previous kernel, in
 // eager mode and inside captured CUDA graphs alike.  A predecessor that is not one of ours never triggers early, so the
 // dependency degrades to ordinary stream order.  APE_PDL=0 in the environment disables the attribute (A/B runs).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

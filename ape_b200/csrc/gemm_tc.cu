@@ -1,6 +1,6 @@
-// gemm_tc.cu — C[M,N] = A[M,K] · W[N,K]^T (+bias, activation, residual) on the 5th-gen tensor
-// cores of sm_100a: TMA-staged 128-byte-swizzled operand tiles, tcgen05.mma issued by one thread
-// with fp32 accumulators in TMEM, tcgen05.ld epilogue.  Hand-written (no CUTLASS/cuBLAS).
+// gemm_tc.cu — C[M,N] = A[M,K] · W[N,K]^T (+bias, activation, residual) on the Hopper (sm_90a) tensor cores:
+// TMA-staged 128-byte-swizzled operand tiles, wgmma issued by two consumer warpgroups with fp32 accumulators in
+// registers, epilogue straight from the accumulator fragments.  Hand-written (no CUTLASS/cuBLAS).
 //
 // This is the dense workhorse behind the reference's nn.Linear calls on the detection path:
 //   ViT q/k/v/proj and SwiGLU w1/w2/w3      ape/modeling/backbone/vit_eva_clip.py:225-232,266-267,125-132
@@ -9,14 +9,15 @@
 //   VisionLanguageAlign contraction            ape/layers/vision_language_align.py:36-48
 // `W` is consumed in nn.Linear's own [out_features, in_features] layout: both operands are K-major.
 //
-// Kernel shape (persistent, warp-specialised, 320 threads, 1 CTA / SM):
-//   warp 0     TMA producer   : STAGES-deep ring of {A 128x64, B BNx64} 16-bit tiles, mbarrier full/empty
-//   warp 1     MMA issuer     : 4 x tcgen05.mma (M=128, N=BN, K=16) per stage; owns the TMEM allocation
-//   warps 2-9  epilogue       : TMEM quadrant (warp_id % 4), column half ((warp_id-2)/4): tcgen05.ld ->
-//                               bias/act/residual in registers -> 16-bit pack -> 128B-swizzled smem slab
-//                               (32 rows x 64 cols) -> TMA store (coalesced, clips the M/N edges)
-//   TMEM holds two BN-column accumulators so tile i's epilogue overlaps tile i+1's main loop.
+// Kernel shape (persistent, warp-specialised, 288 threads, 1 CTA / SM):
+//   warps 0-7  consumers : warpgroup g owns rows 64g..64g+63 of the 128 x BN tile: 4 x wgmma m64nBNk16 per k-block,
+//                          one k-block in flight (the stage of the previous one is released when it has completed),
+//                          then bias / activation / residual / rotary / LayerNorm fold in registers and direct stores
+//   warp 8     producer  : STAGES-deep ring of {A 128x64, B BNx64} 16-bit tiles, mbarrier full/empty; it runs ahead
+//                          into the next tile's k-blocks while the consumers finish the epilogue of the current one
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc.cuh"
@@ -24,7 +25,9 @@
 namespace ape {
 namespace {
 
-constexpr int BM = 128, BK = 64, UMMA_K = 16;
+constexpr int BM = 128, BK = 64, WG_K = 16;
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * kConsumerWarps + 32;
 
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SWIGLU = 3, ACT_CLAMP = 4 };
 
@@ -39,13 +42,13 @@ struct GemmParams {
   int res_dtype;  // APE_DTYPE_* of `residual` (fp32-output GEMMs may add a 16-bit residual and vice versa)
   int act;
   int n_fastest;  // tile order: consecutive tiles walk the column blocks of one row group (A stays hot in L2)
+  int vec_out;    // C rows allow paired (2-element) stores
+  int vec_res;    // residual rows allow paired loads
   // optional 2-D rotary embedding on output columns [0, rope_cols) (q and k thirds of a fused qkv projection;
   // VisionRotaryEmbeddingFast, utils_eva02.py:248-252,346), applied after the bias in fp32: 64-channel heads
   const float *rope_cos, *rope_sin;  // [npos, 64]
   const int *rope_pos;               // [M] row -> position, or nullptr: row % rope_npos
   int rope_cols, rope_npos;
-  int tma_store;  // 16-bit output with 16-byte aligned rows: epilogue goes through smem + TMA store
-  uint32_t idesc;
   // LayerNorm folded around the GEMM (sub-LN of the EVA-02 block, vit_eva_clip.py:266,130: inner_attn_ln before proj, ffn_ln
   // before w3).  The producer of A (attention / SwiGLU epilogue) leaves per-row partial (sum, sum of squares) of the 16-bit
   // values it wrote; this GEMM runs on the RAW A with weights pre-scaled by gamma and finishes
@@ -59,10 +62,9 @@ struct GemmParams {
   float *stats_out;
   int stats_nslab;
   // implicit-GEMM 3x3 convolution (stride 1, zero padding 1) over an NHWC image: an m block is a conv_tw x conv_th pixel
-  // tile of one image, k block kb = (filter tap kb / conv_cblks, 64-channel block kb % conv_cblks); map_a / map_c are 4-D
-  int lean;      // lean whole-tile epilogue selected on the host (epilogue_dispatch), 0 = general code only
+  // tile of one image, k block kb = (filter tap kb / conv_cblks, 64-channel block kb % conv_cblks); map_a is 4-D
   int conv;  // 0 = plain GEMM
-  int conv_tw, conv_th, conv_tiles_x, conv_tiles_img, conv_cblks;
+  int conv_tw, conv_th, conv_tiles_x, conv_tiles_img, conv_cblks, conv_W, conv_H;
   // development aid (ape_gemm_set_trace): 8 clock64 stamps per CTA — 0 entry, 1 set-up done, 2 first operands landed,
   // 3 last MMA issued, 4 first accumulator complete, 5 last accumulator complete, 6 epilogue drained, 7 exit
   long long *trace;
@@ -76,666 +78,165 @@ template <int BN, int STAGES>
 struct alignas(1024) GemmSmem {
   uint8_t a[STAGES][BM * BK * 2];
   uint8_t b[STAGES][BN * BK * 2];
-  uint8_t c[8][32 * 128];  // per epilogue warp: 32 rows x 64 16-bit columns, 128-byte swizzle (1024 B aligned)
   uint64_t full[STAGES], empty[STAGES];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
 };
 
-constexpr int kThreads = 320;
-
-// Activation over N accumulator values; the switch is OUTSIDE the unrolled loops (one uniform branch per chunk, not per
-// element: with the branch inside, the three-way select around the inlined erff made the ReLU epilogue 4x slower).
-template <int N>
-__device__ __forceinline__ void apply_act(float *v, int act) {
-  if (act == ACT_RELU) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
-  } else if (act == ACT_GELU) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = 0.5f * v[i] * (1.f + erff(v[i] * 0.70710678118654752f));
-  } else if (act == ACT_CLAMP) {  // vision_language_align.py:49-51
-#pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = fminf(fmaxf(v[i], -50000.f), 50000.f);
-  }
+__device__ __forceinline__ float act1(float v, int act) {
+  if (act == ACT_RELU) return fmaxf(v, 0.f);
+  if (act == ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+  if (act == ACT_CLAMP) return fminf(fmaxf(v, -50000.f), 50000.f);  // vision_language_align.py:49-51
+  return v;
 }
 
-// 32 accumulator columns of one row += residual[m, n0 .. n0+31] read in its own dtype (fp32 or 16-bit).
-__device__ __forceinline__ void add_residual32(const GemmParams &p, float *v, int m, int n0) {
-  if (p.res_dtype == APE_DTYPE_F32) {
-    const float *res = reinterpret_cast<const float *>(p.residual) + (size_t)m * p.ldr + n0;
-    if (n0 + 32 <= p.N && (reinterpret_cast<uintptr_t>(res) & 15) == 0) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 f = __ldg(reinterpret_cast<const float4 *>(res) + i);
-        v[4 * i] += f.x; v[4 * i + 1] += f.y; v[4 * i + 2] += f.z; v[4 * i + 3] += f.w;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (n0 + i < p.N) v[i] += __ldg(res + i);
-    }
-  } else {
-    const uint16_t *res = reinterpret_cast<const uint16_t *>(p.residual) + (size_t)m * p.ldr + n0;
-    const bool half = p.res_dtype == APE_DTYPE_F16;
-    if (n0 + 32 <= p.N && (reinterpret_cast<uintptr_t>(res) & 15) == 0) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float f[8];
-        const uint4 u = __ldg(reinterpret_cast<const uint4 *>(res) + i);
-        if (half) Elem<__half>::unpack(u, f); else Elem<__nv_bfloat16>::unpack(u, f);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[8 * i + k] += f[k];
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (n0 + i < p.N) {
-          const uint16_t u = __ldg(res + i);
-          v[i] += half ? __half2float(__ushort_as_half(u)) : __uint_as_float((uint32_t)u << 16);
-        }
-    }
-  }
+__device__ __forceinline__ float ld16(const uint16_t *p, bool half) {
+  const uint16_t u = __ldg(p);
+  return half ? __half2float(__ushort_as_half(u)) : __uint_as_float((uint32_t)u << 16);
+}
+
+// Element offset of output row m: the row itself, or for the convolution the NHWC pixel the tile row stands for.
+__device__ __forceinline__ size_t out_row_offset(const GemmParams &p, int m) {
+  if (!p.conv) return (size_t)m * p.ldc;
+  const int m_blk = m / BM, r = m - m_blk * BM;
+  const int img = m_blk / p.conv_tiles_img, t = m_blk - img * p.conv_tiles_img;
+  const int ty = t / p.conv_tiles_x, tx = t - ty * p.conv_tiles_x;
+  const int x = tx * p.conv_tw + r % p.conv_tw, y = ty * p.conv_th + r / p.conv_tw;
+  return (((size_t)img * p.conv_H + y) * p.conv_W + x) * p.ldc;
 }
 
 template <typename TO>
-__device__ __forceinline__ void store_row(TO *dst, const float *v, int n) {  // n <= 32 contiguous outputs
-  if (n == 32 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+__device__ __forceinline__ void store_pair(TO *dst, float v0, float v1, bool ok1, bool vec) {
+  if (vec && ok1) {
     if constexpr (sizeof(TO) == 4) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        reinterpret_cast<uint4 *>(dst)[i] = make_uint4(__float_as_uint(v[4 * i]), __float_as_uint(v[4 * i + 1]),
-                                                       __float_as_uint(v[4 * i + 2]), __float_as_uint(v[4 * i + 3]));
+      *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);
+    } else if constexpr (std::is_same<TO, __half>::value) {
+      *reinterpret_cast<__half2 *>(dst) = __floats2half2_rn(v0, v1);
     } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) reinterpret_cast<uint4 *>(dst)[i] = Elem<TO>::pack(v + 8 * i);
+      *reinterpret_cast<__nv_bfloat162 *>(dst) = __floats2bfloat162_rn(v0, v1);
     }
   } else {
-    for (int i = 0; i < n; ++i) dst[i] = Elem<TO>::from_f(v[i]);
+    dst[0] = Elem<TO>::from_f(v0);
+    if (ok1) dst[1] = Elem<TO>::from_f(v1);
   }
 }
 
-template <typename TO>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams &p, const uint32_t *r, int m, int n0) {
-  // r: 32 fp32 accumulators of row m, columns n0..n0+31
-  float v[32];
-  const int nvalid = min(32, p.N - n0);
-  if (nvalid <= 0) return;
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-  if (p.bias != nullptr) {
-    if (nvalid == 32) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 b = __ldg(reinterpret_cast<const float4 *>(p.bias + n0) + i);
-        v[4 * i] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-      }
-    } else {
-      for (int i = 0; i < nvalid; ++i) v[i] += __ldg(p.bias + n0 + i);
-    }
-  }
-  TO *C = reinterpret_cast<TO *>(p.C);
-  if (p.act == ACT_SWIGLU) {
-    // interleaved (gate, up) column pairs -> silu(gate) * up, N/2 outputs (vit_eva_clip.py:126-128)
-    float o[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float g = v[2 * i];
-      o[i] = g / (1.f + __expf(-g)) * v[2 * i + 1];
-    }
-    TO *dst = C + (size_t)m * p.ldc + n0 / 2;
-    const int no = nvalid / 2;
-    if (no == 16 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0 && sizeof(TO) == 2) {
-      reinterpret_cast<uint4 *>(dst)[0] = Elem<TO>::pack(o);
-      reinterpret_cast<uint4 *>(dst)[1] = Elem<TO>::pack(o + 8);
-    } else {
-      for (int i = 0; i < no; ++i) dst[i] = Elem<TO>::from_f(o[i]);
-    }
-    return;
-  }
-  apply_act<32>(v, p.act);
-  if (p.residual != nullptr) add_residual32(p, v, m, n0);
-  store_row<TO>(C + (size_t)m * p.ldc + n0, v, nvalid);
-}
-
-
-// bias[n0 .. n0+31] added to 32 accumulator columns (columns >= N untouched).
-__device__ __forceinline__ void add_bias32(const GemmParams &p, float *v, int n0) {
-  if (p.bias == nullptr) return;
-  if (n0 + 32 <= p.N) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 b = __ldg(reinterpret_cast<const float4 *>(p.bias + n0) + i);
-      v[4 * i] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (n0 + i < p.N) v[i] += __ldg(p.bias + n0 + i);
-  }
-}
-
-// 2-D rotary embedding on 32 accumulator columns n0..n0+31 of row m (half of one 64-channel head of q or k).
-__device__ __forceinline__ void rope32(const GemmParams &p, float *v, int m, int n0) {
-  const int pos = p.rope_pos ? __ldg(p.rope_pos + m) : m % p.rope_npos;
-  const float4 *c4 = reinterpret_cast<const float4 *>(p.rope_cos + (size_t)pos * 64 + (n0 & 63));
-  const float4 *s4 = reinterpret_cast<const float4 *>(p.rope_sin + (size_t)pos * 64 + (n0 & 63));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 c = __ldg(c4 + i), sn = __ldg(s4 + i);
-    const float t0 = v[4 * i], t1 = v[4 * i + 1], t2 = v[4 * i + 2], t3 = v[4 * i + 3];
-    v[4 * i] = t0 * c.x - t1 * sn.x;       // rotate_half pairs (2i, 2i+1) -> (-t[2i+1], t[2i])
-    v[4 * i + 1] = t1 * c.y + t0 * sn.y;
-    v[4 * i + 2] = t2 * c.z - t3 * sn.z;
-    v[4 * i + 3] = t3 * c.w + t2 * sn.w;
-  }
-}
-
-// Epilogue of one warp for its (32 rows) x (BN/2 accumulator columns) part of a tile, 16-bit output, staged through a
-// swizzled shared-memory slab (32 rows x 64 output columns) and written with TMA stores.
-//
-// The accumulator is walked in pieces of 32 columns, ONE PIECE AHEAD: the tcgen05.ld of piece i+1 is in flight while piece i
-// is finished and written, so the tensor-memory read port (64 B/clk per SM: 2048 clocks for a 128x256 fp32 tile) streams
-// instead of alternating with the arithmetic.  Measured before this change (clock64 stamps, profiles/r02_gemm_phases.txt):
-// ~4400-4950 clocks per tile, which bounded every K = 256 GEMM of the encoder (mainloop floor 2048 clocks per tile).
+// Epilogue of one warpgroup for its 64 rows x BN columns of tile (m_blk, n_blk), from the wgmma accumulator fragment:
+// thread (warp w, lane l) holds rows r0 = 16 w + l/4 and r0 + 8, column pairs 8 j + 2 (l % 4) + {0, 1}.  Adjacent column
+// pairs are exactly what SwiGLU (interleaved gate / up) and the rotary embedding (rotate_half pairs) combine.
 template <typename TO, int BN>
-__device__ __forceinline__ void epilogue_tma(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab,
-                                             uint32_t tmem_tile, int quad, int half, int lane, int m_blk, int n_blk,
-                                             uint64_t *full_bar, uint32_t full_phase) {
-  const int row0 = m_blk * BM + quad * 32;
-  const int m = row0 + lane;
-  const uint32_t trow = tmem_tile + ((uint32_t)(quad * 32) << 16);
-  uint8_t *my_row = slab + lane * 128;
-  constexpr int HALF = BN / 2;
+__device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, int m_blk, int n_blk, int wg, int lane) {
+  const int warp4 = (threadIdx.x >> 5) & 3, tq = lane & 3;
+  const int c_base = n_blk * BN + 2 * tq;
   const bool swiglu = p.act == ACT_SWIGLU;
-  const int per_slab = swiglu ? 4 : 2;  // pieces (32 accumulator columns) per 64-column output slab
-  const int c_begin = half * HALF, c_end = c_begin + HALF;
-  tc::mbar_wait(full_bar, full_phase);
-  tc::fence_after_sync();
-  if (n_blk * BN + c_begin >= p.N) return;
-  uint32_t rn[32];
-  tc::tmem_ld_32x32b_x32(trow + c_begin, rn);
-  float st_sum = 0.f, st_sq = 0.f;
-  bool dirty = false;
-  int slab_c0 = c_begin;  // accumulator column (inside the tile) of the slab being filled
-#pragma unroll 1
-  for (int c = c_begin; c < c_end; c += 32) {
-    const int n0 = n_blk * BN + c;
-    if (n0 >= p.N) break;
-    const int q = ((c - c_begin) >> 5) % per_slab;
-    tc::tmem_ld_wait();
-    float v[32];
+  TO *C = reinterpret_cast<TO *>(p.C);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rn[i]);
-    if (c + 32 < c_end && n0 + 32 < p.N) tc::tmem_ld_32x32b_x32(trow + c + 32, rn);
-    add_bias32(p, v, n0);
-    if (q == 0) {
-      slab_c0 = c;
-      if (lane == 0) tc::tma_store_wait_read0();  // the previous store of this warp has drained the slab
-      __syncwarp();
-    }
-    if (swiglu) {
-      // interleaved (gate, up) column pairs -> silu(gate) * up: 16 outputs (vit_eva_clip.py:126-128)
-      float o[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float g = v[2 * i];
-        o[i] = g / (1.f + __expf(-g)) * v[2 * i + 1];
+  for (int h = 0; h < 2; ++h) {
+    const int m = m_blk * BM + wg * 64 + warp4 * 16 + (lane >> 2) + 8 * h;
+    const bool row_ok = m < p.M;
+    const int mr = row_ok ? m : p.M - 1;  // rows past M read a valid row and store nothing
+    float ln_rstd = 1.f, ln_shift = 0.f;  // ln_shift = rstd * mean
+    if (p.ln_part != nullptr) {  // row statistics from the producer's partials, summed in a fixed order
+      const float2 *pp = reinterpret_cast<const float2 *>(p.ln_part) + (size_t)mr * p.ln_nparts;
+      float sum = 0.f, sq = 0.f;
+      for (int i = 0; i < p.ln_nparts; ++i) {
+        const float2 t = __ldg(pp + i);
+        sum += t.x;
+        sq += t.y;
       }
+      const float mean = sum * p.ln_inv_c;
+      ln_rstd = rsqrtf(fmaxf(sq * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
+      ln_shift = ln_rstd * mean;
+    }
+    const float *rcos = nullptr, *rsin = nullptr;
+    if (p.rope_cos != nullptr) {
+      const int pos = p.rope_pos ? __ldg(p.rope_pos + mr) : mr % p.rope_npos;
+      rcos = p.rope_cos + (size_t)pos * 64;
+      rsin = p.rope_sin + (size_t)pos * 64;
+    }
+    TO *crow = C + out_row_offset(p, mr);
+    float st_sum = 0.f, st_sq = 0.f;
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const uint4 pk = Elem<TO>::pack(o + 8 * j);
-        *reinterpret_cast<uint4 *>(my_row + (((2 * q + j) ^ (lane & 7)) << 4)) = pk;
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = c_base + 8 * j;
+      const bool ok0 = n < p.N, ok1 = n + 1 < p.N;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (ok0) {
+        if (p.ln_part != nullptr) {  // rstd * acc - rstd * mean * colsum; the bias below is beta W^T + b
+          v0 = fmaf(ln_rstd, v0, -ln_shift * __ldg(p.ln_colsum + n));
+          if (ok1) v1 = fmaf(ln_rstd, v1, -ln_shift * __ldg(p.ln_colsum + n + 1));
+        }
+        if (p.bias != nullptr) {
+          v0 += __ldg(p.bias + n);
+          if (ok1) v1 += __ldg(p.bias + n + 1);
+        }
+      }
+      if (swiglu) {
+        // interleaved (gate, up) column pair -> silu(gate) * up, output column n / 2 (vit_eva_clip.py:126-128); N is even
+        const float o = v0 / (1.f + __expf(-v0)) * v1;
+        const TO ot = Elem<TO>::from_f(o);
+        if (ok0 && row_ok) crow[n / 2] = ot;
         if (p.stats_out != nullptr) {  // statistics of the values as stored (16-bit), columns beyond N/2 excluded
-          float f[8];
-          Elem<TO>::unpack(pk, f);
-          const int col0 = n0 / 2 + 8 * j;
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            if (col0 + i < p.N / 2) { st_sum += f[i]; st_sq += f[i] * f[i]; }
+          const float f = ok0 ? Elem<TO>::to_f(ot) : 0.f;
+          st_sum += f;
+          st_sq = fmaf(f, f, st_sq);
+          if ((j & 15) == 15) {  // 128 accumulator columns = one 64-column output slab complete
+            st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 1);
+            st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 1);
+            st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 2);
+            st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 2);
+            const int slab_idx = (n_blk * BN + 8 * (j - 15)) / 128;
+            if (tq == 0 && row_ok && slab_idx < p.stats_nslab)
+              *reinterpret_cast<float2 *>(p.stats_out + ((size_t)m * p.stats_nslab + slab_idx) * 2) = make_float2(st_sum, st_sq);
+            st_sum = 0.f;
+            st_sq = 0.f;
+          }
         }
+        continue;
       }
-    } else {
-      if (p.rope_cos != nullptr && n0 < p.rope_cols && m < p.M) rope32(p, v, m, n0);
-      apply_act<32>(v, p.act);
-      if (p.residual != nullptr && m < p.M) add_residual32(p, v, m, n0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4 *>(my_row + (((4 * q + j) ^ (lane & 7)) << 4)) = Elem<TO>::pack(v + 8 * j);
-    }
-    dirty = true;
-    if (q == per_slab - 1 || c + 32 >= c_end || n0 + 32 >= p.N) {  // slab complete (or last piece of this warp): store it
-      const int out_n0 = swiglu ? (n_blk * BN + slab_c0) / 2 : n_blk * BN + slab_c0;
-      if (swiglu && p.stats_out != nullptr && m < p.M) {
-        const int slab_idx = (n_blk * BN + slab_c0) / 128;
-        if (slab_idx < p.stats_nslab)
-          *reinterpret_cast<float2 *>(p.stats_out + ((size_t)m * p.stats_nslab + slab_idx) * 2) = make_float2(st_sum, st_sq);
-        st_sum = 0.f; st_sq = 0.f;
+      if (rcos != nullptr && n < p.rope_cols) {  // rotate_half pair (n, n+1) -> (-t[n+1], t[n])
+        const float2 c = __ldg(reinterpret_cast<const float2 *>(rcos + (n & 63)));
+        const float2 s = __ldg(reinterpret_cast<const float2 *>(rsin + (n & 63)));
+        const float t0 = v0, t1 = v1;
+        v0 = t0 * c.x - t1 * s.x;
+        v1 = t1 * c.y + t0 * s.y;
       }
-      tc::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (p.conv) {  // the slab's 32 tile rows are min(tw, 32) x 32 / min(tw, 32) pixels of the output image
-          const int img = m_blk / p.conv_tiles_img, t = m_blk - img * p.conv_tiles_img;
-          const int ty = t / p.conv_tiles_x, tx = t - ty * p.conv_tiles_x;
-          const int r0 = quad * 32;
-          tc::tma_store_4d(map_c, slab, out_n0, tx * p.conv_tw + r0 % p.conv_tw, ty * p.conv_th + r0 / p.conv_tw, img);
+      v0 = act1(v0, p.act);
+      v1 = act1(v1, p.act);
+      if (p.residual != nullptr && ok0) {
+        if (p.res_dtype == APE_DTYPE_F32) {
+          const float *res = reinterpret_cast<const float *>(p.residual) + (size_t)mr * p.ldr + n;
+          if (p.vec_res && ok1) {
+            const float2 r2 = __ldg(reinterpret_cast<const float2 *>(res));
+            v0 += r2.x;
+            v1 += r2.y;
+          } else {
+            v0 += __ldg(res);
+            if (ok1) v1 += __ldg(res + 1);
+          }
         } else {
-          tc::tma_store_2d(map_c, slab, out_n0, row0);
+          const uint16_t *res = reinterpret_cast<const uint16_t *>(p.residual) + (size_t)mr * p.ldr + n;
+          const bool half = p.res_dtype == APE_DTYPE_F16;
+          v0 += ld16(res, half);
+          if (ok1) v1 += ld16(res + 1, half);
         }
-        tc::tma_store_commit();
       }
-      dirty = false;
-    }
-  }
-  (void)dirty;
-}
-
-// fp32 output: the warp's (32 rows) x (BN/2 columns) part of a tile in pieces of 32 columns = one 128-byte-swizzled slab
-// (32 rows x 128 B) per TMA store.  Used for the residual stream (sum kept in fp32 between the 16-bit GEMMs) and for
-// logits that feed top-k / NMS.
-//
-// Everything this epilogue reads from global memory is requested BEFORE it is needed: the row statistics and the first
-// piece's residual before the accumulator is even complete, the residual of piece i+1 (and its tcgen05.ld) while piece i
-// is finished and stored.  Measured before (clock64 stamps): 25-28 k clocks for the one tile of a proj / w3 CTA against a
-// 10 k-clock mainloop — three dependent round trips (colsum, bias, residual) per piece behind the tensor-memory wait.
-template <int BN>
-__device__ __forceinline__ void epilogue_tma_f32(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab,
-                                                 uint32_t tmem_tile, int quad, int half, int lane, int m_blk, int n_blk,
-                                                 uint64_t *full_bar, uint32_t full_phase) {
-  const int row0 = m_blk * BM + quad * 32;
-  const int m = row0 + lane;
-  const uint32_t trow = tmem_tile + ((uint32_t)(quad * 32) << 16);
-  uint8_t *my_row = slab + lane * 128;
-  constexpr int HALF = BN / 2;
-  const int c_begin = half * HALF, c_end = c_begin + HALF;
-  // residual rows that may be fetched as aligned float4 ahead of time
-  const bool fast_res = p.residual != nullptr && p.res_dtype == APE_DTYPE_F32 && (p.ldr & 3) == 0 &&
-                        (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && m < p.M;
-  const float *res_row = reinterpret_cast<const float *>(p.residual) + (size_t)m * p.ldr;
-  float4 rs_next[8];
-  auto fetch_res = [&](int n0) {
-    if (fast_res && n0 + 32 <= p.N) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) rs_next[i] = __ldg(reinterpret_cast<const float4 *>(res_row + n0) + i);
-    }
-  };
-  const int n_first = n_blk * BN + c_begin;
-  if (n_first < p.N) fetch_res(n_first);
-  float ln_mean = 0.f, ln_rstd = 1.f;
-  if (p.ln_part != nullptr && m < p.M) {  // row statistics from the producer's partials, summed in a fixed order
-    const float2 *pp = reinterpret_cast<const float2 *>(p.ln_part) + (size_t)m * p.ln_nparts;
-    float sum = 0.f, sq = 0.f;
-    for (int i = 0; i < p.ln_nparts; ++i) {
-      const float2 t = __ldg(pp + i);
-      sum += t.x;
-      sq += t.y;
-    }
-    ln_mean = sum * p.ln_inv_c;
-    ln_rstd = rsqrtf(fmaxf(sq * p.ln_inv_c - ln_mean * ln_mean, 0.f) + p.ln_eps);
-  }
-  tc::mbar_wait(full_bar, full_phase);
-  tc::fence_after_sync();
-  if (n_first >= p.N) return;
-  uint32_t rn[32];
-  tc::tmem_ld_32x32b_x32(trow + c_begin, rn);
-#pragma unroll 1
-  for (int c = c_begin; c < c_end; c += 32) {
-    const int n0 = n_blk * BN + c;
-    if (n0 >= p.N) break;
-    tc::tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rn[i]);
-    float4 rs[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) rs[i] = rs_next[i];
-    if (c + 32 < c_end && n0 + 32 < p.N) {
-      tc::tmem_ld_32x32b_x32(trow + c + 32, rn);
-      fetch_res(n0 + 32);
-    }
-    if (p.ln_part != nullptr) {  // rstd * (acc - mean * colsum); the bias below is beta W^T + b
-      if (n0 + 32 <= p.N) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 cs = __ldg(reinterpret_cast<const float4 *>(p.ln_colsum + n0) + i);
-          v[4 * i] = ln_rstd * (v[4 * i] - ln_mean * cs.x);
-          v[4 * i + 1] = ln_rstd * (v[4 * i + 1] - ln_mean * cs.y);
-          v[4 * i + 2] = ln_rstd * (v[4 * i + 2] - ln_mean * cs.z);
-          v[4 * i + 3] = ln_rstd * (v[4 * i + 3] - ln_mean * cs.w);
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (n0 + i < p.N) v[i] = ln_rstd * (v[i] - ln_mean * __ldg(p.ln_colsum + n0 + i));
-      }
-    }
-    add_bias32(p, v, n0);
-    apply_act<32>(v, p.act);
-    if (fast_res && n0 + 32 <= p.N) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        v[4 * i] += rs[i].x; v[4 * i + 1] += rs[i].y; v[4 * i + 2] += rs[i].z; v[4 * i + 3] += rs[i].w;
-      }
-    } else if (p.residual != nullptr && m < p.M) {
-      add_residual32(p, v, m, n0);
-    }
-    if (lane == 0) tc::tma_store_wait_read0();
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<uint4 *>(my_row + ((j ^ (lane & 7)) << 4)) =
-          make_uint4(__float_as_uint(v[4 * j]), __float_as_uint(v[4 * j + 1]), __float_as_uint(v[4 * j + 2]),
-                     __float_as_uint(v[4 * j + 3]));
-    tc::fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-      tc::tma_store_2d(map_c, slab, n0, row0);
-      tc::tma_store_commit();
+      if (ok0 && row_ok) store_pair<TO>(crow + n, v0, v1, ok1, p.vec_out);
     }
   }
 }
 
-// ---- lean epilogues -------------------------------------------------------------------------------------------------
-// ncu on the K = 256 encoder GEMMs (profiles/r02_gemm_ffn1_ncu_source.txt): the general epilogues above execute ~270 SASS
-// instructions per piece of 32 columns where the arithmetic needs ~90 (address / predicate / branch code for ragged edges,
-// rotary embedding, residual dtypes and activation selection inside the piece loop, IEEE division in the SwiGLU gate), and with
-// two epilogue warps per scheduler the tile time follows the instruction count: ~8 k clocks per 128 x 256 tile against a
-// 2 k-clock main loop.  Every GEMM of the step was bounded by that (single CTA = multicast = CTA pair to within noise).
-// The functions below cover the whole-tile cases the model actually runs — everything decided at compile time, piece loop
-// fully unrolled, shared-memory stores through 32-bit shared addresses, the next piece's tensor-memory read and bias in
-// flight while the current one is finished — and fall back to the general code for ragged column blocks / other options.
-__device__ __forceinline__ void sts_v4(uint32_t addr, const uint4 &v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-// 16-bit output, bias (optional), ACT in {none, relu}: the warp's 32 rows x BN/2 columns = BN/128 slabs of 64 columns.
-template <typename TO, int ACT, bool HAS_BIAS, int BN>
-__device__ __forceinline__ void epi16_fast(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab, uint32_t tmem_tile,
-                                           int quad, int half, int lane, int m_blk, int n_blk, uint64_t *full_bar,
-                                           uint32_t full_phase) {
-  constexpr int HALF = BN / 2, PIECES = HALF / 32;
-  const int row0 = m_blk * BM + quad * 32;
-  const int n0 = n_blk * BN + half * HALF;
-  const uint32_t trow = tmem_tile + ((uint32_t)(quad * 32) << 16) + half * HALF;
-  const uint32_t my_row = tc::smem_u32(slab) + lane * 128;
-  const uint32_t sw = lane & 7;
-  const float4 *bias4 = reinterpret_cast<const float4 *>(p.bias + n0);
-  float4 bn[8];
-  if (HAS_BIAS) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) bn[i] = __ldg(bias4 + i);
-  }
-  tc::mbar_wait(full_bar, full_phase);
-  tc::fence_after_sync();
-  uint32_t rn[32];
-  tc::tmem_ld_32x32b_x32(trow, rn);
-#pragma unroll
-  for (int q = 0; q < PIECES; ++q) {
-    tc::tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rn[i]);
-    if (HAS_BIAS) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        v[4 * i] += bn[i].x; v[4 * i + 1] += bn[i].y; v[4 * i + 2] += bn[i].z; v[4 * i + 3] += bn[i].w;
-      }
-    }
-    if (q + 1 < PIECES) {
-      tc::tmem_ld_32x32b_x32(trow + 32 * (q + 1), rn);
-      if (HAS_BIAS) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) bn[i] = __ldg(bias4 + 8 * (q + 1) + i);
-      }
-    }
-    if (ACT == ACT_RELU) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-    }
-    if ((q & 1) == 0) {
-      if (lane == 0) tc::tma_store_wait_read0();  // the previous store of this warp has drained the slab
-      __syncwarp();
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) sts_v4(my_row + (((4 * (q & 1) + j) ^ sw) << 4), Elem<TO>::pack(v + 8 * j));
-    if (q & 1) {
-      tc::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (p.conv) {  // the slab's 32 tile rows are min(tw, 32) x 32 / min(tw, 32) pixels of the output image
-          const int img = m_blk / p.conv_tiles_img, t = m_blk - img * p.conv_tiles_img;
-          const int ty = t / p.conv_tiles_x, tx = t - ty * p.conv_tiles_x;
-          const int r0 = quad * 32;
-          tc::tma_store_4d(map_c, slab, n0 + 64 * (q >> 1), tx * p.conv_tw + r0 % p.conv_tw, ty * p.conv_th + r0 / p.conv_tw, img);
-        } else {
-          tc::tma_store_2d(map_c, slab, n0 + 64 * (q >> 1), row0);
-        }
-        tc::tma_store_commit();
-      }
-    }
-  }
-}
-
-// SwiGLU: interleaved (gate, up) accumulator columns -> silu(gate) * up, BN/4 output columns per warp (vit_eva_clip.py:126-128);
-// STATS: per-row (sum, sum of squares) of every 64-column output slab as stored (LayerNorm fold of the next GEMM).
-template <typename TO, bool STATS, int BN>
-__device__ __forceinline__ void epi16_swiglu_fast(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab, uint32_t tmem_tile,
-                                                  int quad, int half, int lane, int m_blk, int n_blk, uint64_t *full_bar,
-                                                  uint32_t full_phase) {
-  constexpr int HALF = BN / 2, PIECES = HALF / 32;  // 4 pieces of 32 accumulator columns = 16 outputs each -> one slab
-  static_assert(PIECES == 4, "SwiGLU epilogue: 256-wide tiles");
-  const int row0 = m_blk * BM + quad * 32;
-  const int m = row0 + lane;
-  const int n0 = n_blk * BN + half * HALF;
-  const uint32_t trow = tmem_tile + ((uint32_t)(quad * 32) << 16) + half * HALF;
-  const uint32_t my_row = tc::smem_u32(slab) + lane * 128;
-  const uint32_t sw = lane & 7;
-  const float4 *bias4 = reinterpret_cast<const float4 *>(p.bias + n0);
-  float4 bn[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) bn[i] = __ldg(bias4 + i);
-  tc::mbar_wait(full_bar, full_phase);
-  tc::fence_after_sync();
-  uint32_t rn[32];
-  tc::tmem_ld_32x32b_x32(trow, rn);
-  float st_sum = 0.f, st_sq = 0.f;
-  if (lane == 0) tc::tma_store_wait_read0();
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < PIECES; ++q) {
-    tc::tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rn[i]);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      v[4 * i] += bn[i].x; v[4 * i + 1] += bn[i].y; v[4 * i + 2] += bn[i].z; v[4 * i + 3] += bn[i].w;
-    }
-    if (q + 1 < PIECES) {
-      tc::tmem_ld_32x32b_x32(trow + 32 * (q + 1), rn);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) bn[i] = __ldg(bias4 + 8 * (q + 1) + i);
-    }
-    float o[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float g = v[2 * i];
-      o[i] = __fdividef(g, 1.f + __expf(-g)) * v[2 * i + 1];
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint4 pk = Elem<TO>::pack(o + 8 * j);
-      sts_v4(my_row + (((2 * q + j) ^ sw) << 4), pk);
-      if (STATS) {
-        float f[8];
-        Elem<TO>::unpack(pk, f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { st_sum += f[i]; st_sq = fmaf(f[i], f[i], st_sq); }
-      }
-    }
-  }
-  if (STATS && m < p.M) {
-    const int slab_idx = n0 / 128;
-    if (slab_idx < p.stats_nslab)
-      *reinterpret_cast<float2 *>(p.stats_out + ((size_t)m * p.stats_nslab + slab_idx) * 2) = make_float2(st_sum, st_sq);
-  }
-  tc::fence_proxy_async();
-  __syncwarp();
-  if (lane == 0) {
-    tc::tma_store_2d(map_c, slab, n0 / 2, row0);
-    tc::tma_store_commit();
-  }
-}
-
-// fp32 output (+ fp32 residual, + LayerNorm fold), no activation: pieces of 32 columns = one 128-byte-wide slab each.
-//   LN:  out = rstd * acc + (bias - rstd * mean * colsum) + residual        (two FMAs and one add per element)
-template <bool HAS_RES, bool LN, int BN>
-__device__ __forceinline__ void epi32_fast(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab, uint32_t tmem_tile,
-                                           int quad, int half, int lane, int m_blk, int n_blk, uint64_t *full_bar,
-                                           uint32_t full_phase) {
-  constexpr int HALF = BN / 2, PIECES = HALF / 32;
-  const int row0 = m_blk * BM + quad * 32;
-  const int m = min(row0 + lane, p.M - 1);  // rows past M: read a valid row, the TMA store clips them
-  const int n0 = n_blk * BN + half * HALF;
-  const uint32_t trow = tmem_tile + ((uint32_t)(quad * 32) << 16) + half * HALF;
-  const uint32_t my_row = tc::smem_u32(slab) + lane * 128;
-  const uint32_t sw = lane & 7;
-  const float4 *bias4 = reinterpret_cast<const float4 *>(p.bias + n0);
-  const float4 *cs4 = reinterpret_cast<const float4 *>(p.ln_colsum + n0);
-  const float4 *res4 = reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p.residual) + (size_t)m * p.ldr + n0);
-  float4 rs_next[8];
-  if (HAS_RES) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) rs_next[i] = __ldg(res4 + i);
-  }
-  float ln_rstd = 1.f, ln_shift = 0.f;  // ln_shift = rstd * mean
-  if (LN) {
-    const float2 *pp = reinterpret_cast<const float2 *>(p.ln_part) + (size_t)m * p.ln_nparts;
-    float sum = 0.f, sq = 0.f;
-    for (int i = 0; i < p.ln_nparts; ++i) {
-      const float2 t = __ldg(pp + i);
-      sum += t.x;
-      sq += t.y;
-    }
-    const float mean = sum * p.ln_inv_c;
-    ln_rstd = rsqrtf(fmaxf(sq * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
-    ln_shift = ln_rstd * mean;
-  }
-  tc::mbar_wait(full_bar, full_phase);
-  tc::fence_after_sync();
-  uint32_t rn[32];
-  tc::tmem_ld_32x32b_x32(trow, rn);
-#pragma unroll
-  for (int q = 0; q < PIECES; ++q) {
-    float4 t[8];  // per column: bias - rstd * mean * colsum (LN) or bias
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      t[i] = __ldg(bias4 + 8 * q + i);
-      if (LN) {
-        const float4 cs = __ldg(cs4 + 8 * q + i);
-        t[i].x = fmaf(-ln_shift, cs.x, t[i].x); t[i].y = fmaf(-ln_shift, cs.y, t[i].y);
-        t[i].z = fmaf(-ln_shift, cs.z, t[i].z); t[i].w = fmaf(-ln_shift, cs.w, t[i].w);
-      }
-    }
-    tc::tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rn[i]);
-    float4 rs[8];
-    if (HAS_RES) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) rs[i] = rs_next[i];
-    }
-    if (q + 1 < PIECES) {
-      tc::tmem_ld_32x32b_x32(trow + 32 * (q + 1), rn);
-      if (HAS_RES) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rs_next[i] = __ldg(res4 + 8 * (q + 1) + i);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      if (LN) {
-        v[4 * i] = fmaf(ln_rstd, v[4 * i], t[i].x); v[4 * i + 1] = fmaf(ln_rstd, v[4 * i + 1], t[i].y);
-        v[4 * i + 2] = fmaf(ln_rstd, v[4 * i + 2], t[i].z); v[4 * i + 3] = fmaf(ln_rstd, v[4 * i + 3], t[i].w);
-      } else {
-        v[4 * i] += t[i].x; v[4 * i + 1] += t[i].y; v[4 * i + 2] += t[i].z; v[4 * i + 3] += t[i].w;
-      }
-      if (HAS_RES) {
-        v[4 * i] += rs[i].x; v[4 * i + 1] += rs[i].y; v[4 * i + 2] += rs[i].z; v[4 * i + 3] += rs[i].w;
-      }
-    }
-    if (lane == 0) tc::tma_store_wait_read0();
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      sts_v4(my_row + ((j ^ sw) << 4), make_uint4(__float_as_uint(v[4 * j]), __float_as_uint(v[4 * j + 1]),
-                                                  __float_as_uint(v[4 * j + 2]), __float_as_uint(v[4 * j + 3])));
-    tc::fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-      tc::tma_store_2d(map_c, slab, n0 + 32 * q, row0);
-      tc::tma_store_commit();
-    }
-  }
-}
-
-// Epilogue of one warp for its part of tile (m_blk, n_blk) through shared memory + TMA stores: the lean whole-tile variants
-// where they apply (GemmParams::lean, decided on the host), the general code otherwise.
-template <int BN>
-__device__ __forceinline__ void epilogue_dispatch(const GemmParams &p, const CUtensorMap *map_c, uint8_t *slab, uint32_t tmem_tile,
-                                                  int quad, int half, int lane, int m_blk, int n_blk, uint64_t *full_bar,
-                                                  uint32_t full_phase) {
-  constexpr int HALF = BN / 2;
-#define APE_EPI_ARGS p, map_c, slab, tmem_tile, quad, half, lane, m_blk, n_blk, full_bar, full_phase
-  if (p.lean != 0 && n_blk * BN + (half + 1) * HALF <= p.N) {  // whole column range of this warp inside N
-    const bool f16 = p.out_dtype == APE_DTYPE_F16;
-    switch (p.lean) {
-      case 1:  // 16-bit, no activation
-        if (p.bias != nullptr) { if (f16) epi16_fast<__half, ACT_NONE, true, BN>(APE_EPI_ARGS); else epi16_fast<__nv_bfloat16, ACT_NONE, true, BN>(APE_EPI_ARGS); }
-        else { if (f16) epi16_fast<__half, ACT_NONE, false, BN>(APE_EPI_ARGS); else epi16_fast<__nv_bfloat16, ACT_NONE, false, BN>(APE_EPI_ARGS); }
-        return;
-      case 2:  // 16-bit, ReLU (bias present)
-        if (f16) epi16_fast<__half, ACT_RELU, true, BN>(APE_EPI_ARGS); else epi16_fast<__nv_bfloat16, ACT_RELU, true, BN>(APE_EPI_ARGS);
-        return;
-      case 3:  // SwiGLU
-        if constexpr (BN == 256) {
-          if (p.stats_out != nullptr) { if (f16) epi16_swiglu_fast<__half, true, BN>(APE_EPI_ARGS); else epi16_swiglu_fast<__nv_bfloat16, true, BN>(APE_EPI_ARGS); }
-          else { if (f16) epi16_swiglu_fast<__half, false, BN>(APE_EPI_ARGS); else epi16_swiglu_fast<__nv_bfloat16, false, BN>(APE_EPI_ARGS); }
-          return;
-        }
-        break;
-      case 4: epi32_fast<false, false, BN>(APE_EPI_ARGS); return;  // fp32 = acc + bias
-      case 5: epi32_fast<true, false, BN>(APE_EPI_ARGS); return;   // + fp32 residual
-      case 6: epi32_fast<true, true, BN>(APE_EPI_ARGS); return;    // + LayerNorm fold
-      case 7: epi32_fast<false, true, BN>(APE_EPI_ARGS); return;
-      default: break;
-    }
-  }
-  if (p.out_dtype == APE_DTYPE_F32) epilogue_tma_f32<BN>(APE_EPI_ARGS);
-  else if (p.out_dtype == APE_DTYPE_F16) epilogue_tma<__half, BN>(APE_EPI_ARGS);
-  else epilogue_tma<__nv_bfloat16, BN>(APE_EPI_ARGS);
-#undef APE_EPI_ARGS
-}
-
-// CL = cluster size along M (1 or 2).  With CL == 2 the two CTAs of a cluster work on vertically adjacent
-// 128-row tiles of the same BN-column block: each loads half of the B (weight) tile and TMA-multicasts it into
-// both CTAs' shared memory, so the L2 -> SM traffic per CTA drops from 48 KB to 32 KB per k-block (these GEMMs
-// are L2-bandwidth bound at 128x256 tiles: ncu shows ~10 TB/s of xbar2l1tex reads).  A stage may only be
-// refilled when BOTH CTAs' MMAs have finished reading it, so every tcgen05.commit of a stage arrives on the
-// "empty" barrier of both CTAs (multicast commit, barrier count 2).
-template <int BN, int STAGES, int CL>
+// CL = cluster size along M (1 or 2).  With CL == 2 the two CTAs of a cluster work on vertically adjacent 128-row tiles
+// of the same BN-column block: each loads half of the B (weight) tile and TMA-multicasts it into both CTAs' shared
+// memory, which halves the weight traffic from L2 per CTA.  A stage may only be refilled when the consumers of BOTH CTAs
+// have finished reading it, so every consumer warp arrives on the "empty" barrier of both CTAs.
+template <int BN, int STAGES, int CL, typename TI>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_c, const GemmParams p) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
   if (threadIdx.x == 0) trace_stamp(p, 0);
   using Smem = GemmSmem<BN, STAGES>;
   Smem &s = *reinterpret_cast<Smem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr uint32_t STAGE_BYTES = (BM + BN) * BK * 2;
-  constexpr uint32_t TMEM_COLS = 2 * BN;  // 256 or 512: power of two >= 32
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   // work items: (m group of CL row blocks, n block); CTA `rank` of the cluster takes row block CL*m_group + rank
@@ -753,35 +254,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     return true;
   };
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     tc::prefetch_tensormap(&map_a);
     tc::prefetch_tensormap(&map_b);
-    if (p.tma_store) tc::prefetch_tensormap(&map_c);
 #pragma unroll
     for (int i = 0; i < STAGES; ++i) {
       tc::mbar_init(&s.full[i], 1);
-      tc::mbar_init(&s.empty[i], CL);
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&s.tmem_full[i], 1);
-      tc::mbar_init(&s.tmem_empty[i], 8);  // one arrival per epilogue warp
+      tc::mbar_init(&s.empty[i], kConsumerWarps * CL);  // one arrival per consumer warp of each CTA of the cluster
     }
     tc::fence_mbar_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(&s.tmem_base, TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  if (CL > 1) tc::cluster_sync_all();  // peer barriers are initialised before any multicast can reach them
-  tc::fence_after_sync();
-  const uint32_t tmem_base = s.tmem_base;
+  if (CL > 1) tc::cluster_sync_all();  // peer barriers are initialised before any multicast / remote arrive can reach them
   pdl_wait();  // set-up done: operands / residual of the previous kernel may be read, C may be written from here on
   if (threadIdx.x == 0) trace_stamp(p, 1);
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
@@ -810,256 +298,58 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      int m_blk, n_blk;
-      for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
-        tc::mbar_wait(&s.tmem_empty[acc], acc_phase ^ 1);
-        tc::fence_after_sync();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          tc::mbar_wait(&s.full[stage], phase);
-          tc::fence_after_sync();
-          if (kb == 0 && t == 0) trace_stamp(p, 2);
-          const uint64_t da = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage]));
-          const uint64_t db = tc::make_smem_desc_sw128(tc::smem_u32(s.b[stage]));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance 16 elements (32 B) along K inside the 128-byte swizzle row: +2 in the >>4 address field
-            tc::mma_f16(tmem_d, da + 2 * k, db + 2 * k, p.idesc, (kb | k) != 0);
-          }
-          // frees the smem slot once these MMAs have read it (in both CTAs of a cluster: the peer multicasts into it)
-          if (CL == 1) tc::mma_commit(&s.empty[stage]);
-          else tc::mma_commit_multicast(&s.empty[stage], (uint16_t)((1u << CL) - 1));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc::mma_commit(&s.tmem_full[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      trace_stamp(p, 3);
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue (warps 2..9) =====================
-    const int quad = warp % 4;        // TMEM lane quadrant this warp may access
-    const int half = (warp - 2) / 4;  // which half of the tile's columns
-    uint8_t *slab = s.c[warp - 2];
-    uint32_t acc = 0, acc_phase = 0;
-    int m_blk = 0, n_blk = 0;
-    bool have = tile_at(0, m_blk, n_blk);
-    for (int t = 0; have; ++t) {
-      int m_next = 0, n_next = 0;
-      const bool have_next = tile_at(t + 1, m_next, n_next);
-      if (p.trace != nullptr && warp == 2) {  // (tracing only: the stamp needs the wait here; it is repeated below at no cost)
-        tc::mbar_wait(&s.tmem_full[acc], acc_phase);
-        if (lane == 0) {
-          if (t == 0) trace_stamp(p, 4);
-          trace_stamp(p, 5);
-        }
+    // ===================== consumers (two warpgroups) =====================
+    const int wg = warp / 4;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    auto release = [&](uint32_t st) {  // the MMAs that read stage `st` have completed (in this warp's view of the group)
+      if (lane == 0) {
+        tc::mbar_arrive(&s.empty[st]);
+        if (CL > 1) tc::mbar_arrive_cluster(tc::mapa_u32(&s.empty[st], (uint32_t)(rank ^ 1)));
       }
-      if (p.tma_store) {  // these wait for the accumulator themselves, after requesting what they read from global memory
-        epilogue_dispatch<BN>(p, &map_c, slab, tmem_base + acc * BN, quad, half, lane, m_blk, n_blk, &s.tmem_full[acc], acc_phase);
-      } else {
-        tc::mbar_wait(&s.tmem_full[acc], acc_phase);
-        tc::fence_after_sync();
-        const int m = m_blk * BM + quad * 32 + lane;
-#pragma unroll 1
-        for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); ++c) {
-          uint32_t r[32];
-          tc::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN + c * 32, r);
-          tc::tmem_ld_wait();
-          if (m < p.M) {
-            const int n0 = n_blk * BN + c * 32;
-            if (p.out_dtype == APE_DTYPE_F32) epilogue_chunk<float>(p, r, m, n0);
-            else if (p.out_dtype == APE_DTYPE_F16) epilogue_chunk<__half>(p, r, m, n0);
-            else epilogue_chunk<__nv_bfloat16>(p, r, m, n0);
-          }
+    };
+    uint32_t stage = 0, phase = 0;
+    int m_blk, n_blk;
+    for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
+      uint32_t prev = 0;
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        tc::mbar_wait(&s.full[stage], phase);
+        if (kb == 0 && t == 0 && threadIdx.x == 0) trace_stamp(p, 2);
+        const uint64_t da = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage] + wg * 64 * BK * 2));
+        const uint64_t db = tc::make_smem_desc_sw128(tc::smem_u32(s.b[stage]));
+        tc::fence_regs<BN / 2>(acc);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WG_K; ++k)  // advance 16 elements (32 B) along K inside the 128-byte swizzle row
+          tc::Wgmma<BN, TI>::template ss<0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        tc::wgmma_commit();
+        tc::fence_regs<BN / 2>(acc);
+        if (kb > 0) {
+          tc::wgmma_wait<1>();
+          release(prev);
         }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      m_blk = m_next; n_blk = n_next; have = have_next;
+      tc::wgmma_wait<0>();
+      tc::fence_regs<BN / 2>(acc);
+      release(prev);
+      if (threadIdx.x == 0) {
+        trace_stamp(p, 3);
+        if (t == 0) trace_stamp(p, 4);
+        trace_stamp(p, 5);
+      }
+      if (p.out_dtype == APE_DTYPE_F32) epilogue<float, BN>(p, acc, m_blk, n_blk, wg, lane);
+      else if (p.out_dtype == APE_DTYPE_F16) epilogue<__half, BN>(p, acc, m_blk, n_blk, wg, lane);
+      else epilogue<__nv_bfloat16, BN>(p, acc, m_blk, n_blk, wg, lane);
     }
-    if (p.tma_store && lane == 0) tc::tma_store_wait_all();  // global writes complete before the CTA exits
-    __syncwarp();
-    if (warp == 2 && lane == 0) trace_stamp(p, 6);
+    if (threadIdx.x == 0) trace_stamp(p, 6);
   }
-  tc::fence_before_sync();
   __syncthreads();
   if (CL > 1) tc::cluster_sync_all();  // no CTA leaves while its peer can still signal its barriers
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc(tmem_base, TMEM_COLS);
-  }
   if (threadIdx.x == 0) trace_stamp(p, 7);
-}
-
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs owns a 256 x BN output tile.  CTA r loads its own
-// 128 rows of A and its own BN/2 rows of the weight tile; ONE thread of the leader CTA issues M=256 MMAs that read
-// both CTAs' shared memory and write both CTAs' tensor memory (CTA r holds rows 128r..128r+127 of the tile).
-// Per SM and k-block that is 32 KB written + 32 KB read from shared memory for 128x256x64 MACs — two thirds of
-// the single-CTA kernel's traffic, which ncu showed pinned at the shared-memory / L2->SM limits.
-//   full[stage]      leader only; expect_tx = both CTAs' bytes; every TMA of the pair completes on it
-//   empty[stage]     in each CTA; one multicast tcgen05.commit per k-block arrives on both
-//   tmem_full[acc]   in each CTA; multicast commit after the last k-block of a tile
-//   tmem_empty[acc]  leader only; 16 arrivals (8 epilogue warps of each CTA, the peer's arrive remotely)
-template <int BN, int STAGES>
-struct alignas(1024) PairSmem {
-  uint8_t a[STAGES][BM * BK * 2];
-  uint8_t b[STAGES][(BN / 2) * BK * 2];
-  uint8_t c[8][32 * 128];
-  uint64_t full[STAGES], empty[STAGES];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
-};
-
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_c, const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  using Smem = PairSmem<BN, STAGES>;
-  Smem &s = *reinterpret_cast<Smem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr uint32_t CTA_STAGE_BYTES = (BM + BN / 2) * BK * 2;
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const uint32_t rank = tc::cluster_ctarank();
-  const bool leader = rank == 0;
-  const int m_pairs = (p.m_blocks + 1) / 2;
-  const int num_tiles = m_pairs * p.n_blocks;
-  const int first = blockIdx.x / 2, stride = gridDim.x / 2;
-
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tensormap(&map_a);
-    tc::prefetch_tensormap(&map_b);
-    if (p.tma_store) tc::prefetch_tensormap(&map_c);
-#pragma unroll
-    for (int i = 0; i < STAGES; ++i) {
-      tc::mbar_init(&s.full[i], 1);
-      tc::mbar_init(&s.empty[i], 1);
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&s.tmem_full[i], 1);
-      tc::mbar_init(&s.tmem_empty[i], 16);
-    }
-    tc::fence_mbar_init();
-  }
-  __syncthreads();
-  tc::cluster_sync_all();  // both CTAs' barriers exist before any remote arrive / multicast commit
-  if (warp == 1) {
-    tc::tmem_alloc_pair(&s.tmem_base, TMEM_COLS);
-    tc::tmem_relinquish_pair();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = s.tmem_base;
-  pdl_wait();
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = first; tile < num_tiles; tile += stride) {
-        const int mg = p.n_fastest ? tile / p.n_blocks : tile % m_pairs;
-        const int n_blk = p.n_fastest ? tile % p.n_blocks : tile / m_pairs;
-        const int m_blk = mg * 2 + (int)rank;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          tc::mbar_wait(&s.empty[stage], phase ^ 1);
-          if (leader) tc::mbar_expect_tx(&s.full[stage], 2 * CTA_STAGE_BYTES);
-          const uint32_t full_leader = tc::mapa_u32(&s.full[stage], 0);
-          if (p.conv) {  // implicit-GEMM 3x3 convolution: the pixel tile shifted by the filter tap (see gemm_tc_kernel)
-            const int img = m_blk / p.conv_tiles_img, tt = m_blk - img * p.conv_tiles_img;
-            const int ty = tt / p.conv_tiles_x, tx = tt - ty * p.conv_tiles_x;
-            const int tap = kb / p.conv_cblks, cb = kb - tap * p.conv_cblks;
-            tc::tma_load_4d_pair(s.a[stage], &map_a, full_leader, cb * BK, tx * p.conv_tw + tap % 3 - 1, ty * p.conv_th + tap / 3 - 1, img);
-          } else {
-            tc::tma_load_2d_pair(s.a[stage], &map_a, full_leader, kb * BK, m_blk * BM);
-          }
-          tc::tma_load_2d_pair(s.b[stage], &map_b, full_leader, kb * BK, n_blk * BN + (int)rank * (BN / 2));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (int tile = first; tile < num_tiles; tile += stride) {
-        tc::mbar_wait(&s.tmem_empty[acc], acc_phase ^ 1);
-        tc::fence_after_sync();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          tc::mbar_wait(&s.full[stage], phase);
-          tc::fence_after_sync();
-          const uint64_t da = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage]));
-          const uint64_t db = tc::make_smem_desc_sw128(tc::smem_u32(s.b[stage]));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) tc::mma_f16_pair(tmem_d, da + 2 * k, db + 2 * k, p.idesc, (kb | k) != 0);
-          tc::mma_commit_pair(&s.empty[stage], 3);  // both CTAs may refill this stage once the MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc::mma_commit_pair(&s.tmem_full[acc], 3);  // accumulator complete -> both CTAs' epilogues
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..9, both CTAs) =====================
-    const int quad = warp % 4;
-    const int half = (warp - 2) / 4;
-    uint8_t *slab = s.c[warp - 2];
-    uint32_t acc = 0, acc_phase = 0;
-    auto pair_tile = [&](int tile, int &m_blk, int &n_blk) {
-      const int mg = p.n_fastest ? tile / p.n_blocks : tile % m_pairs;
-      n_blk = p.n_fastest ? tile % p.n_blocks : tile / m_pairs;
-      m_blk = mg * 2 + (int)rank;
-    };
-    for (int tile = first; tile < num_tiles; tile += stride) {
-      int m_blk, n_blk;
-      pair_tile(tile, m_blk, n_blk);
-      if (p.tma_store) {  // these wait for the accumulator themselves, after requesting what they read from global memory
-        epilogue_dispatch<BN>(p, &map_c, slab, tmem_base + acc * BN, quad, half, lane, m_blk, n_blk, &s.tmem_full[acc], acc_phase);
-      } else {
-        tc::mbar_wait(&s.tmem_full[acc], acc_phase);
-        tc::fence_after_sync();
-        const int m = m_blk * BM + quad * 32 + lane;
-#pragma unroll 1
-        for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); ++c) {
-          uint32_t r[32];
-          tc::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN + c * 32, r);
-          tc::tmem_ld_wait();
-          if (m < p.M) {
-            const int n0 = n_blk * BN + c * 32;
-            if (p.out_dtype == APE_DTYPE_F32) epilogue_chunk<float>(p, r, m, n0);
-            else if (p.out_dtype == APE_DTYPE_F16) epilogue_chunk<__half>(p, r, m, n0);
-            else epilogue_chunk<__nv_bfloat16>(p, r, m, n0);
-          }
-        }
-      }
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive_cluster(tc::mapa_u32(&s.tmem_empty[acc], 0));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (p.tma_store && lane == 0) tc::tma_store_wait_all();
-    __syncwarp();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();  // no CTA leaves (or frees tensor memory) while its peer can still touch it
-  if (warp == 1) {
-    tc::fence_after_sync();
-    tc::tmem_dealloc_pair(tmem_base, TMEM_COLS);
-  }
 }
 
 // ---- host ----------------------------------------------------------------------------------------
@@ -1102,16 +392,16 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-template <int BN, int STAGES, int CL>
-int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mc, GemmParams &p, cudaStream_t st) {
+template <int BN, int STAGES, int CL, typename TI>
+int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
   using Smem = GemmSmem<BN, STAGES>;
   const size_t smem = sizeof(Smem) + 1024;
-  auto k = gemm_tc_kernel<BN, STAGES, CL>;
+  auto k = gemm_tc_kernel<BN, STAGES, CL, TI>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1137,44 +427,22 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap 
   attr[1].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k, ma, mb, mc, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, k, ma, mb, p);
   if (e != cudaSuccess) return fail((int)e, "gemm_tc_kernel launch: %s", cudaGetErrorString(e));
   return check_launch("gemm_tc_kernel");
 }
 
-template <int BN, int STAGES>
-int launch_gemm_pair(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mc, GemmParams &p, cudaStream_t st) {
-  using Smem = PairSmem<BN, STAGES>;
-  const size_t smem = sizeof(Smem) + 1024;
-  auto k = gemm_pair_kernel<BN, STAGES>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail((int)e, "gemm: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
-    attr_set = true;
-  }
-  p.n_blocks = (p.N + BN - 1) / BN;
-  p.n_fastest = p.n_blocks <= 8;
-  const int tiles = (p.m_blocks + 1) / 2 * p.n_blocks;
-  const int max_clusters = num_sms() / 2;
-  const int clusters = tiles < max_clusters ? tiles : max_clusters;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(clusters * 2));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k, ma, mb, mc, p);
-  if (e != cudaSuccess) return fail((int)e, "gemm_pair_kernel launch: %s", cudaGetErrorString(e));
-  return check_launch("gemm_pair_kernel");
+// 4 stages of 48 KB (BN = 256) or 6 of 32 KB (BN = 128): 192 KB of the 227 KB a block may use.
+template <int CL, typename TI>
+int launch_bn(int bn, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+  if (bn == 256) return launch_gemm<256, 4, CL, TI>(ma, mb, p, st);
+  return launch_gemm<128, 6, CL, TI>(ma, mb, p, st);
+}
+
+int launch_any(int bn, bool cluster, int in_dtype, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+  if (in_dtype == APE_DTYPE_BF16)
+    return cluster ? launch_bn<2, __nv_bfloat16>(bn, ma, mb, p, st) : launch_bn<1, __nv_bfloat16>(bn, ma, mb, p, st);
+  return cluster ? launch_bn<2, __half>(bn, ma, mb, p, st) : launch_bn<1, __half>(bn, ma, mb, p, st);
 }
 
 }  // namespace
@@ -1219,97 +487,50 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
     return fail(APE_ERR_INVALID_ARG, "gemm: A/W base and row pitch must be 16-byte aligned (TMA)");
   if (lda < K || ldw < K) return fail(APE_ERR_INVALID_ARG, "gemm: row pitch smaller than K");
   if (act == ACT_SWIGLU && ((N & 1) || residual)) return fail(APE_ERR_INVALID_ARG, "gemm: swiglu needs even N, no residual");
-  const int bn = (tile_n & 0xfff) > 0 ? (tile_n & 0xfff) : (N > 128 ? 256 : 128);
+  // default tile width 128: a 128 x 256 tile holds 128 fp32 accumulators per consumer thread, more than the 168 registers a
+  // thread of this 288-thread block may use leave room for next to the epilogue (it spills); 256 stays selectable
+  const int bn = (tile_n & 0xfff) > 0 ? (tile_n & 0xfff) : 128;
   if (bn != 128 && bn != 256) return fail(APE_ERR_INVALID_ARG, "gemm: tile_n must be 128 or 256");
+  if (tile_n & 0x2000) return fail(APE_ERR_UNSUPPORTED, "gemm: tile_n flag 0x2000 (CTA-pair MMA) is not available on sm_90a");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // kernel variant: single CTA, or a cluster of 2 along M sharing the weight tile by TMA multicast.  The cluster pays off
+  // when the K loop is long (K >= 2048: w3, FFN2, the 3x3 convolutions), where the weight tile is the larger share of the
+  // operand traffic; bit 0x1000 forces the single CTA, bit 0x4000 the cluster.
+  const int m_blocks = (M + BM - 1) / BM;
+  const bool cluster = m_blocks >= 2 && (tile_n & 0x1000) == 0 && ((tile_n & 0x4000) != 0 || K >= 2048);
   CUtensorMap ma, mb;
   if (int rc = make_map(&ma, A, in_dtype, M, K, lda, BM)) return rc;
-  // cluster of 2 along M whenever there are at least two row blocks (tile_n bit 0x1000 forces single-CTA)
-  // default variant per shape from the measured sweep (profiles/r01_gemm_sweep.txt): the multicast cluster only wins when
-  // the K loop is long (K >= 2048: w3, FFN2); bit 0x4000 forces it, bit 0x1000 forces the single-CTA kernel
-  // APE_GEMM_POLICY=mc|single overrides the per-shape default for A/B runs of the whole step (read once)
-  static const int policy = [] {
-    const char *e = getenv("APE_GEMM_POLICY");
-    return e == nullptr ? 0 : (e[0] == 'm' ? 1 : e[0] == 's' ? 2 : 0);
-  }();
-  const int bn_pre = (tile_n & 0xfff) > 0 ? (tile_n & 0xfff) : (N > 128 ? 256 : 128);
-  const bool pair_shape = K >= 2048 || ((N + bn_pre - 1) / bn_pre <= 4 && M >= 4096) || N >= 4096;
-  const bool auto_single = policy == 2 || (policy == 0 && !pair_shape);
-  const bool single = (tile_n & 0x1000) != 0 || M <= BM || (auto_single && (tile_n & 0xE000) == 0);
-  // kernel variant: default = cluster of 2 along M sharing the weight tile by TMA multicast (1-CTA MMA); 0x2000 = CTA-pair
-  // MMA (cta_group::2, 256 x bn tiles; measured equal or slower on B200 for these shapes, kept selectable);
-  // measured (profiles/r02_gemm_phases.jsonl): the CTA pair is the fastest variant for the long K loops (w3 4096x1024x2730:
-  // 33.6 us against 37.7 single / 38.6 multicast; FFN2 87296x256x2048: 105.9 against 113.3 / 116.3)
-  // with the lean epilogues (profiles/r02_gemm_phases_lean.jsonl) it also wins where a CTA has few column blocks to walk
-  // (proj 20.6 us against 23.6 single, the 87296 x 256 x 256 projections 27.9 / 30.2, qo 48.7 / 53.8) and on the widest GEMM
-  // (w12 44.1 / 46.9); the single-CTA kernel keeps qkv (27.6 / 28.8), FFN1 (115 / 164) and the 900-row decoder GEMMs
-  const int n_blocks_bn = (N + bn - 1) / bn;
-  const bool auto_pair = K >= 2048 || (n_blocks_bn <= 4 && M >= 4096) || N >= 4096;
-  const bool pair = !single && ((tile_n & 0x2000) != 0 || (policy == 0 && auto_pair && (tile_n & 0xC000) == 0));
-  if (int rc = make_map(&mb, W, in_dtype, N, K, ldw, single ? bn : bn / 2)) return rc;
+  if (int rc = make_map(&mb, W, in_dtype, N, K, ldw, cluster ? bn / 2 : bn)) return rc;
   GemmParams p{};
   p.C = C; p.bias = bias; p.residual = residual; p.ldc = ldc; p.ldr = ldr;
   p.M = M; p.N = N; p.K = K;
-  p.m_blocks = (M + BM - 1) / BM;
+  p.m_blocks = m_blocks;
   p.k_blocks = (K + BK - 1) / BK;
   p.out_dtype = out_dtype; p.act = act; p.res_dtype = res_dtype;
   p.trace = g_gemm_trace;
-  p.idesc = tc::make_idesc_f16(BM, bn, in_dtype == APE_DTYPE_BF16 ? 1 : 0);
-  // 16-bit outputs with 16-byte aligned rows leave through shared memory + TMA stores
-  const int n_out = act == ACT_SWIGLU ? N / 2 : N;
-  CUtensorMap mc = ma;
   const int oe = out_dtype == APE_DTYPE_F32 ? 4 : 2;
-  p.tma_store = (ldc * oe) % 16 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0 &&
-                (act != ACT_SWIGLU || (bn == 256 && oe == 2)) && (oe == 2 || n_out >= 32);
-  if (p.tma_store)  // one slab = 32 rows x 128 bytes
-    if (int rc = make_map(&mc, C, out_dtype, M, n_out, ldc, 32, 128 / oe)) return rc;
+  p.vec_out = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) % (2 * oe)) == 0;
+  p.vec_res = residual != nullptr && (ldr % 2) == 0 && (reinterpret_cast<uintptr_t>(residual) % 8) == 0;
+  const int n_out = act == ACT_SWIGLU ? N / 2 : N;
   if (fuse) {
     if (fuse->ln_part) {
-      if (!p.tma_store || out_dtype != APE_DTYPE_F32 || !fuse->ln_colsum || fuse->ln_nparts <= 0 || act == ACT_SWIGLU)
-        return fail(APE_ERR_INVALID_ARG, "gemm+ln: needs an fp32 output with 16-byte aligned rows (N >= 32), column sums and partial statistics");
+      if (out_dtype != APE_DTYPE_F32 || !fuse->ln_colsum || fuse->ln_nparts <= 0 || act == ACT_SWIGLU)
+        return fail(APE_ERR_INVALID_ARG, "gemm+ln: needs an fp32 output, column sums and partial statistics");
       p.ln_part = fuse->ln_part; p.ln_colsum = fuse->ln_colsum; p.ln_nparts = fuse->ln_nparts;
       p.ln_inv_c = fuse->ln_inv_c; p.ln_eps = fuse->ln_eps;
     }
     if (fuse->stats_out) {
-      if (!p.tma_store || act != ACT_SWIGLU || fuse->stats_nslab != (n_out + 63) / 64)
-        return fail(APE_ERR_INVALID_ARG, "gemm+stats: needs the SwiGLU epilogue with a 16-bit aligned output and stats_nslab = ceil(N/2/64)");
+      if (oe != 2 || act != ACT_SWIGLU || fuse->stats_nslab != (n_out + 63) / 64)
+        return fail(APE_ERR_INVALID_ARG, "gemm+stats: needs the SwiGLU epilogue with a 16-bit output and stats_nslab = ceil(N/2/64)");
       p.stats_out = fuse->stats_out; p.stats_nslab = fuse->stats_nslab;
     }
   }
   if (rope) {
-    if (!p.tma_store || oe != 2 || act != ACT_NONE || rope->cols % 64 != 0 || rope->cols > N || rope->npos <= 0 || !rope->cos || !rope->sin)
-      return fail(APE_ERR_INVALID_ARG, "gemm+rope: needs a 16-bit aligned output, no activation, rope_cols a multiple of 64 <= N");
+    if (oe != 2 || act != ACT_NONE || rope->cols % 64 != 0 || rope->cols > N || rope->npos <= 0 || !rope->cos || !rope->sin)
+      return fail(APE_ERR_INVALID_ARG, "gemm+rope: needs a 16-bit output, no activation, rope_cols a multiple of 64 <= N");
     p.rope_cos = rope->cos; p.rope_sin = rope->sin; p.rope_pos = rope->pos; p.rope_cols = rope->cols; p.rope_npos = rope->npos;
   }
-  // lean epilogue (see epilogue_dispatch): whole-tile cases with 16-byte aligned vectors; APE_GEMM_LEAN=0 disables (A/B runs)
-  static const bool lean_on = [] {
-    const char *e = getenv("APE_GEMM_LEAN");
-    return !(e != nullptr && e[0] == '0');
-  }();
-  p.lean = 0;
-  const bool al16 = ((reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(fuse ? fuse->ln_colsum : nullptr)) & 15) == 0;
-  if (lean_on && p.tma_store && !rope && al16) {
-    if (oe == 2 && act == ACT_SWIGLU && bias != nullptr && bn == 256) p.lean = 3;
-    else if (oe == 2 && residual == nullptr && act == ACT_NONE) p.lean = 1;
-    else if (oe == 2 && residual == nullptr && act == ACT_RELU && bias != nullptr) p.lean = 2;
-    else if (oe == 4 && act == ACT_NONE && bias != nullptr && !(fuse && fuse->stats_out)) {
-      const bool res_ok = residual == nullptr || (res_dtype == APE_DTYPE_F32 && (ldr & 3) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0);
-      const bool ln = fuse != nullptr && fuse->ln_part != nullptr;
-      if (res_ok) p.lean = residual != nullptr ? (ln ? 6 : 5) : (ln ? 7 : 4);
-    }
-  }
-  if (pair) {
-    p.idesc = tc::make_idesc_f16(2 * BM, bn, in_dtype == APE_DTYPE_BF16 ? 1 : 0);
-    // 5 stages of 32 KB: a sixth was measured slower in the step (13.68 against 13.36 ms)
-    if (bn == 256) return launch_gemm_pair<256, 5>(ma, mb, mc, p, st);
-    return launch_gemm_pair<128, 6>(ma, mb, mc, p, st);
-  }
-  if (single) {
-    if (bn == 256) return launch_gemm<256, 4, 1>(ma, mb, mc, p, st);
-    return launch_gemm<128, 6, 1>(ma, mb, mc, p, st);
-  }
-  if (bn == 256) return launch_gemm<256, 4, 2>(ma, mb, mc, p, st);
-  return launch_gemm<128, 6, 2>(ma, mb, mc, p, st);
+  return launch_any(bn, cluster, in_dtype, ma, mb, p, st);
 }
 
 extern "C" int ape_gemm_tn(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,
@@ -1350,7 +571,7 @@ static int make_map_nhwc(CUtensorMap *map, const void *base, int dtype, int B, i
   return APE_OK;
 }
 
-// 3x3 convolution, stride 1, zero padding 1, no dilation / groups, over NHWC activations as an implicit GEMM on the tcgen05
+// 3x3 convolution, stride 1, zero padding 1, no dilation / groups, over NHWC activations as an implicit GEMM on the wgmma
 // kernel: M = B*H*W output pixels, N = Cout, K = 9*Cin walked as (filter tap, 64-channel block).  The A tile of tap
 // (dy, dx) is the 128-pixel tile shifted by (dy-1, dx-1): one 4-D TMA box, out-of-image parts arrive as zeros.
 extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const float *bias, int B, int H, int W, int Cin, int Cout,
@@ -1367,38 +588,21 @@ extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const flo
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(y)) & 15)
     return fail(APE_ERR_INVALID_ARG, "conv3x3: tensors must be 16-byte aligned");
   const int K = 9 * Cin, M = B * H * W, N = Cout;
-  const int bn = N > 128 ? 256 : 128;
-  CUtensorMap ma, mb, mc;
+  const int bn = 128;
+  const int m_blocks = M / BM;
+  const bool cluster = m_blocks >= 2 && m_blocks % 2 == 0;  // K = 9 * Cin is a long loop: share the weight tile (see gemm_impl)
+  CUtensorMap ma, mb;
   if (int rc = make_map_nhwc(&ma, x, dtype, B, H, W, Cin, tw, th)) return rc;
-  if (int rc = make_map(&mb, w, dtype, N, K, K, bn)) return rc;
-  const int sw = tw < 32 ? tw : 32;
-  if (int rc = make_map_nhwc(&mc, y, dtype, B, H, W, Cout, sw, 32 / sw)) return rc;
+  if (int rc = make_map(&mb, w, dtype, N, K, K, cluster ? bn / 2 : bn)) return rc;
   GemmParams p{};
   p.C = y; p.bias = bias; p.ldc = N; p.M = M; p.N = N; p.K = K;
-  p.m_blocks = M / BM;
+  p.m_blocks = m_blocks;
   p.k_blocks = K / BK;
   p.out_dtype = dtype; p.res_dtype = dtype; p.act = act;
-  p.idesc = tc::make_idesc_f16(BM, bn, dtype == APE_DTYPE_BF16 ? 1 : 0);
-  p.tma_store = 1;
-  if (((reinterpret_cast<uintptr_t>(bias)) & 15) == 0) {  // lean whole-tile epilogue (epi16_fast) for the cases the pyramid / mask head run
-    if (act == ACT_NONE) p.lean = 1;
-    else if (act == ACT_RELU && bias != nullptr) p.lean = 2;
-  }
+  p.vec_out = 1;
   p.conv = 1; p.conv_tw = tw; p.conv_th = th; p.conv_tiles_x = W / tw; p.conv_tiles_img = (W / tw) * (H / th); p.conv_cblks = Cin / 64;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // K = 9 * Cin is a long loop: the CTA pair (half of the weight tile per SM) when the row blocks pair up; APE_CONV_PAIR=0 -> single
-  static const bool conv_pair = [] {
-    const char *e = getenv("APE_CONV_PAIR");
-    return !(e != nullptr && e[0] == '0');
-  }();
-  if (conv_pair && p.m_blocks % 2 == 0 && p.m_blocks >= 2) {
-    if (int rc = make_map(&mb, w, dtype, N, K, K, bn / 2)) return rc;
-    p.idesc = tc::make_idesc_f16(2 * BM, bn, dtype == APE_DTYPE_BF16 ? 1 : 0);
-    if (bn == 256) return launch_gemm_pair<256, 5>(ma, mb, mc, p, st);
-    return launch_gemm_pair<128, 6>(ma, mb, mc, p, st);
-  }
-  if (bn == 256) return launch_gemm<256, 4, 1>(ma, mb, mc, p, st);
-  return launch_gemm<128, 6, 1>(ma, mb, mc, p, st);
+  p.conv_W = W; p.conv_H = H;
+  return launch_any(bn, cluster, dtype, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,

@@ -1,4 +1,4 @@
-// msda_bwd.cu — multi-scale deformable attention, backward (sm_100a).
+// msda_bwd.cu — multi-scale deformable attention, backward (sm_90a).
 //
 // Replaces torch.ops.ape.ms_deform_attn_backward
 //   (ape/layers/csrc/vision.cpp:78, ms_deform_attn.h:42-61, host ms_deform_attn_cuda.cu:84-160,

@@ -1,4 +1,4 @@
-// msda_fwd.cu — multi-scale deformable attention forward for sm_100a (B200).
+// msda_fwd.cu — multi-scale deformable attention forward for sm_90a (H100).
 //
 // Replaces torch.ops.ape.ms_deform_attn_forward
 //   (ape/layers/csrc/MsDeformAttn/ms_deform_attn_cuda.cu:21-81, kernel
@@ -6,7 +6,7 @@
 // and, in the fused entry point, the softmax + sampling-location arithmetic of
 //   ape/layers/multi_scale_deform_attn.py:283-311.
 //
-// Design (B200-first, not a translation of the reference's thread-per-scalar kernel):
+// Design (GPU-first, not a translation of the reference's thread-per-scalar kernel):
 //   * a "row" is one (b, q, h) output vector of D channels.  One lane owns 16 bytes of a row
 //     (4 fp32 / 8 fp16|bf16 channels), so a row is LPR = D*sizeof(T)/16 lanes and every corner
 //     fetch is one 128-bit load per lane — a full 128 B line per fp32 row of D=32.
@@ -482,7 +482,7 @@ template <typename T>
 int launch_scalar(const MsdaParams &p, int D, cudaStream_t st) {
   const long long n = (long long)p.B * p.Q * p.H * D;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148LL * 64) blocks = 148LL * 64;
+  if (blocks > 132LL * 64) blocks = 132LL * 64;
   if (blocks < 1) blocks = 1;
   msda_fwd_scalar_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(p, D, n);
   return check_launch("msda_fwd_scalar_kernel");

@@ -338,7 +338,7 @@ extern "C" int ape_nms_classwise(const float *boxes, const float *scores, int64_
   int sms = 0, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int ctas = min(sms, (N + kCwWarps - 1) / kCwWarps);
   cw_scan_kernel<<<ctas, kCwWarps * 32, smem, st>>>(reinterpret_cast<const unsigned *>(workspace), scores, ld_scores, row_valid, Q,
                                                     N, W, score_thresh, out);

@@ -208,7 +208,7 @@ vlf_pool_kernel(const T *__restrict__ v, const float *__restrict__ scores, const
 }
 
 int strips_for(int S, int *strip_out) {
-  int nct = 148 * 2;
+  int nct = 132 * 2;  // two strips per SM of an H100 SXM
   int strip = (S + nct - 1) / nct;
   if (strip > kMaxStrip) strip = kMaxStrip;
   if (strip < 8) strip = 8;

@@ -39,7 +39,7 @@ class MultiScaleDeformableAttention(nn.Module):
             raise ValueError(
                 "embed_dim must be divisible by num_heads, but got {} and {}".format(embed_dim, num_heads))
         if not _is_power_of_2(embed_dim // num_heads):
-            warnings.warn("head dim should be a power of 2 for the vectorised sm_100a path")
+            warnings.warn("head dim should be a power of 2 for the vectorised sm_90a path")
         self.dropout = nn.Dropout(dropout)
         self.batch_first = batch_first
         self.im2col_step = img2col_step
@@ -54,9 +54,8 @@ class MultiScaleDeformableAttention(nn.Module):
         # accepted for config compatibility; this engine has exactly one (CUDA) path
         self.pytorch_attn = pytorch_attn
         # engine: calls with at least this many queries gather from the pair layout (csrc/msda_pair.cu).  Off by default
-        # (None): measured on B200 the pair kernel is 265-275 us against 293 us for the generic fused kernel on the
-        # encoder call, but the pairing pass costs 33 us, a net loss in the model (DESIGN.md section 9);
-        # APE_MSDA_PAIR=<min queries> (e.g. 2048) switches it on for A/B runs.
+        # (None): the gather itself is faster than the generic fused kernel on the encoder call, but the pairing pass
+        # costs more than it saves in the model; APE_MSDA_PAIR=<min queries> (e.g. 2048) switches it on for A/B runs.
         env = os.environ.get("APE_MSDA_PAIR", "")
         self.pair_layout_min_queries = int(env) if env.isdigit() and int(env) > 0 else None
         self._qcat = None
@@ -125,7 +124,7 @@ class MultiScaleDeformableAttention(nn.Module):
         engine = query.dtype in (torch.float16, torch.bfloat16) and value.dtype == query.dtype
         wq, bq = self._query_side_weights()
         if engine:
-            # tensor-core path: tcgen05 GEMMs (fp32 accumulate), fused gather kernel, residual in the epilogue
+            # tensor-core path: wgmma GEMMs (fp32 accumulate), fused gather kernel, residual in the epilogue
             value = ops.linear_module_tc(self.value_proj, value)
             w16, b32 = ops.cached(self, "_q16", query.dtype, (wq._version, wq.data_ptr()),
                                   lambda: (wq.to(query.dtype).contiguous(), bq.float().contiguous()))

@@ -47,7 +47,7 @@ class VisionLanguageAlign(nn.Module):
 
     def forward_engine(self, x, embedding):
         """Engine path (x [B,Q,C] fp16 / bf16 CUDA): the text projection, the language bias and the query x text contraction
-        are tcgen05 GEMMs (ape_gemm_tn); fp32 accumulation, fp32 logits, bias + clamp in the epilogue.  The reference's own
+        are wgmma GEMMs (ape_gemm_tn); fp32 accumulation, fp32 logits, bias + clamp in the epilogue.  The reference's own
         eval recipe runs this module in fp16 end to end (tools/train_net.py:641-642); here only the operands are 16-bit."""
         from .. import ops
 

@@ -37,7 +37,7 @@ class BiMultiHeadAttention(nn.Module):
             m.bias.data.fill_(0)
 
     def forward_engine(self, v, l):
-        """Engine path for several language tokens (phrase / text prompts): the six projections are tcgen05 GEMMs and
+        """Engine path for several language tokens (phrase / text prompts): the six projections are wgmma GEMMs and
         each softmax direction is ONE flash-attention pass of ape_attn_cross_fwd over 256-channel heads — the S x N_t
         score matrix of fuse_helper.py:86 (31 GB per head set at 1536^2 / 5 000 phrases) is never materialised, there is
         no host synchronisation and no data-dependent choice of algorithm.  v [B,S,v_dim] 16-bit and l [B,N,l_dim] are the
@@ -136,7 +136,7 @@ class BiAttentionBlock(nn.Module):
         if v.is_cuda and v.dtype in (torch.float16, torch.bfloat16) and l.shape[1] > 1 and attention_mask_l is None and \
                 not (a.use_attention_mask_v and attention_mask_v is not None) and a.head_dim in (64, 256) and \
                 v.shape[-1] % 8 == 0 and l.shape[-1] % 8 == 0:
-            from .. import ops  # engine: LayerNorm kernel, tcgen05 GEMMs, two flash-attention passes (forward_engine)
+            from .. import ops  # engine: LayerNorm kernel, wgmma GEMMs, two flash-attention passes (forward_engine)
 
             vn = ops.layernorm_module(self.layer_norm_v, v.contiguous())
             with torch.autocast("cuda", enabled=False):

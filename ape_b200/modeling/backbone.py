@@ -215,7 +215,7 @@ class ViT(nn.Module):
         # (+26 us per GEMM with the general epilogue, +27 us with a lean one: per-thread cos / sin rows are 32 different lines per
         # warp load) against 8.7 us for the pass; APE_FUSED_ROPE=1 switches it on for A/B runs
         self.fused_rope = os.environ.get("APE_FUSED_ROPE", "0") == "1"
-        self.engine_attention = True  # ape_attn_fwd (own tcgen05 kernel) for head_dim 64 / n % 128 == 0, else library SDPA
+        self.engine_attention = True  # ape_attn_fwd (own wgmma kernel) for head_dim 64 / n % 128 == 0, else library SDPA
         # inner_attn_ln / ffn_ln folded around proj / w3 (ape_gemm_tn_fused): two LayerNorm launches and two trips of the
         # activations through HBM fewer per block
         self.fold_sub_layernorms = True
@@ -250,7 +250,7 @@ class ViT(nn.Module):
         return {self._out_features[0]: x.permute(0, 3, 1, 2)}
 
     # ---------------------------------------------------------------------------------------------
-    # Engine path (fp16 / bf16): libape_b200 kernels — tcgen05 GEMMs with fused bias / SwiGLU /
+    # Engine path (fp16 / bf16): libape_b200 kernels — wgmma GEMMs with fused bias / SwiGLU /
     # residual epilogues, LayerNorm and RoPE kernels; tokens stay in WINDOW-MAJOR order for the
     # whole network (attention is permutation-equivariant once the RoPE table follows the tokens), so
     # window_partition / window_unpartition (utils_eva02.py:19-63) cost one permutation at the
@@ -369,7 +369,7 @@ class ViT(nn.Module):
                 nb, n = B, g * g
             fold = self.fold_sub_layernorms
             if self.engine_attention and ops.attention_supported(n, hd, qkv.dtype):
-                # tcgen05 flash attention, no head-split copies; with `fold` it also leaves per-(row, head) statistics
+                # wgmma flash attention, no head-split copies; with `fold` it also leaves per-(row, head) statistics
                 o = ops.attention_qkv(qkv, nb, n, heads, hd, blk.attn.scale, stats_out=fold)
                 o, st = o if fold else (o, None)
             else:
@@ -494,7 +494,7 @@ class SimpleFeaturePyramid(nn.Module):
                 for n in self._out_features}
 
     # Engine path: activations stay token-major (NHWC) from the ViT to the encoder.  2x2/stride-2 transposed
-    # convolutions and 1x1 convolutions are tcgen05 GEMMs over tokens; the pixel shuffle of a transposed conv is
+    # convolutions and 1x1 convolutions are wgmma GEMMs over tokens; the pixel shuffle of a transposed conv is
     # folded into the row map of the LayerNorm kernel that follows it; channels-first LayerNorm (detectron2 "LN")
     # is a row LayerNorm in this layout; only the 3x3 convolutions still go to cuDNN (channels_last, no copies).
     def _shuffle_map(self, B, g, device):

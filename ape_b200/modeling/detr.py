@@ -75,7 +75,7 @@ class ChannelMapper(nn.Module):
         first = inputs[self.in_features[0]]
         if first.is_cuda and first.dtype in (torch.float16, torch.bfloat16) and \
                 all(c.conv.kernel_size == (1, 1) and isinstance(c.norm, nn.GroupNorm) for c in self.convs):
-            # engine path: 1x1 conv = tcgen05 GEMM over tokens, GroupNorm kernel on the token-major layout, written
+            # engine path: 1x1 conv = wgmma GEMM over tokens, GroupNorm kernel on the token-major layout, written
             # straight into its slice of the flattened [B, S, C] tensor the transformer consumes
             # (deformable_transformer_vl.py:435-452 flattens + concatenates the levels): no concat copy.
             xs = [inputs[f] for f in self.in_features]
@@ -671,7 +671,7 @@ class DeformableDETRSegmVL(nn.Module):
             # (:507-517) only the last level's masks reach inference (the other levels are added times 0.0)
             mf = mask_features
             if states16.dtype in (torch.float16, torch.bfloat16) and mf.dtype == states16.dtype and mf.shape[1] % 8 == 0:
-                # engine: einsum("bqc,bchw->bqhw") = one tcgen05 GEMM per image over the token-major mask features
+                # engine: einsum("bqc,bchw->bqhw") = one wgmma GEMM per image over the token-major mask features
                 # (fp32 accumulation, fp32 logits: their sign decides the mask)
                 B, C, mh, mw = mf.shape
                 tok = mf.permute(0, 2, 3, 1).reshape(B, mh * mw, C)  # free: the engine's mask features are channels_last
@@ -726,7 +726,7 @@ class DeformableDETRSegmVL(nn.Module):
         p2 = features[self.mask_in_features[0]]
         if memory.is_cuda and memory.dtype in (torch.float16, torch.bfloat16) and p2.dtype == memory.dtype \
                 and isinstance(self.lateral_conv.norm, nn.GroupNorm) and p2.shape[1] % 8 == 0:
-            # engine: token-major throughout; the two 1x1 convolutions are tcgen05 GEMMs, GroupNorm is the repo's kernel, the
+            # engine: token-major throughout; the two 1x1 convolutions are wgmma GEMMs, GroupNorm is the repo's kernel, the
             # memory slice of the encode level is already token-major (no permute); the 3x3 convolution is the library's
             from .backbone import _conv_weights
 
@@ -771,7 +771,7 @@ class DeformableDETRSegmVL(nn.Module):
         for b, (qi, size, inp) in enumerate(zip(keep, image_sizes, batched_inputs)):
             cls = F.softmax(sem_cls[b, qi].float().sigmoid() / 0.06, dim=-1)
             if self.engine_dtype in (torch.float16, torch.bfloat16) and mask_pred.is_cuda and len(qi) > 0:
-                # engine: einsum("qc,qhw->chw") (757 GFLOP at K = 300 kept queries x 1203 names x 1024^2) as ONE tcgen05 GEMM:
+                # engine: einsum("qc,qhw->chw") (757 GFLOP at K = 300 kept queries x 1203 names x 1024^2) as ONE wgmma GEMM:
                 # the resize runs channels_last so that the sigmoid masks come out pixel-major [H*W, K] = the K-major operand
                 dt = self.engine_dtype
                 K = len(qi)

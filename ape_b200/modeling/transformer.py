@@ -57,7 +57,7 @@ class _SelfAttention(nn.Module):
     def forward(self, x, pos):
         E, nh = self.embed_dim, self.num_heads
         if x.is_cuda and x.dtype in (torch.float16, torch.bfloat16) and E // nh <= 64:
-            # engine path: tcgen05 GEMMs for the in / out projections (residual in the epilogue) and the repo's tcgen05
+            # engine path: wgmma GEMMs for the in / out projections (residual in the epilogue) and the repo's wgmma
             # flash-attention kernel over the queries (rows padded to a multiple of 128, padded keys masked)
             wqk, bqk, wv, bv, wo, bo = self._packed(x.dtype)
             B, N, _ = x.shape
@@ -134,7 +134,7 @@ class _DecoderLayer(nn.Module):
 
     def forward(self, query, value, query_pos, key_padding_mask, reference_points, spatial_shapes, level_start_index):
         if query.is_cuda and query.dtype in (torch.float16, torch.bfloat16) and value.dtype == query.dtype:
-            # engine path: every linear is a tcgen05 GEMM, norms are libape_b200 row kernels
+            # engine path: every linear is a wgmma GEMM, norms are libape_b200 row kernels
             dt = query.dtype  # residual sums in fp32 (GEMM epilogues), LayerNorm outputs / GEMM operands in dt
             x = self.attentions[0](query, query_pos)
             x = ops.layernorm_module(self.norms[0], x, out_dtype=dt)
@@ -200,7 +200,7 @@ class DeformableDetrTransformerEncoderVL(nn.Module):
           tiny fp32 ops on the language token (delta_v, folded score operands)
           -> ONE row kernel: [last norm of the previous layer] -> layer_norm_v -> + gamma_v*delta_v -> (query, query+pos)
           -> pooling kernels over `query` (language-side update; fuse_helper.py:67-166 restructured)
-          -> deformable self-attention + FFN (tcgen05 GEMMs, fused gather), last norm deferred to the next layer.
+          -> deformable self-attention + FFN (wgmma GEMMs, fused gather), last norm deferred to the next layer.
         Same functions as `vl_layer(...)` followed by `layer(...)`; the activations cross HBM once per row kernel."""
         pending = None
         dt = x.dtype

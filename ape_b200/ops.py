@@ -189,7 +189,7 @@ ACT = {None: 0, "none": 0, "relu": 1, "gelu": 2, "swiglu": 3, "clamp": 4}
 
 
 def linear_tc(x, weight, bias=None, act=None, out_dtype=None, residual=None, tile_n=0, out=None, ln_fold=None, stats_out=False):
-    """act(x @ weight.T + bias) (+ residual) on the tcgen05 tensor cores (ape_gemm_tn).
+    """act(x @ weight.T + bias) (+ residual) on the wgmma tensor cores (ape_gemm_tn).
 
     x [..., K] and weight [N, K] fp16/bf16 with unit inner stride; bias fp32 [N] (or None); residual
     [..., N] fp32 / fp16 / bf16 (any of them with any output dtype: fp32 sums over 16-bit operands).
@@ -266,7 +266,7 @@ def conv3x3_supported(H, W, Cin, Cout, dtype):
 
 def conv3x3_nhwc(x, weight_ohwi, bias=None, act=None):
     """3x3 / stride 1 / zero padding 1 convolution over token-major activations x [B,H,W,Cin] (ape_conv3x3_nhwc: implicit GEMM on
-    the tcgen05 kernel, 4-D TMA boxes at shifted positions).  weight_ohwi [Cout,3,3,Cin] contiguous, same 16-bit dtype."""
+    the wgmma kernel, 4-D TMA boxes at shifted positions).  weight_ohwi [Cout,3,3,Cin] contiguous, same 16-bit dtype."""
     _require(x.is_cuda and x.dim() == 4 and x.is_contiguous() and weight_ohwi.is_contiguous() and x.dtype == weight_ohwi.dtype,
              "conv3x3: contiguous CUDA NHWC input and OHWI weight of one dtype")
     B, H, W, Cin = x.shape
@@ -428,7 +428,7 @@ def attention_supported(n, head_dim, dtype):
 
 def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_out=False, seq_stride=None, causal=False):
     """softmax(q k^T * scale) v for every (sequence, head) straight from the fused qkv buffer [num_seq*n, 3*heads*64]
-    (ape_attn_fwd: flash attention on the tcgen05 tensor cores).  Returns [num_seq*n, heads*64].
+    (ape_attn_fwd: flash attention on the wgmma tensor cores).  Returns [num_seq*n, heads*64].
     n_valid: sequences are padded to n rows and only the first n_valid keys count (rows beyond must be finite).
     stats_out=True: also returns fp32 [rows, heads, 2] (sum, sum of squares of each row's stored values per head).
     seq_stride: rows between sequences when they are packed tighter than n (then n_valid <= seq_stride < n; rows of a tile

@@ -53,7 +53,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -107,9 +107,54 @@ class ClockSampler:
         return out
 
 
+DUMP_SAMPLE = 2 * 1024 * 1024  # elements kept of a larger array
+DUMP_LIMIT = 64 * 1024 * 1024  # bytes
+
+
+def dump_outputs(dirname, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array the timed path returned in its last step, float32 (float64 for integer
+    and boolean fields, which float32 cannot hold exactly).  An array of more than DUMP_SAMPLE elements is replaced by the
+    elements at DUMP_SAMPLE fixed positions of its flattened form (seeded, so the same shape gives the same positions):
+    two builds run with the same arguments see identical inputs and can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(dirname, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        t = t.detach().reshape(-1)
+        if t.numel() > DUMP_SAMPLE:
+            idx = torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(0))
+            t = t[idx.to(t.device)]
+        a = t.cpu().to(torch.float32 if t.is_floating_point() else torch.float64).numpy()
+        total += a.nbytes
+        assert total <= DUMP_LIMIT, "--dump-outputs: more than 64 MB of outputs"
+        np.save(os.path.join(dirname, f"{name}.npy"), a)
+
+
+def detection_arrays(out):
+    """The tensors of the model's per-image results: Instances fields (boxes as their [N, 4] tensor, COCO run-length codes as
+    their concatenated counts) and the semantic / panoptic maps."""
+    arrays = {}
+    for k, o in enumerate(out):
+        for key, v in o.items():
+            if key == "instances":
+                for f, x in v.get_fields().items():
+                    if hasattr(x, "tensor"):
+                        x = x.tensor
+                    elif isinstance(x, list):
+                        x = torch.cat([torch.as_tensor(r["counts"]).reshape(-1) for r in x]) if x else torch.zeros(0)
+                    arrays[f"img{k}_{f}"] = x
+            elif isinstance(v, torch.Tensor):
+                arrays[f"img{k}_{key}"] = v
+            elif isinstance(v, tuple):  # panoptic_seg: (segment map, segments info)
+                arrays[f"img{k}_{key}"] = v[0]
+    return arrays
+
+
 def host_threads():
     """Threads for the CPU arms: every core up to 32.  The ops of this path stop scaling around there; with one thread
-    per core of a 200-core host the oracle forward measured 136 s per image on the B200 box against 29 s on 8 cores."""
+    per core of a many-core host the oracle forward runs several times slower than on 8 cores (thread start-up and
+    synchronisation dominate the small ops)."""
     return max(1, min(os.cpu_count() or 1, 32))
 
 
@@ -169,7 +214,7 @@ def bench_weights(model):
 def cpu_model_arm(steps, warmup, n_text=1203, sd=None, seed=0):
     """Reference arm for the ape_l_d workload: the oracle's CPU port of the reference forward
     (oracle/ape_forward.py; /root/reference itself cannot travel to the GPU box), fp32, up to 32 host threads.
-    One whole-image forward is ~25 s of host time on the B200 box, so the arm runs at most 1 warm-up and 3 timed
+    One whole-image forward takes tens of seconds of host time, so the arm runs at most 1 warm-up and 3 timed
     forwards and DECLARES what it ran.  Same spec, same weights, same threshold, same image generator as the GPU arm."""
     from ape_b200 import synthetic
     from ape_b200.modeling import build_model
@@ -204,7 +249,7 @@ def msda_microbench(dev, quick=False):
     """BASELINE.json config 5 inside the driver-run record: ms_deform_attn forward on 4-level (128^2..16^2) and the
     model's 5-level pyramids, Q in {300, 900, S}, fp32 / fp16 / bf16, L2 flushed before every timed launch, median of 7:
     the drop-in operator (ape_msda_fwd), the engine's fused kernels (generic and pair layout, incl. the pairing pass) and —
-    when oracle/_ref/libref_msda.so travelled with the repo — the REFERENCE's own CUDA kernel recompiled for sm_100a on
+    when oracle/_ref/libref_msda.so travelled with the repo — the REFERENCE's own CUDA kernel recompiled for sm_90a on
     identical tensors (measurement only: the 'kernel to beat'; never on the product path)."""
     from ape_b200 import ops
 
@@ -328,6 +373,8 @@ def phrase_bench(args, rank, local_rank, world):
     b.record()
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, detection_arrays(out))
     ops.PROFILE_EVENTS = []
     n0 = ape_b200._lib.launch_count()
     step()
@@ -342,7 +389,7 @@ def phrase_bench(args, rank, local_rank, world):
     xflops = sum(4.0 * t[1] * t[4] * t[2] * t[3] * t[5] for t, _ in xs)
     xms = sum(d for _, d in xs)
     clocks = sampler.stop()
-    tpeak = 1590.0
+    tpeak = 989.0  # NVIDIA H100 SXM data sheet, dense BF16
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         tpeak = float(json.load(open(pk)).get("bf16_tflops", 0) or 0) or tpeak
@@ -356,7 +403,7 @@ def phrase_bench(args, rank, local_rank, world):
                     "note": "the timed steps already take pinned host images and return host detections"},
             "roofline": {"bound": "tensor", "achieved": xflops / (xms * 1e-3) / 1e12 if xms > 0 else None, "peak": tpeak, "unit": "TFLOP/s",
                          "frac": (xflops / (xms * 1e-3) / 1e12 / tpeak) if xms > 0 else None, "traffic": None,
-                         "kernel": "attn_xfwd_kernel (VisionLanguageFusion, 12 launches per step)", "flops_per_step": xflops, "ms_per_step": xms},
+                         "kernel": "attn_kernel (VisionLanguageFusion, 12 launches per step)", "flops_per_step": xflops, "ms_per_step": xms},
             "gpu_launches": int(launches) * args.steps, "clocks": clocks,
             "peak_memory_GB": torch.cuda.max_memory_allocated() / 2 ** 30,
             "own_kernel_ms_per_step": {k: round(v, 2) for k, v in sorted(own.items(), key=lambda kv: -kv[1])},
@@ -370,7 +417,7 @@ def model_bench(args, rank, local_rank, world):
     config = {"workload": "APE-L_D detection forward, 1024x1024 image, 1203-name vocabulary, boxes only, batch 1 per GPU",
               "weights": "random init of the real architecture (380 M params): ape_b200/synthetic.py, invalid anchors at the 0.01 prior",
               "text": "seeded synthetic features (text tower out of path)",
-              "l2": "per-step working set (weights 0.75 GB 16-bit + activations) >> 126 MB L2",
+              "l2": "per-step working set (weights 0.75 GB 16-bit + activations) >> 50 MB L2",
               "selection": f"test_score_thresh {BENCH_SCORE_THRESH} (~500 of 1.08M scores pass with these weights; README recipe: 0.1 "
                            "with trained weights); NMS 0.7; top-300",
               "parallelism": f"dp{args.gpus} (one image per GPU; one NCCL gather of packed detections per step when N>1)"}
@@ -457,6 +504,8 @@ def model_bench(args, rank, local_rank, world):
     b.record()
     barrier()
     total_ms = a.elapsed_time(b)
+    if args.dump_outputs and rank == 0 and isinstance(out, list):
+        dump_outputs(args.dump_outputs, detection_arrays(out))
     # Per-kernel durations for the roofline object: CUDA events cannot be recorded inside a graph replay, so
     # the same steps are run a few more times eagerly (same kernels, same inputs, same stream) with an event
     # pair around every launch of our library; launches per step are counted here too.
@@ -494,16 +543,8 @@ def model_bench(args, rank, local_rank, world):
     for (t, x, y) in events:
         own_ms[t[0]] = own_ms.get(t[0], 0.0) + x.elapsed_time(y) / prof_steps
     own_ms = {k: round(v, 3) for k, v in sorted(own_ms.items(), key=lambda kv: -kv[1])}
-    if rank == 0 and os.path.isdir(os.path.join(ROOT, "gpurun_out")):  # per-shape table for tuning (not part of the line)
-        detail = {}
-        for (t, x, y) in events:
-            d = detail.setdefault(" ".join(str(v) for v in t), [0.0, 0])
-            d[0] += x.elapsed_time(y) / prof_steps
-            d[1] += 1.0 / prof_steps
-        json.dump({k: [round(v[0], 4), round(v[1], 2)] for k, v in sorted(detail.items(), key=lambda kv: -kv[1][0])},
-                  open(os.path.join(ROOT, "gpurun_out", "own_kernel_detail.json"), "w"), indent=0)
     # tensor-core side of the step: all GEMM launches (2*M*N*K flops each) and the ViT attention launches
-    # (4*seq*heads*n*n*64 flops) against the measured cuBLAS bf16 peak of this pool
+    # (4*seq*heads*n*n*64 flops) against the dense 16-bit tensor peak
     # GEMMs with at least 2048 rows: their device time dwarfs the host's launch gap, which an event pair in this eager pass cannot
     # separate from a 7 us kernel (the 900-row decoder GEMMs: latency-bound, < 3 % of the step's GEMM flops, left out and said so)
     gemm_flops_all = sum(2.0 * t[1] * t[2] * t[3] for (t, x, y) in events if t[0] == "gemm_tn") / prof_steps
@@ -557,7 +598,7 @@ def model_bench(args, rank, local_rank, world):
         achieved = nbytes / (enc_ms * 1e-3) / 1e9
         lsu_bytes = B * Q * H * L * P * 4 * D * e
         props = torch.cuda.get_device_properties(dev)
-        lsu_peak = props.multi_processor_count * 128 * float((clocks or {}).get("sm_max_mhz") or 1965.0) * 1e6 / 1e9
+        lsu_peak = props.multi_processor_count * 128 * float((clocks or {}).get("sm_max_mhz") or 1980.0) * 1e6 / 1e9
         traffic = None
         tp = os.path.join(ROOT, "profiles", "traffic.json")
         if os.path.exists(tp):
@@ -600,20 +641,20 @@ def model_bench(args, rank, local_rank, world):
         pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(pk):
             tpeak = float(json.load(open(pk)).get("bf16_tflops", 0) or 0) or None
-        tpeak_src = "measured (MEASURED_PEAKS.json bf16_tflops, burst)" if tpeak else "fallback (B200_PROFILING.md 1590 TFLOP/s)"
-        tpeak = tpeak or 1590.0
+        tpeak_src = "measured (MEASURED_PEAKS.json bf16_tflops, burst)" if tpeak else "fallback (NVIDIA H100 SXM data sheet, dense BF16 989 TFLOP/s)"
+        tpeak = tpeak or 989.0
         if gemm_ms > 0:
             a = gemm_flops / (gemm_ms * 1e-3) / 1e12
             line["roofline_gemm"] = {"bound": "tensor", "achieved": a, "peak": tpeak, "unit": "TFLOP/s", "frac": a / tpeak,
                                      "peak_source": tpeak_src,
-                                     "kernel": "gemm_tc_kernel / gemm_pair_kernel (every linear layer with >= 2048 rows: "
+                                     "kernel": "gemm_tc_kernel (every linear layer with >= 2048 rows: "
                                                f"{100.0 * gemm_flops / max(gemm_flops_all, 1.0):.1f} % of the step's GEMM flops)",
                                      "flops_per_step": gemm_flops, "ms_per_step": gemm_ms,
                                      "timing": "event pairs around each launch in eager repeats of the step, enqueued behind a GPU-side delay so the pairs see device time only"}
         if attn_ms > 0:
             a = attn_flops / (attn_ms * 1e-3) / 1e12
             line["roofline_attention"] = {"bound": "tensor", "achieved": a, "peak": tpeak, "unit": "TFLOP/s", "frac": a / tpeak,
-                                          "peak_source": tpeak_src, "kernel": "attn_fwd_kernel (24 ViT blocks)",
+                                          "peak_source": tpeak_src, "kernel": "attn_kernel (24 ViT blocks)",
                                           "flops_per_step": attn_flops, "ms_per_step": attn_ms}
         if world == 1 and not args.no_microbench:
             line["msda_microbench"] = msda_microbench(dev, quick=args.quick_microbench)
@@ -641,6 +682,8 @@ def main():
     ap.add_argument("--no-microbench", action="store_true", help="skip the config-5 ms_deform_attn microbench keys")
     ap.add_argument("--quick-microbench", action="store_true")
     ap.add_argument("--no-graphs", action="store_true", help="disable CUDA-graph capture of the static stages")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32 / float64, at most 64 MB in all)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -651,7 +694,7 @@ def main():
     tdt = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}[args.dtype]
     esize = 4 if args.dtype == "fp32" else 2
     config = {"workload": "ms_deform_attn_forward APE-L_D 1024^2 encoder shape (B=1/GPU, Q=S=87296, L=5, H=8, D=32, P=4)",
-              "loc": "uniform(0,1) seed 3 (SURVEY 8d)", "l2": "4 rotating input sets (1.4 GB fp32) > 126 MB L2",
+              "loc": "uniform(0,1) seed 3 (SURVEY 8d)", "l2": "4 rotating input sets (1.4 GB fp32) > 50 MB L2",
               "parallelism": f"dp{args.gpus} (one image per GPU, no data-path collective)"}
 
     if args.workload in ("ape_l_d", "ape_l_d_masks"):
@@ -720,10 +763,12 @@ def main():
     t_start.record()
     for i in range(args.steps):
         evs[i][0].record()
-        step(i)
+        out = step(i)
         evs[i][1].record()
     t_end.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"msda_out": out})
     launches = ape_b200._lib.launch_count() - n0
     total_ms = t_start.elapsed_time(t_end)
     kern_ms = sum(a.elapsed_time(b) for a, b in evs) / args.steps

@@ -1,5 +1,5 @@
 /*
- * ape_b200.h — C-ABI of libape_b200.so, the sm_100a (B200) kernels behind APE's
+ * ape_b200.h — C-ABI of libape_b200.so, the sm_90a (H100) kernels behind APE's
  * detection forward pass.
  *
  * Every entry point is `extern "C"`, takes plain device pointers and sizes, a
@@ -136,17 +136,17 @@ int ape_msda_bwd(const void *value, const int64_t *spatial_shapes, const int64_t
                  int S, int H, int D, int L, int Q, int P, int dtype, void *stream);
 
 /*
- * Tensor-core linear layer: C[M,N] = act(A[M,K] * W[N,K]^T + bias) (+ residual), tcgen05 / TMA / TMEM.
+ * Tensor-core linear layer: C[M,N] = act(A[M,K] * W[N,K]^T + bias) (+ residual), TMA + wgmma.
  * Replaces the nn.Linear (cuBLAS) calls of the detection path (vit_eva_clip.py:225-232,266-267,125-132;
  * deformable_transformer_vl.py:36-54; multi_scale_deform_attn.py:278-295,353; vision_language_align.py:36-48).
  *
  * A [M,K] and W [N,K] (nn.Linear weight layout) are fp16 or bf16 (in_dtype), K contiguous, row pitches
- * lda / ldw in elements (16-byte aligned rows).  fp32 accumulation in tensor memory.
+ * lda / ldw in elements (16-byte aligned rows).  fp32 accumulation in registers (wgmma).
  * bias: fp32 [N] or NULL.  residual: [M,N] of out_dtype with pitch ldr, or NULL.
  * act: 0 none, 1 ReLU, 2 GELU(erf), 3 SwiGLU over interleaved (gate, up) column pairs -> C is [M, N/2],
  *      4 clamp to +-50000 (VisionLanguageAlign, vision_language_align.py:49-51).
- * out_dtype: APE_DTYPE_* of C (pitch ldc elements).  tile_n: 0 = auto, or 128 / 256 (| 0x1000 single CTA, 0x4000 cluster of
- * two CTAs sharing the weight tile by TMA multicast, 0x2000 CTA-pair MMA; 0x4000 forces the multicast cluster).
+ * out_dtype: APE_DTYPE_* of C (pitch ldc elements).  tile_n: 0 = auto, or 128 / 256 (| 0x1000 forces a single CTA, | 0x4000 a
+ * cluster of two CTAs sharing the weight tile by TMA multicast; without either the cluster is used for K >= 2048).
  */
 int ape_gemm_tn(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc, const float *bias,
                 const void *residual, int64_t ldr, int M, int N, int K, int in_dtype, int out_dtype, int act,
@@ -173,7 +173,7 @@ int ape_gemm_tn_fused(const void *A, int64_t lda, const void *W, int64_t ldw, vo
                       float ln_eps, float *stats_out, int stats_nslab, void *stream);
 
 /*
- * 3x3 convolution (stride 1, zero padding 1) over NHWC activations as an implicit GEMM on the tcgen05 kernel: the 3x3
+ * 3x3 convolution (stride 1, zero padding 1) over NHWC activations as an implicit GEMM on the wgmma kernel: the 3x3
  * convolutions of SimpleFeaturePyramid (vit_eva_clip.py:804-847) and of the mask head (deformable_detr_segm_vl.py:741-747).
  * x [B,H,W,Cin], w [Cout,3,3,Cin] (= the Conv2d weight permuted (0,2,3,1)), y [B,H,W,Cout], bias fp32 [Cout] or NULL;
  * fp16 / bf16, fp32 accumulation; act 0 / 1 (ReLU) / 2 (GELU).  Cin % 64 == 0; the image must be a whole number of
@@ -194,7 +194,7 @@ int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, voi
 
 /*
  * Development aid (no reference counterpart): when device_buffer is not NULL, every CTA of the following ape_gemm_tn*
- * launches (single-CTA / multicast variants) writes 8 clock64() stamps to device_buffer[8 * blockIdx.x ..]:
+ * launches writes 8 clock64() stamps to device_buffer[8 * blockIdx.x ..]:
  * entry, set-up done, first operands landed, last MMA issued, first / last accumulator complete, epilogue drained, exit.
  * NULL switches it off.  Process-wide, not for concurrent use.
  */
@@ -245,7 +245,7 @@ int ape_rope_qk(void *qkv, int64_t ld, const float *cos_table, const float *sin_
 /*
  * Softmax attention core of the ViT blocks (Attention.forward, ape/modeling/backbone/vit_eva_clip.py:218-319, the
  * part xformers / F.scaled_dot_product_attention computes there): out = softmax(q k^T * scale) v per (sequence, head),
- * flash-attention style on tcgen05 tensor cores.  qkv [num_seq * n, >= 3*heads*64] (pitch ld elements): columns
+ * flash-attention style on the wgmma tensor cores.  qkv [num_seq * n, >= 3*heads*64] (pitch ld elements): columns
  * [0,C) = q, [C,2C) = k, [2C,3C) = v with C = heads*64, head h at columns h*64 (the layout the fused qkv GEMM writes,
  * RoPE already applied); sequence s owns rows [s*n, (s+1)*n).  out [num_seq * n, >= C] (pitch ldo).  fp16 or bf16,
  * head_dim 64, n a multiple of 128; fp32 softmax statistics and accumulation.
@@ -264,8 +264,8 @@ int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t ldo, int num
                     int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
                     void *stream);
 
-/* Kernel structure behind ape_attn_fwd*: 0 = P through shared memory (4 CTAs / SM), 1 = P in tensor memory as the A operand of
- * tcgen05.mma, double-buffered scores (2 CTAs / SM).  set >= 0 selects it for the process; returns the value in force
+/* Kernel structure behind ape_attn_fwd*: 0 = P written to shared memory and read from there by the P.V wgmma, 1 = P kept in
+ * registers as the A operand of the P.V wgmma.  set >= 0 selects it for the process; returns the value in force
  * (initially APE_ATTN_VARIANT or the built-in default). */
 int ape_attn_variant(int set);
 

@@ -7,7 +7,7 @@
  * source is copied into this repository).  Built by oracle/Makefile into
  * oracle/_ref/libref_msda.so (git-ignored; travels to the GPU box) and used there as
  *   (1) a second oracle for the CUDA parity tests (tests/test_msda_gpu.py), and
- *   (2) the "kernel to beat": the reference's 2020-era SIMT kernel recompiled for sm_100a,
+ *   (2) the "kernel to beat": the reference's 2020-era SIMT kernel recompiled for sm_90a,
  *       timed beside ours by bench.py on identical tensors.
  * The launcher plays the role of ms_deform_attn_cuda_forward
  * (ape/layers/csrc/MsDeformAttn/ms_deform_attn_cuda.cu:21-81) minus the ATen plumbing:

@@ -1,4 +1,4 @@
-"""Launches ONE kernel family a few times at the APE-L_D model shapes, for `ncu --set full` captures (profiles/):
+"""Launches ONE kernel family a few times at the APE-L_D model shapes, for `ncu --set full` captures:
 
     ncu --set full --import-source on -k regex:attn_fwd -s 1 -c 1 -o gpurun_out/r02_attn_window python tests/ncu_targets.py attn_window
 

@@ -24,7 +24,7 @@ SHAPES = [  # (M, N, K, act, count per step, what)
     (65536, 256, 256, None, 2, "p2 1x1"),
     (900, 256, 256, None, 31, "dec small"),
 ]
-VARIANTS = {"mc256": 256, "pair256": 256 | 0x2000, "mc128": 128, "single256": 256 | 0x1000}
+VARIANTS = {"mc256": 256 | 0x4000, "mc128": 128 | 0x4000, "single256": 256 | 0x1000, "single128": 128 | 0x1000}
 
 
 def main():

@@ -6,7 +6,7 @@ the number) and dissected by the kernel's own clock64 stamps (ape_gemm_set_trace
 
 Per shape and variant: us per launch (graph of 20 launches, warm operands; `cold` = 8 rotating weight / activation sets larger
 than L2 together), TFLOP/s, and medians over CTAs of the phases in SM cycles:
-  setup   entry -> barriers / tensor memory ready     load   -> first operands landed
+  setup   entry -> barriers ready                        load   -> first operands landed
   issue   first operands -> last MMA issued           acc1   first operands -> first accumulator complete
   tail    last accumulator complete -> stores drained total  entry -> exit"""
 import json
@@ -33,7 +33,7 @@ SHAPES = [  # (what, M, N, K, act, epilogue, count per step)
     ("dec ffn1", 900, 2048, 256, "relu", "f16", 6),
     ("dec ffn2", 900, 256, 2048, None, "f32+res", 6),
 ]
-VARIANTS = {"single": 0x1000, "mc2": 0x4000, "pair": 0x2000}
+VARIANTS = {"single": 0x1000, "mc2": 0x4000}
 if os.environ.get("PERF_GEMM_VARIANTS"):
     VARIANTS = {k: v for k, v in VARIANTS.items() if k in os.environ["PERF_GEMM_VARIANTS"].split(",")}
 
@@ -156,7 +156,7 @@ def sustained(sets, act, tile, seconds=1.5):
 
 
 def phases(sets, act, tile):
-    buf = torch.zeros(148 * 8 * 2, dtype=torch.int64, device=DEV)
+    buf = torch.zeros(torch.cuda.get_device_properties(DEV).multi_processor_count * 8 * 2, dtype=torch.int64, device=DEV)
     _lib.lib.ape_gemm_set_trace(buf.data_ptr())
     try:
         run(sets, act, tile, 0)
@@ -189,8 +189,7 @@ def main():
                 us = graph_time(cold, act, tile)
                 rec.update(us_cold=round(us, 2), tflops_cold=round(flops / us / 1e6, 1), cold_sets=len(cold),
                            ms_per_step_cold=round(us * cnt / 1e3, 3))
-                if name != "pair":
-                    rec["cycles"] = phases(warm, act, tile)
+                rec["cycles"] = phases(warm, act, tile)
                 if name == "single" and M >= 4096:
                     us, ck = sustained(warm, act, tile)
                     rec.update(us_sustained=round(us, 2), tflops_sustained=round(flops / us / 1e6, 1), clocks_sustained=ck)

@@ -1,9 +1,9 @@
-"""GPU microbench sweep for ms_deform_attn forward (BASELINE.json config 5) — run on the B200 box:
+"""GPU microbench sweep for ms_deform_attn forward (BASELINE.json config 5) — run on the GPU:
 
     python tests/perf_msda_sweep.py [--quick] > gpurun_out/msda_sweep.jsonl
 
 For every (shape, dtype, loc distribution) it times each kernel variant of libape_b200 and the
-reference's own CUDA kernel (oracle/_ref, recompiled for sm_100a) on identical tensors, with an
+reference's own CUDA kernel (oracle/_ref, recompiled for sm_90a) on identical tensors, with an
 L2 flush before every timed launch, and prints one JSON line per measurement.
 Lives under tests/ because it uses the oracle (reference kernel) as comparison."""
 import argparse

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 flash-attention kernel (ape_attn_fwd) against a plain PyTorch fp32 reference of the same op
+"""GPU: the wgmma flash-attention kernel (ape_attn_fwd) against a plain PyTorch fp32 reference of the same op
 (softmax(q k^T * scale) v per head) on the same 16-bit inputs."""
 import pytest
 import torch
@@ -9,7 +9,9 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module", params=[0, 1], ids=["smemP", "tmemP"])
 def ops(request):
-    """Every test of this file runs against both structures of the ViT attention kernel (ape_attn_variant)."""
+    """Every test of this file runs against both structures of the ViT attention kernel (ape_attn_variant): P read by the
+    P.V MMA from shared memory ("smemP") or kept on-chip in registers as its A operand (id "tmemP", kept from earlier
+    hardware where it lived in tensor memory)."""
     import ape_b200
 
     prev = ape_b200._lib.lib.ape_attn_variant(-1)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMA/TMEM linear layer (ape_gemm_tn) against a plain PyTorch fp32 reference of
+"""GPU: the TMA/wgmma linear layer (ape_gemm_tn) against a plain PyTorch fp32 reference of
 the same op on the same (16-bit rounded) operands.  Tolerance: fp32 accumulation over K terms of
 16-bit products -> relative 2e-3 on fp16/bf16 outputs (output rounding), 1e-4 on fp32 outputs."""
 import pytest
@@ -87,7 +87,7 @@ def test_vit_swiglu_shape_16bit_out(ops, dtype):
     assert ((pad == 9.0) | (pad == 0.0)).all()
 
 
-@pytest.mark.parametrize("tile", [128, 256, 128 | 0x1000, 256 | 0x1000, 128 | 0x2000, 256 | 0x2000, 128 | 0x4000, 256 | 0x4000])  # default: per-shape policy; 0x1000: single CTA; 0x2000: CTA-pair MMA; 0x4000: cluster of 2 (TMA multicast)
+@pytest.mark.parametrize("tile", [128, 256, 128 | 0x1000, 256 | 0x1000, 128 | 0x4000, 256 | 0x4000])  # default: per-shape policy; 0x1000: single CTA; 0x4000: cluster of 2 (TMA multicast)
 def test_tma_store_epilogue_edges(ops, tile):
     # M and N both ragged, bias + relu + residual, 16-bit output with an aligned pitch
     M, N, K = 777, 840, 192
@@ -113,12 +113,13 @@ def test_cluster_pairs_with_odd_row_block_counts(ops, M, tile):
     torch.testing.assert_close(y, ref_linear(x, w, b), rtol=2e-4, atol=2e-4)
     y1 = ops.linear_tc(x, w, b, out_dtype=torch.float32, tile_n=tile | 0x1000)
     assert torch.equal(y, y1)  # same accumulation order with and without the cluster
-    for flag in (0x2000, 0x4000):  # CTA-pair MMA (cta_group::2) and the multicast cluster of 2
-        assert torch.equal(y, ops.linear_tc(x, w, b, out_dtype=torch.float32, tile_n=tile | flag))
+    assert torch.equal(y, ops.linear_tc(x, w, b, out_dtype=torch.float32, tile_n=tile | 0x4000))  # the multicast cluster of 2
+    with pytest.raises(RuntimeError):  # the CTA-pair MMA flag names an instruction sm_90a lacks: rejected, not ignored
+        ops.linear_tc(x, w, b, out_dtype=torch.float32, tile_n=tile | 0x2000)
 
 
 def test_many_tiles_per_cta_ring_wraparound(ops):
-    # 87 296 encoder tokens x FFN: 682 x 8 tiles over 148 persistent CTAs, K = 2048 (32 k-blocks)
+    # 87 296 encoder tokens x FFN: 682 x 8 tiles over 132 persistent CTAs, K = 2048 (32 k-blocks)
     M, N, K = 87296, 256, 2048
     x = rnd(M, K, dtype=torch.float16, seed=31, scale=0.5)
     w = rnd(N, K, dtype=torch.float16, seed=32, scale=K ** -0.5)
@@ -245,7 +246,7 @@ def test_conv3x3_implicit_gemm_matches_conv2d(ops, dtype, B, H, W, Cin, Cout):
 
 
 @pytest.mark.parametrize("M,N,K,act,out32", [
-    (19100, 256, 256, None, False),     # one column block, 150 row tiles on 148 CTAs (second round for two of them)
+    (19100, 256, 256, None, False),     # 150 row tiles: more tiles than the 132 persistent CTAs
     (40000, 256, 192, "relu", False),   # 3 k blocks, several tiles per CTA, ragged last tile
     (25000, 200, 256, None, True),      # N < tile, fp32 output + residual
     (19000, 2048, 256, "relu", False),  # 149 row blocks x 8 column blocks (encoder FFN1 geometry)

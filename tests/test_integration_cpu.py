@@ -11,6 +11,7 @@
 import ast
 import importlib.util
 import inspect
+import json
 import os
 import re
 import sys
@@ -125,9 +126,10 @@ def _reference_model_tree():
     return tree
 
 
-@needs_ref
 def test_integration_target_overrides_name_real_config_nodes(built):
-    tree = _reference_model_tree()
+    """The overrides name real nodes of the reference's model config tree (_reference_model_tree over the reference's own
+    config files), recorded in tests/golden/ref_model_config_tree.json by tests/golden/gen_cpu_golden.py."""
+    tree = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_model_config_tree.json")))
     text = open(os.path.join(ROOT, "INTEGRATION.md")).read()
     overrides = re.findall(r"(model(?:\.\w+)+)\._target_=(ape_b200(?:\.\w+)+)", text)
     assert len(overrides) >= 9

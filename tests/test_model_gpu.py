@@ -165,7 +165,7 @@ def test_mini_matches_oracle_port(mini):
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float16, 2e-2), (torch.bfloat16, 1e-1)])
 def test_vit_engine_path_matches_fp32_library_path(mini, dtype, tol):
-    """The tensor-core ViT path (tcgen05 GEMMs + LayerNorm/RoPE kernels, window-major token order)
+    """The tensor-core ViT path (wgmma GEMMs + LayerNorm/RoPE kernels, window-major token order)
     against the fp32 path of the same module (which is pinned to the reference goldens above)."""
     model, _ = mini
     net = model.backbone.net
@@ -251,7 +251,7 @@ def test_ape_l_d_1024_matches_oracle_port_stagewise():
     for k in ("p2", "p4", "p6"):
         torch.testing.assert_close(lo["features"][k].cpu(), taps[f"backbone.{k}"], rtol=2e-3, atol=2e-3)
     # 6 encoder layers after a 24-block ViT, fp32 on both sides with different reduction orders: 241 of 22 M
-    # elements exceeded 2e-3 (max 4.4e-3) on B200, so the bound here is 1e-2 absolute on O(1) values
+    # elements exceed 2e-3, so the bound here is 1e-2 absolute on O(1) values
     torch.testing.assert_close(lo["memory"].cpu(), taps["memory"], rtol=1e-2, atol=1e-2)
     sel, want = model.transformer.last_topk_proposals.cpu(), taps["topk_proposals"]
     # Stage-wise parity of the selection itself (bit-exact requirement): the engine's top-k / NMS / quota code on
@@ -299,7 +299,7 @@ def test_ape_ti_1024_matches_reference_golden():
     for k in ("p2", "p4", "p6"):
         torch.testing.assert_close(lo["features"][k][:, ::16, ::4, ::4].cpu(), g[f"backbone.{k}"], rtol=2e-3, atol=2e-3)
     # fp32 on both sides, different reduction orders over 6 encoder layers (cf. the APE-L_D full-size test)
-    torch.testing.assert_close(lo["memory"][:, ::128].cpu(), g["memory"], rtol=1e-2, atol=1e-2)
+    torch.testing.assert_close(lo["memory"][:, ::128, ::4].cpu(), g["memory"], rtol=1e-2, atol=1e-2)
     sel, want = model.transformer.last_topk_proposals.cpu()[0].tolist(), g["topk_proposals"][0].tolist()
     frac = len(set(sel) & set(want)) / len(want)
     print(f"APE-Ti proposal set agreement with the reference: {frac:.4f}")

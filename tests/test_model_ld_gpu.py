@@ -4,7 +4,7 @@ layers, 900 queries), one 1024 x 768 image padded to 1024^2, 1203-name vocabular
 `tests/golden/model_ld_1024.npz` was recorded by running the reference's own files on the CPU (fp32, pytorch_attn=True;
 tests/golden/gen_model_golden.py ld).  The engine is compared with it stage by stage in three numeric modes:
   float32           library GEMMs + the repo's MSDA / NMS kernels (strict mode)
-  float16 + graphs  the SHIPPED path of bench.py: tcgen05 GEMMs / attention, fused MSDA, one CUDA graph
+  float16 + graphs  the SHIPPED path of bench.py: wgmma GEMMs / attention, fused MSDA, one CUDA graph
   bfloat16 + graphs same kernels, bf16 operands
 Each stage prints max |err|, the RMS of the golden tensor and the max / median error relative to that RMS."""
 import numpy as np
@@ -19,10 +19,7 @@ pytestmark = [pytest.mark.gpu, pytest.mark.slow]
 DEV = "cuda:0"
 N_TEXT = 1203
 
-# median|err| / rms(golden) allowed per stage and mode; the maximum may be 5x that.  Measured on B200 (round 2, DESIGN.md 3.1):
-#   float32  backbone 1.6e-6 (max 1.1e-5), memory 2.4e-6 (max 2.1e-5), logits max 2.2e-3, boxes max 2.7e-3
-#   float16  backbone 9.5e-4 (max 6.4e-3), memory 1.0e-3 (max 9.0e-3), logits median 2.5e-3 max 4.7e-2
-#   bfloat16 backbone 7.6e-3 (max 5.5e-2), memory 8.4e-3 (max 7.0e-2), logits median 6.7e-3 max 6.2e-2, boxes max 1.5e-1
+# median|err| / rms(golden) allowed per stage and mode; the maximum may be 5x that.
 # The decoder amplifies encoder-output differences about 100x with these untrained weights (fp32 GPU vs fp32 CPU: memory
 # 2e-5 -> logits 2e-3), so north_star's 1e-3 on the logits is met by the median of the fp32 mode only; see DESIGN.md.
 TOL = {
@@ -88,15 +85,15 @@ def test_ld_1024_stagewise_vs_reference_golden(setup, mode):
     print(f"\n== APE-L_D 1024^2 / 1203 names, engine mode {mode}" + (" + CUDA graph replay" if mode != "float32" else ""))
     out, lo = run(model, mode)
     for k in ("p2", "p3", "p4", "p5", "p6"):
-        r = err(f"backbone.{k}", lo["features"][k][:, ::16, ::4, ::4], g[f"backbone.{k}"], report)
+        r = err(f"backbone.{k}", lo["features"][k][:, ::16, ::8, ::8], g[f"backbone.{k}"], report)
         assert r["max_over_rms"] < tol["backbone"] * 5 and r["median_over_rms"] < tol["backbone"]
     for i in range(5):
-        r = err(f"neck.{i}", lo["neck"][i][:, ::16, ::4, ::4], g[f"neck.{i}"], report)
+        r = err(f"neck.{i}", lo["neck"][i][:, ::16, ::8, ::8], g[f"neck.{i}"], report)
         assert r["max_over_rms"] < tol["neck"] * 5 and r["median_over_rms"] < tol["neck"]
     for k, v in sorted(lo["taps"].items()):  # per-layer fusion / encoder-layer outputs (engine schedule exposes them as taps)
-        r = err(k, v[:, ::512], g[k], report)
+        r = err(k, v[:, ::2048, ::4], g[k], report)
         assert r["max_over_rms"] < tol["encoder"] * 5 and r["median_over_rms"] < tol["encoder"]
-    r = err("memory", lo["memory"][:, ::128], g["memory"], report)
+    r = err("memory", lo["memory"][:, ::512, ::4], g["memory"], report)
     assert r["max_over_rms"] < tol["memory"] * 5 and r["median_over_rms"] < tol["memory"]
     # two-stage selection: proposal indices.  Bit-exactness of the selection CODE on identical inputs is asserted in
     # tests/test_model_gpu.py (oracle inputs); end to end the 16-bit encoder output perturbs near-ties of top-k / NMS(0.9)
@@ -108,8 +105,8 @@ def test_ld_1024_stagewise_vs_reference_golden(setup, mode):
     assert frac > (0.99 if mode == "float32" else 0.95 if mode == "float16" else 0.9)
     ia = torch.tensor([sel.index(i) for i in common])
     ib = torch.tensor([want.index(i) for i in common])
-    r = err("pred_logits (common q)", lo["pred_logits"][0][ia][:, ::8], g["pred_logits"][0][ib], report)
-    logit_rel = ((lo["pred_logits"][0][ia][:, ::8].float().cpu() - g["pred_logits"][0][ib]).abs() / g["pred_logits"][0][ib].abs()).max().item()
+    r = err("pred_logits (common q)", lo["pred_logits"][0][ia][:, ::32], g["pred_logits"][0][ib], report)
+    logit_rel = ((lo["pred_logits"][0][ia][:, ::32].float().cpu() - g["pred_logits"][0][ib]).abs() / g["pred_logits"][0][ib].abs()).max().item()
     print(f"  pred_logits max RELATIVE error on commonly selected queries: {logit_rel:.3e} (north_star: 1e-3)")
     assert r["max_over_rms"] < tol["logits"]
     r = err("pred_boxes (common q)", lo["pred_boxes"][0][ia], g["pred_boxes"][0][ib], report)

@@ -1,7 +1,6 @@
 """GPU parity tests for ms_deform_attn_forward through the C-ABI (ape_b200 -> libape_b200.so),
-against (1) the C oracle, (2) golden vectors generated from the reference, (3) the reference's
-own CUDA kernel compiled for sm_100a (oracle/_ref), plus size-independent properties at the
-full APE-L_D shapes."""
+against (1) the C oracle, (2) golden vectors generated from the reference, (3) stored outputs of the
+reference's own CUDA kernel, plus size-independent properties at the full APE-L_D shapes."""
 import glob
 import os
 
@@ -118,28 +117,28 @@ def test_exact_corner_and_edge_locations(ape):
     torch.testing.assert_close(got.cpu().view(H_ * W_, 8), v.view(H_ * W_, 8), rtol=0, atol=1e-4)
 
 
-@pytest.mark.skipif(not O.have_ref_cuda(), reason="oracle/_ref not built")
+# The reference's own CUDA kernel (oracle/_ref, built from the reference checkout) ran on these seeded inputs once; its outputs,
+# sampled along the query axis, are stored as tests/golden/refcuda_msda_*.npz (tests/golden/gen_msda_ref_cuda_golden.py).
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
 def test_against_reference_cuda_kernel_decoder_shape(ape, dtype):
     ins = to_dev(O.make_inputs(2, 900, 8, 32, L5_1024, 4, seed=3, border=True), dtype)
-    ref = O.ref_cuda(*ins)
-    got = run(ape, *ins)
+    ref = load_golden(f"refcuda_msda_decoder_{'f32' if dtype == torch.float32 else 'f16'}.npz")["out"].to(DEV)
+    got = run(ape, *ins)[:, ::4]
     if dtype == torch.float32:
         torch.testing.assert_close(got, ref, rtol=1e-5, atol=5e-6)
     else:
         # the reference accumulates in half (…cuh:270); we accumulate in fp32
-        torch.testing.assert_close(got.float(), ref.float(), rtol=2e-2, atol=2e-2)
+        torch.testing.assert_close(got.float(), ref, rtol=2e-2, atol=2e-2)
 
 
-@pytest.mark.skipif(not O.have_ref_cuda(), reason="oracle/_ref not built")
 def test_against_reference_cuda_kernel_encoder_shape_full_size(ape):
     """BASELINE.json config 2 shape: Q = S = 87 296, 5 levels (too slow for the CPU oracle; the
     reference's own kernel is the checker)."""
     S = sum(h * w for h, w in L5_1024)
     ins = to_dev(O.make_inputs(1, S, 8, 32, L5_1024, 4, seed=3, border=True))
-    ref = O.ref_cuda(*ins)
+    ref = load_golden("refcuda_msda_encoder_f32.npz")["out"].to(DEV)
     for variant in (-1, 1, 8):
-        got = run(ape, *ins, variant=variant)
+        got = run(ape, *ins, variant=variant)[:, ::256]
         torch.testing.assert_close(got, ref, rtol=1e-5, atol=5e-6)
 
 

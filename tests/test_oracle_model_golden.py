@@ -101,7 +101,7 @@ def test_port_matches_reference_golden_ape_ti():
     tol = dict(rtol=1e-5, atol=1e-5)  # measured: 0.0 through the encoder (same ATen kernels in the same order)
     for k in ("p2", "p3", "p4", "p5", "p6"):
         torch.testing.assert_close(taps[f"backbone.{k}"][:, ::16, ::4, ::4], g[f"backbone.{k}"], **tol)
-    torch.testing.assert_close(taps["memory"][:, ::128], g["memory"], **tol)
+    torch.testing.assert_close(taps["memory"][:, ::128, ::4], g["memory"], **tol)
     torch.testing.assert_close(taps["enc_outputs_class"][:, ::16], g["enc_outputs_class"], **tol)
     # selected proposals: exact on the valid ones (ties among zero-score padding entries of the 16x16 level are
     # implementation-defined in the reference's torch.topk, see test_port_matches_reference_golden)

@@ -1,4 +1,4 @@
-"""GPU: the text tower's engine path (tcgen05 GEMMs, causal flash attention over packed 77-token prompts, LayerNorm kernels,
+"""GPU: the text tower's engine path (wgmma GEMMs, causal flash attention over packed 77-token prompts, LayerNorm kernels,
 fp32 residual stream) against the golden recorded from the reference's TextTransformer and, at EVA02-CLIP-bigE geometry
 (width 1280, 20 heads x 64), against the literal fp32 path of the same module."""
 import pytest

@@ -1,6 +1,6 @@
 """CPU: the streaming evaluation of BiMultiHeadAttention (two attention calls, no S x N_t score tensor; used above
 `stream_threshold_bytes`, i.e. for phrase prompts at scale) against the literal op sequence of the reference
-(ape/layers/fuse_helper.py:67-166) as restated in the same module, and against the reference module itself."""
+(ape/layers/fuse_helper.py:67-166) as restated in the same module, and against outputs recorded from the reference module itself."""
 import pytest
 import torch
 
@@ -37,27 +37,30 @@ def test_streaming_is_skipped_when_the_clamps_could_bind():
     assert torch.equal(v1, v0) and torch.equal(l1, l0)
 
 
-def test_literal_path_equals_reference_module():
-    """The restated literal path against the reference's own BiAttentionBlock (run from /root/reference when present)."""
-    from oracle import refshim
-
-    if not refshim.available():
-        pytest.skip("reference sources not present (GPU box)")
-    refshim.install()
-    fh = refshim.load("ape.layers.fuse_helper")
+def make_block_and_inputs():
+    """Seeded weights and inputs of test_literal_path_equals_reference_module (also used by tests/golden/gen_cpu_golden.py)."""
     torch.manual_seed(2)
-    ref = fh.BiAttentionBlock(v_dim=256, l_dim=128, embed_dim=512, num_heads=8, dropout=0.0, drop_path=0.0, init_values=1 / 6,
-                              stable_softmax_2d=True, clamp_min_for_underflow=True, clamp_max_for_overflow=True).eval()
     mine = BiAttentionBlock(256, 128, 512, 8, init_values=1 / 6, stable_softmax_2d=True).eval()
-    mine.load_state_dict(ref.state_dict())
-    v, l = torch.randn(2, 400, 256), torch.randn(2, 9, 128)
     with torch.no_grad():
-        rv, rl = ref(v, l, attention_mask_v=None, attention_mask_l=None)
+        for p in mine.parameters():
+            if p.dim() == 1:
+                p.add_(torch.randn_like(p) * 0.05)
+    return mine, torch.randn(2, 100, 256), torch.randn(2, 9, 128)
+
+
+def test_literal_path_equals_reference_module():
+    """The restated literal path against the reference's own BiAttentionBlock (fuse_helper.py) on the same weights and
+    inputs, recorded in tests/golden/vlf_block_ref.npz by tests/golden/gen_cpu_golden.py."""
+    from conftest import load_golden
+
+    g = load_golden("vlf_block_ref.npz")
+    mine, v, l = make_block_and_inputs()
+    with torch.no_grad():
         mine.attn.stream_threshold_bytes = 1 << 60
         mv, ml = mine(v, l)
         mine.attn.stream_threshold_bytes = 0
         sv, sl = mine(v, l)
-    torch.testing.assert_close(mv, rv, rtol=1e-6, atol=1e-6)
-    torch.testing.assert_close(ml, rl, rtol=1e-6, atol=1e-6)
-    torch.testing.assert_close(sv, rv, rtol=1e-5, atol=1e-5)
-    torch.testing.assert_close(sl, rl, rtol=1e-5, atol=1e-5)
+    torch.testing.assert_close(mv, g["v"], rtol=1e-6, atol=1e-6)
+    torch.testing.assert_close(ml, g["l"], rtol=1e-6, atol=1e-6)
+    torch.testing.assert_close(sv, g["v"], rtol=1e-5, atol=1e-5)
+    torch.testing.assert_close(sl, g["l"], rtol=1e-5, atol=1e-5)

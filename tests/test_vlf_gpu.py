@@ -47,7 +47,7 @@ def test_vlf_pool_extreme_scores_follow_reference_clamps():
 @pytest.mark.parametrize("S,N,dtype,tol", [(500, 3, torch.float16, 4e-3), (2048, 256, torch.float16, 4e-3),
                                            (5000, 1203, torch.float16, 4e-3), (1000, 77, torch.bfloat16, 3e-2)])
 def test_multi_token_engine_path_matches_literal_attention(S, N, dtype, tol):
-    """Phrase / text prompts (N_t > 1): BiAttentionBlock's engine path (LayerNorm kernel, tcgen05 GEMMs, two
+    """Phrase / text prompts (N_t > 1): BiAttentionBlock's engine path (LayerNorm kernel, wgmma GEMMs, two
     ape_attn_cross_fwd passes over 256-channel heads) against the literal op sequence of fuse_helper.py:67-166 in fp32
     (score matrix, global-max shift, clamps, two softmaxes) at N_t = 3, 77, 256 and 1203."""
     from ape_b200.layers.vision_language_fusion import BiAttentionBlock
