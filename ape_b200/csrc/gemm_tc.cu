@@ -30,6 +30,17 @@ constexpr int kConsumerWarps = 8;
 constexpr int kThreads = 32 * kConsumerWarps + 32;
 
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SWIGLU = 3, ACT_CLAMP = 4 };
+enum Res { RES_NONE = 0, RES_F32 = 1, RES_16 = 2 };  // RES_16: a residual of the operand type
+
+// The epilogue of a kernel instantiation, fixed at compile time: output fp32 (or the 16-bit operand type), activation,
+// residual, LayerNorm fold, rotary embedding, SwiGLU row statistics.  A runtime-generic epilogue tests every feature for
+// each of the 64 accumulator values of a thread; it compiled to ~29 k SASS instructions per kernel, more than the
+// instruction caches hold, and its issue time exceeded the main loop of the short-K GEMMs.  Bias is a uniform runtime test.
+template <bool OUT32, int ACT, int RES, bool LN = false, bool ROPE = false, bool STATS = false>
+struct Epi {
+  static constexpr bool out32 = OUT32, ln = LN, rope = ROPE, stats = STATS;
+  static constexpr int act = ACT, res = RES;
+};
 
 struct GemmParams {
   void *C;
@@ -38,12 +49,9 @@ struct GemmParams {
   long long ldc, ldr;
   int M, N, K;
   int m_blocks, n_blocks, k_blocks;
-  int out_dtype;  // APE_DTYPE_*
-  int res_dtype;  // APE_DTYPE_* of `residual` (fp32-output GEMMs may add a 16-bit residual and vice versa)
-  int act;
-  int n_fastest;  // tile order: consecutive tiles walk the column blocks of one row group (A stays hot in L2)
-  int vec_out;    // C rows allow paired (2-element) stores
-  int vec_res;    // residual rows allow paired loads
+  int band;     // tile order: row groups per raster band (see tile_at)
+  int vec_out;  // C rows allow paired (2-element) stores
+  int fast;     // C, residual, bias and column sums allow paired accesses: tiles inside M x N take the unguarded epilogue
   // optional 2-D rotary embedding on output columns [0, rope_cols) (q and k thirds of a fused qkv projection;
   // VisionRotaryEmbeddingFast, utils_eva02.py:248-252,346), applied after the bias in fp32: 64-channel heads
   const float *rope_cos, *rope_sin;  // [npos, 64]
@@ -81,16 +89,24 @@ struct alignas(1024) GemmSmem {
   uint64_t full[STAGES], empty[STAGES];
 };
 
-__device__ __forceinline__ float act1(float v, int act) {
-  if (act == ACT_RELU) return fmaxf(v, 0.f);
-  if (act == ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
-  if (act == ACT_CLAMP) return fminf(fmaxf(v, -50000.f), 50000.f);  // vision_language_align.py:49-51
+template <int ACT>
+__device__ __forceinline__ float act1(float v) {
+  if constexpr (ACT == ACT_RELU) return fmaxf(v, 0.f);
+  if constexpr (ACT == ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+  if constexpr (ACT == ACT_CLAMP) return fminf(fmaxf(v, -50000.f), 50000.f);  // vision_language_align.py:49-51
   return v;
 }
 
-__device__ __forceinline__ float ld16(const uint16_t *p, bool half) {
-  const uint16_t u = __ldg(p);
-  return half ? __half2float(__ushort_as_half(u)) : __uint_as_float((uint32_t)u << 16);
+// (p[n], p[n + 1]) of an fp32 vector: one 8-byte load when VEC (n even, base 8-byte aligned), else p[n + 1] only if ok1
+template <bool VEC>
+__device__ __forceinline__ float2 ld_pair(const float *p, int n, bool ok1) {
+  if constexpr (VEC) return __ldg(reinterpret_cast<const float2 *>(p + n));
+  return make_float2(__ldg(p + n), ok1 ? __ldg(p + n + 1) : 0.f);
+}
+template <bool VEC, typename T>
+__device__ __forceinline__ float2 ld_res_pair(const T *p, bool ok1) {
+  if constexpr (VEC) return Elem<T>::load2(p);
+  return make_float2(Elem<T>::load1(p), ok1 ? Elem<T>::load1(p + 1) : 0.f);
 }
 
 // Element offset of output row m: the row itself, or for the convolution the NHWC pixel the tile row stands for.
@@ -122,19 +138,22 @@ __device__ __forceinline__ void store_pair(TO *dst, float v0, float v1, bool ok1
 // Epilogue of one warpgroup for its 64 rows x BN columns of tile (m_blk, n_blk), from the wgmma accumulator fragment:
 // thread (warp w, lane l) holds rows r0 = 16 w + l/4 and r0 + 8, column pairs 8 j + 2 (l % 4) + {0, 1}.  Adjacent column
 // pairs are exactly what SwiGLU (interleaved gate / up) and the rotary embedding (rotate_half pairs) combine.
-template <typename TO, int BN>
+// FULL: the tile lies inside M x N and p.fast holds, so no row or column test and paired loads throughout; edge tiles
+// (and outputs / residuals / vectors without 8-byte pairs) take the guarded instantiation.
+template <class E, typename TI, int BN, bool FULL>
 __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, int m_blk, int n_blk, int wg, int lane) {
+  using TO = std::conditional_t<E::out32, float, TI>;
+  constexpr bool swiglu = E::act == ACT_SWIGLU;
   const int warp4 = (threadIdx.x >> 5) & 3, tq = lane & 3;
   const int c_base = n_blk * BN + 2 * tq;
-  const bool swiglu = p.act == ACT_SWIGLU;
   TO *C = reinterpret_cast<TO *>(p.C);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int m = m_blk * BM + wg * 64 + warp4 * 16 + (lane >> 2) + 8 * h;
-    const bool row_ok = m < p.M;
+    const bool row_ok = FULL || m < p.M;
     const int mr = row_ok ? m : p.M - 1;  // rows past M read a valid row and store nothing
     float ln_rstd = 1.f, ln_shift = 0.f;  // ln_shift = rstd * mean
-    if (p.ln_part != nullptr) {  // row statistics from the producer's partials, summed in a fixed order
+    if constexpr (E::ln) {  // row statistics from the producer's partials, summed in a fixed order
       const float2 *pp = reinterpret_cast<const float2 *>(p.ln_part) + (size_t)mr * p.ln_nparts;
       float sum = 0.f, sq = 0.f;
       for (int i = 0; i < p.ln_nparts; ++i) {
@@ -146,35 +165,35 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
       ln_rstd = rsqrtf(fmaxf(sq * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
       ln_shift = ln_rstd * mean;
     }
-    const float *rcos = nullptr, *rsin = nullptr;
-    if (p.rope_cos != nullptr) {
-      const int pos = p.rope_pos ? __ldg(p.rope_pos + mr) : mr % p.rope_npos;
-      rcos = p.rope_cos + (size_t)pos * 64;
-      rsin = p.rope_sin + (size_t)pos * 64;
-    }
+    int rope_row = 0;  // first table element of the row's position (an offset, not two pointers: it keeps BN = 128 spill-free)
+    if constexpr (E::rope) rope_row = (p.rope_pos ? __ldg(p.rope_pos + mr) : mr % p.rope_npos) * 64;
     TO *crow = C + out_row_offset(p, mr);
+    const float *res32 = reinterpret_cast<const float *>(p.residual) + (size_t)mr * p.ldr;
+    const TI *res16 = reinterpret_cast<const TI *>(p.residual) + (size_t)mr * p.ldr;
     float st_sum = 0.f, st_sq = 0.f;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       const int n = c_base + 8 * j;
-      const bool ok0 = n < p.N, ok1 = n + 1 < p.N;
+      const bool ok0 = FULL || n < p.N, ok1 = FULL || n + 1 < p.N;
       float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
       if (ok0) {
-        if (p.ln_part != nullptr) {  // rstd * acc - rstd * mean * colsum; the bias below is beta W^T + b
-          v0 = fmaf(ln_rstd, v0, -ln_shift * __ldg(p.ln_colsum + n));
-          if (ok1) v1 = fmaf(ln_rstd, v1, -ln_shift * __ldg(p.ln_colsum + n + 1));
+        if constexpr (E::ln) {  // rstd * acc - rstd * mean * colsum; the bias below is beta W^T + b
+          const float2 cs = ld_pair<FULL>(p.ln_colsum, n, ok1);
+          v0 = fmaf(ln_rstd, v0, -ln_shift * cs.x);
+          if (ok1) v1 = fmaf(ln_rstd, v1, -ln_shift * cs.y);
         }
-        if (p.bias != nullptr) {
-          v0 += __ldg(p.bias + n);
-          if (ok1) v1 += __ldg(p.bias + n + 1);
+        if (p.bias != nullptr) {  // with the LN fold, paired bias loads cost the cluster kernel 8 bytes of spill
+          const float2 b = ld_pair<FULL && !E::ln>(p.bias, n, ok1);
+          v0 += b.x;
+          if (ok1) v1 += b.y;
         }
       }
-      if (swiglu) {
+      if constexpr (swiglu) {
         // interleaved (gate, up) column pair -> silu(gate) * up, output column n / 2 (vit_eva_clip.py:126-128); N is even
         const float o = v0 / (1.f + __expf(-v0)) * v1;
         const TO ot = Elem<TO>::from_f(o);
         if (ok0 && row_ok) crow[n / 2] = ot;
-        if (p.stats_out != nullptr) {  // statistics of the values as stored (16-bit), columns beyond N/2 excluded
+        if constexpr (E::stats) {  // statistics of the values as stored (16-bit), columns beyond N/2 excluded
           const float f = ok0 ? Elem<TO>::to_f(ot) : 0.f;
           st_sum += f;
           st_sq = fmaf(f, f, st_sq);
@@ -191,35 +210,27 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
           }
         }
         continue;
-      }
-      if (rcos != nullptr && n < p.rope_cols) {  // rotate_half pair (n, n+1) -> (-t[n+1], t[n])
-        const float2 c = __ldg(reinterpret_cast<const float2 *>(rcos + (n & 63)));
-        const float2 s = __ldg(reinterpret_cast<const float2 *>(rsin + (n & 63)));
-        const float t0 = v0, t1 = v1;
-        v0 = t0 * c.x - t1 * s.x;
-        v1 = t1 * c.y + t0 * s.y;
-      }
-      v0 = act1(v0, p.act);
-      v1 = act1(v1, p.act);
-      if (p.residual != nullptr && ok0) {
-        if (p.res_dtype == APE_DTYPE_F32) {
-          const float *res = reinterpret_cast<const float *>(p.residual) + (size_t)mr * p.ldr + n;
-          if (p.vec_res && ok1) {
-            const float2 r2 = __ldg(reinterpret_cast<const float2 *>(res));
-            v0 += r2.x;
-            v1 += r2.y;
-          } else {
-            v0 += __ldg(res);
-            if (ok1) v1 += __ldg(res + 1);
+      } else {
+        if constexpr (E::rope) {
+          if (n < p.rope_cols) {  // rotate_half pair (n, n+1) -> (-t[n+1], t[n])
+            const float2 c = __ldg(reinterpret_cast<const float2 *>(p.rope_cos + rope_row + (n & 63)));
+            const float2 s = __ldg(reinterpret_cast<const float2 *>(p.rope_sin + rope_row + (n & 63)));
+            const float t0 = v0, t1 = v1;
+            v0 = t0 * c.x - t1 * s.x;
+            v1 = t1 * c.y + t0 * s.y;
           }
-        } else {
-          const uint16_t *res = reinterpret_cast<const uint16_t *>(p.residual) + (size_t)mr * p.ldr + n;
-          const bool half = p.res_dtype == APE_DTYPE_F16;
-          v0 += ld16(res, half);
-          if (ok1) v1 += ld16(res + 1, half);
         }
+        v0 = act1<E::act>(v0);
+        v1 = act1<E::act>(v1);
+        if constexpr (E::res != RES_NONE) {
+          if (ok0) {
+            const float2 r = E::res == RES_F32 ? ld_res_pair<FULL>(res32 + n, ok1) : ld_res_pair<FULL>(res16 + n, ok1);
+            v0 += r.x;
+            if (ok1) v1 += r.y;
+          }
+        }
+        if (ok0 && row_ok) store_pair<TO>(crow + n, v0, v1, ok1, FULL || p.vec_out);
       }
-      if (ok0 && row_ok) store_pair<TO>(crow + n, v0, v1, ok1, p.vec_out);
     }
   }
 }
@@ -228,7 +239,7 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
 // of the same BN-column block: each loads half of the B (weight) tile and TMA-multicasts it into both CTAs' shared
 // memory, which halves the weight traffic from L2 per CTA.  A stage may only be refilled when the consumers of BOTH CTAs
 // have finished reading it, so every consumer warp arrives on the "empty" barrier of both CTAs.
-template <int BN, int STAGES, int CL, typename TI>
+template <int BN, int STAGES, int CL, typename TI, class E>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -244,13 +255,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int m_groups = (p.m_blocks + CL - 1) / CL;
   const int num_tiles = m_groups * p.n_blocks;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
-  // t-th tile of this CTA: tiles first, first + stride, ... of the (row group, column block) grid
+  // t-th tile of this CTA: tiles first, first + stride, ... of the (row group, column block) grid, walked in bands of
+  // p.band row groups; inside a band the row group changes fastest.  The tiles resident at one time then cover a few row
+  // groups across all column blocks, so each A row block is read from HBM once, not once per column block.
   auto tile_at = [&](int t, int &m_blk, int &n_blk) -> bool {
     const int tile = first + t * stride;
     if (tile >= num_tiles) return false;
-    const int mg = p.n_fastest ? tile / p.n_blocks : tile % m_groups;
-    n_blk = p.n_fastest ? tile % p.n_blocks : tile / m_groups;
-    m_blk = mg * CL + rank;
+    const int per_band = p.band * p.n_blocks;
+    const int band = tile / per_band, r = tile - band * per_band;
+    const int rows = min(p.band, m_groups - band * p.band);
+    n_blk = r / rows;
+    m_blk = (band * p.band + r - n_blk * rows) * CL + rank;
     return true;
   };
 
@@ -341,9 +356,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if (t == 0) trace_stamp(p, 4);
         trace_stamp(p, 5);
       }
-      if (p.out_dtype == APE_DTYPE_F32) epilogue<float, BN>(p, acc, m_blk, n_blk, wg, lane);
-      else if (p.out_dtype == APE_DTYPE_F16) epilogue<__half, BN>(p, acc, m_blk, n_blk, wg, lane);
-      else epilogue<__nv_bfloat16, BN>(p, acc, m_blk, n_blk, wg, lane);
+      if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) epilogue<E, TI, BN, true>(p, acc, m_blk, n_blk, wg, lane);
+      else epilogue<E, TI, BN, false>(p, acc, m_blk, n_blk, wg, lane);
     }
     if (threadIdx.x == 0) trace_stamp(p, 6);
   }
@@ -397,11 +411,11 @@ int num_sms() {
   return n;
 }
 
-template <int BN, int STAGES, int CL, typename TI>
+template <int BN, int STAGES, int CL, typename TI, class E>
 int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
   using Smem = GemmSmem<BN, STAGES>;
   const size_t smem = sizeof(Smem) + 1024;
-  auto k = gemm_tc_kernel<BN, STAGES, CL, TI>;
+  auto k = gemm_tc_kernel<BN, STAGES, CL, TI, E>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -409,10 +423,13 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cud
     attr_set = true;
   }
   p.n_blocks = (p.N + BN - 1) / BN;
-  p.n_fastest = p.n_blocks <= 8;  // few column blocks: keep the A rows of a group hot instead of re-reading A per column block
-  const int groups = (p.m_blocks + CL - 1) / CL * p.n_blocks;
+  const int m_groups = (p.m_blocks + CL - 1) / CL;
+  const int groups = m_groups * p.n_blocks;
   const int max_clusters = num_sms() / CL;
   const int clusters = groups < max_clusters ? groups : max_clusters;
+  // raster band: the fewest row groups whose tiles across all column blocks occupy every resident CTA.  Its A rows
+  // (band x 128 x K) and the whole of W stay in L2 for the model's shapes (W is at most 11 MB: the ViT SwiGLU w12).
+  p.band = std::min(m_groups, (clusters + p.n_blocks - 1) / p.n_blocks);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(clusters * CL));
   cfg.blockDim = dim3(kThreads);
@@ -433,16 +450,57 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cud
 }
 
 // 4 stages of 48 KB (BN = 256) or 6 of 32 KB (BN = 128): 192 KB of the 227 KB a block may use.
-template <int CL, typename TI>
+template <int CL, typename TI, class E>
 int launch_bn(int bn, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
-  if (bn == 256) return launch_gemm<256, 4, CL, TI>(ma, mb, p, st);
-  return launch_gemm<128, 6, CL, TI>(ma, mb, p, st);
+  if (bn == 256) return launch_gemm<256, 4, CL, TI, E>(ma, mb, p, st);
+  return launch_gemm<128, 6, CL, TI, E>(ma, mb, p, st);
 }
 
-int launch_any(int bn, bool cluster, int in_dtype, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+struct EpiKey {
+  bool out32;
+  int act, res;
+  bool ln, rope, stats;
+};
+
+// The epilogues with a kernel, X(out32, act, residual, ln, rope, stats), each for fp16 and bf16 operands; a 16-bit output
+// or residual has the operand type.  Any other combination is rejected.
+//   model call sites                                                     tests/test_gemm_gpu.py adds
+//   16-bit  none             most projections, heads, 1x1 / 3x3 convs     16-bit + 16-bit residual, any of none/relu/gelu
+//   16-bit  relu             encoder / decoder FFN1, MLP heads           fp32 + relu / gelu / swiglu
+//   16-bit  gelu             text-tower MLP
+//   16-bit  + fp32 residual  MSDA output projection, MLP with residual
+//   16-bit  swiglu (+stats)  ViT w12
+//   16-bit  rope             ViT qkv with fused rotary embedding
+//   fp32    none / clamp     class / box heads, mask logits, text projection, vision-language logits
+//   fp32    + fp32 / 16-bit residual   ViT proj / w3 / patch embed, encoder FFN2, text blocks, decoder self-attention out
+//   fp32    LN fold + fp32 residual    ViT proj / w3 after the sub-LayerNorms
+#define APE_GEMM_EPILOGUES(X)                                                                                            \
+  X(false, ACT_NONE, RES_NONE, false, false, false) X(false, ACT_RELU, RES_NONE, false, false, false)                   \
+  X(false, ACT_GELU, RES_NONE, false, false, false) X(false, ACT_NONE, RES_F32, false, false, false)                    \
+  X(false, ACT_NONE, RES_16, false, false, false) X(false, ACT_RELU, RES_16, false, false, false)                       \
+  X(false, ACT_GELU, RES_16, false, false, false) X(false, ACT_SWIGLU, RES_NONE, false, false, false)                   \
+  X(false, ACT_SWIGLU, RES_NONE, false, false, true) X(false, ACT_NONE, RES_NONE, false, true, false)                   \
+  X(true, ACT_NONE, RES_NONE, false, false, false) X(true, ACT_RELU, RES_NONE, false, false, false)                     \
+  X(true, ACT_GELU, RES_NONE, false, false, false) X(true, ACT_SWIGLU, RES_NONE, false, false, false)                   \
+  X(true, ACT_CLAMP, RES_NONE, false, false, false) X(true, ACT_NONE, RES_F32, false, false, false)                     \
+  X(true, ACT_NONE, RES_16, false, false, false) X(true, ACT_NONE, RES_F32, true, false, false)
+
+template <int CL, typename TI>
+int launch_epi(int bn, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+#define APE_EPI_CASE(o, a, r, l, ro, s)                                                                                  \
+  if (k.out32 == o && k.act == a && k.res == r && k.ln == l && k.rope == ro && k.stats == s)                           \
+    return launch_bn<CL, TI, Epi<o, a, r, l, ro, s>>(bn, ma, mb, p, st);
+  APE_GEMM_EPILOGUES(APE_EPI_CASE)
+#undef APE_EPI_CASE
+  return fail(APE_ERR_UNSUPPORTED, "gemm: no kernel for the epilogue (fp32 out %d, act %d, residual %d, ln %d, rope %d, stats %d)",
+              (int)k.out32, k.act, k.res, (int)k.ln, (int)k.rope, (int)k.stats);
+}
+
+int launch_any(int bn, bool cluster, int in_dtype, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p,
+               cudaStream_t st) {
   if (in_dtype == APE_DTYPE_BF16)
-    return cluster ? launch_bn<2, __nv_bfloat16>(bn, ma, mb, p, st) : launch_bn<1, __nv_bfloat16>(bn, ma, mb, p, st);
-  return cluster ? launch_bn<2, __half>(bn, ma, mb, p, st) : launch_bn<1, __half>(bn, ma, mb, p, st);
+    return cluster ? launch_epi<2, __nv_bfloat16>(bn, k, ma, mb, p, st) : launch_epi<1, __nv_bfloat16>(bn, k, ma, mb, p, st);
+  return cluster ? launch_epi<2, __half>(bn, k, ma, mb, p, st) : launch_epi<1, __half>(bn, k, ma, mb, p, st);
 }
 
 }  // namespace
@@ -506,11 +564,19 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
   p.M = M; p.N = N; p.K = K;
   p.m_blocks = m_blocks;
   p.k_blocks = (K + BK - 1) / BK;
-  p.out_dtype = out_dtype; p.act = act; p.res_dtype = res_dtype;
   p.trace = g_gemm_trace;
   const int oe = out_dtype == APE_DTYPE_F32 ? 4 : 2;
-  p.vec_out = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) % (2 * oe)) == 0;
-  p.vec_res = residual != nullptr && (ldr % 2) == 0 && (reinterpret_cast<uintptr_t>(residual) % 8) == 0;
+  if (oe == 2 && out_dtype != in_dtype)
+    return fail(APE_ERR_UNSUPPORTED, "gemm: a 16-bit output must have the operand dtype (out %d, operands %d)", out_dtype, in_dtype);
+  if (residual && res_dtype != APE_DTYPE_F32 && res_dtype != in_dtype)
+    return fail(APE_ERR_UNSUPPORTED, "gemm: a 16-bit residual must have the operand dtype (residual %d, operands %d)", res_dtype, in_dtype);
+  const auto pairs = [](const void *ptr, long long ld, int esize) {  // rows start on 2-element boundaries
+    return (ld % 2) == 0 && (reinterpret_cast<uintptr_t>(ptr) % (2 * esize)) == 0;
+  };
+  p.vec_out = pairs(C, ldc, oe);
+  p.fast = p.vec_out && (!residual || pairs(residual, ldr, res_dtype == APE_DTYPE_F32 ? 4 : 2)) &&
+           reinterpret_cast<uintptr_t>(bias) % 8 == 0 && (!fuse || reinterpret_cast<uintptr_t>(fuse->ln_colsum) % 8 == 0);
+  EpiKey key{oe == 4, act, !residual ? RES_NONE : res_dtype == APE_DTYPE_F32 ? RES_F32 : RES_16, false, rope != nullptr, false};
   const int n_out = act == ACT_SWIGLU ? N / 2 : N;
   if (fuse) {
     if (fuse->ln_part) {
@@ -518,11 +584,13 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
         return fail(APE_ERR_INVALID_ARG, "gemm+ln: needs an fp32 output, column sums and partial statistics");
       p.ln_part = fuse->ln_part; p.ln_colsum = fuse->ln_colsum; p.ln_nparts = fuse->ln_nparts;
       p.ln_inv_c = fuse->ln_inv_c; p.ln_eps = fuse->ln_eps;
+      key.ln = true;
     }
     if (fuse->stats_out) {
       if (oe != 2 || act != ACT_SWIGLU || fuse->stats_nslab != (n_out + 63) / 64)
         return fail(APE_ERR_INVALID_ARG, "gemm+stats: needs the SwiGLU epilogue with a 16-bit output and stats_nslab = ceil(N/2/64)");
       p.stats_out = fuse->stats_out; p.stats_nslab = fuse->stats_nslab;
+      key.stats = true;
     }
   }
   if (rope) {
@@ -530,7 +598,7 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
       return fail(APE_ERR_INVALID_ARG, "gemm+rope: needs a 16-bit output, no activation, rope_cols a multiple of 64 <= N");
     p.rope_cos = rope->cos; p.rope_sin = rope->sin; p.rope_pos = rope->pos; p.rope_cols = rope->cols; p.rope_npos = rope->npos;
   }
-  return launch_any(bn, cluster, in_dtype, ma, mb, p, st);
+  return launch_any(bn, cluster, in_dtype, key, ma, mb, p, st);
 }
 
 extern "C" int ape_gemm_tn(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,
@@ -598,11 +666,12 @@ extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const flo
   p.C = y; p.bias = bias; p.ldc = N; p.M = M; p.N = N; p.K = K;
   p.m_blocks = m_blocks;
   p.k_blocks = K / BK;
-  p.out_dtype = dtype; p.res_dtype = dtype; p.act = act;
   p.vec_out = 1;
+  p.fast = reinterpret_cast<uintptr_t>(bias) % 8 == 0;
   p.conv = 1; p.conv_tw = tw; p.conv_th = th; p.conv_tiles_x = W / tw; p.conv_tiles_img = (W / tw) * (H / th); p.conv_cblks = Cin / 64;
   p.conv_W = W; p.conv_H = H;
-  return launch_any(bn, cluster, dtype, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
+  const EpiKey key{false, act, RES_NONE, false, false, false};
+  return launch_any(bn, cluster, dtype, key, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,
