@@ -90,6 +90,8 @@ def _declare(lib):
     lib.ape_attn_fwd.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, ctypes.c_float, _i, _vp]
     lib.ape_attn_fwd_ex.restype = _i
     lib.ape_attn_fwd_ex.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _i, _i64, _vp]
+    lib.ape_attn_fwd_mapped.restype = _i
+    lib.ape_attn_fwd_mapped.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _i, _i64, _vp, _vp]
     lib.ape_attn_variant.restype = _i
     lib.ape_attn_variant.argtypes = [_i]
     lib.ape_attn_cross_fwd.restype = _i
@@ -157,6 +159,7 @@ EXPORTS = (
     "ape_rope_qk",
     "ape_attn_fwd",
     "ape_attn_fwd_ex",
+    "ape_attn_fwd_mapped",
     "ape_attn_variant",
     "ape_attn_cross_fwd",
     "ape_groupnorm_workspace_bytes",

@@ -43,6 +43,7 @@ struct Params {
   int heads;
   float *stats_out;             // [rows, heads, 2] (sum, sum of squares) of each row's stored output values, or nullptr
   float scale_log2;             // softmax scale * log2(e)
+  const int *out_row_map;       // ROW_MAP kernels: query row r is stored at out / stats_out row out_row_map[r]; -1 = not stored
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -62,7 +63,7 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
   }
 }
 
-template <typename T, int NC, int CWG, bool P_IN_SMEM>
+template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false>
 __global__ void __launch_bounds__(CWG * 128 + 32, NC == 1 ? 2 : 1)
 attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
             const __grid_constant__ CUtensorMap map_v, const Params p) {
@@ -231,8 +232,13 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
     l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
     const float inv = 1.f / l[h];
     // packed sequences: rows past the sequence belong to the next one and must not be written
-    const bool store_row = qpos[h] < p.q_store_rows;
-    const size_t row = (size_t)seq * p.q_seq_rows + qpos[h];
+    bool store_row = qpos[h] < p.q_store_rows;
+    size_t row = (size_t)seq * p.q_seq_rows + qpos[h];
+    if constexpr (ROW_MAP) {  // e.g. padded windows back to raster order; pad rows map to -1
+      const int mapped = store_row ? p.out_row_map[row] : -1;
+      store_row = mapped >= 0;
+      row = (size_t)(store_row ? mapped : 0);
+    }
     T *dst = reinterpret_cast<T *>(p.out) + row * p.ldo + head * HD + 2 * tq;
     float st_sum = 0.f, st_sq = 0.f;
 #pragma unroll
@@ -287,10 +293,10 @@ inline int make_map(CUtensorMap *map, const void *base, int dtype, long long row
 }
 
 // grid = (query rows per sequence / (64 * CWG), heads, sequences)
-template <typename T, int NC, int CWG, bool P_IN_SMEM>
+template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false>
 int launch(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const Params &p, dim3 grid, cudaStream_t st) {
   const size_t smem = sizeof(Smem<NC, CWG, P_IN_SMEM>) + 1024;
-  auto k = attn_kernel<T, NC, CWG, P_IN_SMEM>;
+  auto k = attn_kernel<T, NC, CWG, P_IN_SMEM, ROW_MAP>;
   static bool set = false;
   if (!set) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

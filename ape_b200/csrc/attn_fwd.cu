@@ -2,7 +2,8 @@
 // vit_eva_clip.py:218-319: q·k^T·scale -> softmax -> ·v, 16 heads x 64, window (N=1024) and global (N=4096) blocks)
 // and of the EVA02-CLIP text tower (causal, 77-token prompts packed at a row stride): flash-attention forward with wgmma
 // (attn.cuh), Q/K/V tiles staged by TMA straight out of the fused [M, 3C] qkv buffer the qkv GEMM wrote (no head split
-// copies).  One CTA = 128 queries (two consumer warpgroups) of one (sequence, head).
+// copies).  One CTA = 128 queries (two consumer warpgroups) of one (sequence, head).  ape_attn_fwd_mapped stores query rows
+// through a row map (APE-Ti's padded 14x14 windows write straight back to raster token order).
 #include <stdlib.h>
 
 #include "attn.cuh"
@@ -37,9 +38,10 @@ extern "C" int ape_attn_fwd(const void *qkv, int64_t ld, void *out, int64_t ldo,
   return ape_attn_fwd_ex(qkv, ld, out, ldo, num_seq, n, n, heads, head_dim, scale, dtype, nullptr, 0, 0, 0, stream);
 }
 
-extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
-                               int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
-                               void *stream) {
+// ape_attn_fwd_ex / ape_attn_fwd_mapped; out_row_map == nullptr stores query row r at row r
+static int attn_fwd_impl(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                         int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
+                         const int *out_row_map, void *stream) {
   if (n_valid <= 0 || n_valid > n) return fail(APE_ERR_INVALID_ARG, "attn: n_valid=%d must be in [1, n=%d]", n_valid, n);
   if (seq_stride <= 0) seq_stride = n;
   if (seq_stride < n_valid) return fail(APE_ERR_INVALID_ARG, "attn: seq_stride=%d smaller than n_valid=%d", seq_stride, n_valid);
@@ -64,11 +66,35 @@ extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t l
   p.n_valid = n_valid; p.causal = causal ? 1 : 0;
   p.q_store_rows = seq_stride >= n ? n : n_valid;
   p.scale_log2 = scale * 1.4426950408889634f;
+  p.out_row_map = out_row_map;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   dim3 grid((unsigned)(n / QM), (unsigned)heads, (unsigned)num_seq);
   const bool p_smem = ape_attn_variant(-1) == 0;
+  if (out_row_map) {
+    if (dtype == APE_DTYPE_F16)
+      return p_smem ? attn::launch<__half, 1, 2, true, true>(map, map, map, p, grid, st)
+                    : attn::launch<__half, 1, 2, false, true>(map, map, map, p, grid, st);
+    return p_smem ? attn::launch<__nv_bfloat16, 1, 2, true, true>(map, map, map, p, grid, st)
+                  : attn::launch<__nv_bfloat16, 1, 2, false, true>(map, map, map, p, grid, st);
+  }
   if (dtype == APE_DTYPE_F16)
     return p_smem ? attn::launch<__half, 1, 2, true>(map, map, map, p, grid, st) : attn::launch<__half, 1, 2, false>(map, map, map, p, grid, st);
   return p_smem ? attn::launch<__nv_bfloat16, 1, 2, true>(map, map, map, p, grid, st)
                 : attn::launch<__nv_bfloat16, 1, 2, false>(map, map, map, p, grid, st);
+}
+
+extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                               int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
+                               void *stream) {
+  return attn_fwd_impl(qkv, ld, out, ldo, num_seq, n, n_valid, heads, head_dim, scale, dtype, stats_out, seq_stride, causal,
+                       total_rows, nullptr, stream);
+}
+
+extern "C" int ape_attn_fwd_mapped(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                                   int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal,
+                                   int64_t total_rows, const int *out_row_map, void *stream) {
+  if (!out_row_map) return fail(APE_ERR_NULL_PTR, "attn: out_row_map is required (ape_attn_fwd_ex stores rows in place)");
+  if (reinterpret_cast<uintptr_t>(out_row_map) & 3) return fail(APE_ERR_INVALID_ARG, "attn: out_row_map must be int32-aligned");
+  return attn_fwd_impl(qkv, ld, out, ldo, num_seq, n, n_valid, heads, head_dim, scale, dtype, stats_out, seq_stride, causal,
+                       total_rows, out_row_map, stream);
 }

@@ -1,4 +1,4 @@
-"""EVA-02 ViT backbone + SimpleFeaturePyramid of APE-L_D.
+"""EVA-02 ViT backbone + SimpleFeaturePyramid of APE-L_D and APE-Ti.
 
 Mirror of ape/modeling/backbone/vit_eva_clip.py (`ViT` :570-754, `Block` :383-567, `Attention`
 :135-319, `SwiGLU` :101-132, `SimpleFeaturePyramid` :757-922) and utils_eva02.py (`PatchEmbed`
@@ -215,7 +215,9 @@ class ViT(nn.Module):
         # (+26 us per GEMM with the general epilogue, +27 us with a lean one: per-thread cos / sin rows are 32 different lines per
         # warp load) against 8.7 us for the pass; APE_FUSED_ROPE=1 switches it on for A/B runs
         self.fused_rope = os.environ.get("APE_FUSED_ROPE", "0") == "1"
-        self.engine_attention = True  # ape_attn_fwd (own wgmma kernel) for head_dim 64 / n % 128 == 0, else library SDPA
+        # APE-L path: ape_attn_fwd (own wgmma kernel) for head_dim 64 / n % 128 == 0, else library SDPA (the APE-Ti path
+        # always runs ape_attn_fwd*: _engine_ok requires 64-channel heads)
+        self.engine_attention = True
         # inner_attn_ln / ffn_ln folded around proj / w3 (ape_gemm_tn_fused): two LayerNorm launches and two trips of the
         # activations through HBM fewer per block
         self.fold_sub_layernorms = True
@@ -251,17 +253,24 @@ class ViT(nn.Module):
 
     # ---------------------------------------------------------------------------------------------
     # Engine path (fp16 / bf16): libape_b200 kernels — wgmma GEMMs with fused bias / SwiGLU /
-    # residual epilogues, LayerNorm and RoPE kernels; tokens stay in WINDOW-MAJOR order for the
-    # whole network (attention is permutation-equivariant once the RoPE table follows the tokens), so
-    # window_partition / window_unpartition (utils_eva02.py:19-63) cost one permutation at the
-    # patch embedding and one at the end instead of two copies per block.
+    # residual epilogues, LayerNorm and RoPE kernels.  APE-L_*: tokens stay in WINDOW-MAJOR order for
+    # the whole network (attention is permutation-equivariant once the RoPE table follows the tokens),
+    # so window_partition / window_unpartition (utils_eva02.py:19-63) cost one permutation at the
+    # patch embedding and one at the end instead of two copies per block.  APE-Ti (windows that need
+    # not tile the grid): tokens stay in RASTER order and each window block scatters / gathers them
+    # through row maps (_engine_tokens_raster).
     # ---------------------------------------------------------------------------------------------
     def _engine_ok(self, x):
-        if not self._variant_l:  # the tensor-core token path is written for the APE-L block layout
-            return False
         ws = next((b.window_size for b in self.blocks if b.window_size > 0), 0)
-        g = x.shape[-1] // self.patch_embed.proj.kernel_size[0]
-        return x.shape[-1] == x.shape[-2] and (ws == 0 or g % ws == 0)
+        ps = self.patch_embed.proj.kernel_size[0]
+        g = x.shape[-1] // ps
+        if self._variant_l:
+            return x.shape[-1] == x.shape[-2] and (ws == 0 or g % ws == 0)
+        # APE-Ti raster path: any window size (windows are padded), 64-channel heads for the attention kernel, and the global
+        # RoPE table of this grid
+        C, heads = self.pos_embed.shape[-1], self.blocks[0].attn.num_heads
+        return x.shape[-1] == x.shape[-2] and x.shape[-1] % ps == 0 and C == 64 * heads and \
+            self.rope_glb.freqs_cos.shape[0] == g * g
 
     def _pack(self, dtype, device):
         """Weights re-laid out once for the kernels (fused qkv, interleaved SwiGLU pairs, K padded to 8)."""
@@ -277,25 +286,34 @@ class ViT(nn.Module):
             packed["patch_b"] = self.patch_embed.proj.bias.to(**f32).contiguous()
             for blk in self.blocks:
                 a, m = blk.attn, blk.mlp
-                hid = m.w1.weight.shape[0]
+                if self._variant_l:
+                    wqkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0)
+                    w1, w2, b1, b2 = m.w1.weight, m.w2.weight, m.w1.bias, m.w2.bias
+                else:  # vit_eva02.py: fused qkv projection, w12 = [w1; w2] stacked halves
+                    wqkv = a.qkv.weight
+                    w1, w2 = m.w12.weight.chunk(2, 0)
+                    b1, b2 = m.w12.bias.chunk(2, 0)
+                hid = w1.shape[0]
                 hid_p = (hid + 7) // 8 * 8
-                w12 = torch.stack([m.w1.weight, m.w2.weight], 1).reshape(2 * hid, -1)  # rows (w1_j, w2_j)
-                b12 = torch.stack([m.w1.bias, m.w2.bias], 1).reshape(2 * hid)
+                w12 = torch.stack([w1, w2], 1).reshape(2 * hid, -1)  # rows (w1_j, w2_j)
+                b12 = torch.stack([b1, b2], 1).reshape(2 * hid)
                 w3 = torch.zeros(m.w3.weight.shape[0], hid_p, dtype=dtype, device=device)
                 w3[:, :hid] = m.w3.weight
-                packed["blocks"].append(dict(
+                d = dict(
                     n1w=blk.norm1.weight.to(**f32), n1b=blk.norm1.bias.to(**f32),
-                    wqkv=torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0).to(device, dtype).contiguous(),
+                    wqkv=wqkv.to(device, dtype).contiguous(),
                     bqkv=torch.cat([a.q_bias, torch.zeros_like(a.v_bias), a.v_bias]).to(**f32).contiguous(),
-                    lnw=a.inner_attn_ln.weight.to(**f32), lnb=a.inner_attn_ln.bias.to(**f32),
                     wproj=a.proj.weight.to(device, dtype).contiguous(), bproj=a.proj.bias.to(**f32).contiguous(),
                     n2w=blk.norm2.weight.to(**f32), n2b=blk.norm2.bias.to(**f32),
                     w12=w12.to(device, dtype).contiguous(), b12=b12.to(**f32).contiguous(),
-                    fw=m.ffn_ln.weight.to(**f32).contiguous(), fb=m.ffn_ln.bias.to(**f32).contiguous(),
-                    w3=w3, b3=m.w3.bias.to(**f32).contiguous(), hid=hid, hid_p=hid_p))
+                    w3=w3, b3=m.w3.bias.to(**f32).contiguous(), hid=hid, hid_p=hid_p)
+                packed["blocks"].append(d)
+                if not self._variant_l:
+                    continue
+                d.update(lnw=a.inner_attn_ln.weight.to(**f32), lnb=a.inner_attn_ln.bias.to(**f32),
+                         fw=m.ffn_ln.weight.to(**f32).contiguous(), fb=m.ffn_ln.bias.to(**f32).contiguous())
                 # sub-LayerNorms folded around the GEMM that follows them (ape_gemm_tn_fused): gamma .* W as the 16-bit
                 # operand, its row sums, and beta W^T + b as the bias
-                d = packed["blocks"][-1]
                 wp = (a.proj.weight.float() * a.inner_attn_ln.weight.float()[None, :]).to(device, dtype).contiguous()
                 d.update(wproj_ln=wp, sproj=wp.float().sum(1).contiguous(),
                          bproj_ln=(a.proj.weight.float() @ a.inner_attn_ln.bias.float() + a.proj.bias.float()).to(**f32).contiguous())
@@ -321,10 +339,31 @@ class ViT(nn.Module):
         geom[k] = geo
         return geo
 
+    def _raster_geometry(self, B, g, ws, device):
+        """APE-Ti, per input geometry: abs-pos table in raster order, and the maps between raster rows and the padded
+        window-major rows of window_partition (windows of ws x ws over the grid padded to a multiple of ws)."""
+        k = ("raster", B, g, ws, str(device), self.pos_embed._version)
+        geom = self.__dict__.setdefault("_geom", {})
+        if k in geom:
+            return geom[k]
+        pos = get_abs_pos(self.pos_embed.detach().float(), self.pretrain_use_cls_token, (g, g)).reshape(g * g, -1)
+        geo = dict(pos=pos.float().repeat(B, 1).contiguous())  # fp32: first value of the residual stream
+        if ws:
+            nw = -(-g // ws)
+            b, y, x = torch.meshgrid(torch.arange(B), torch.arange(g), torch.arange(g), indexing="ij")
+            row = ((b * nw + y // ws) * nw + x // ws) * (ws * ws) + (y % ws) * ws + x % ws  # raster -> padded window-major
+            inv = torch.full((B * nw * nw * ws * ws,), -1, dtype=torch.int32)
+            inv[row.reshape(-1)] = torch.arange(B * g * g, dtype=torch.int32)  # pad rows stay -1
+            geo.update(win_map=row.reshape(-1).to(device, torch.int32), win_out_map=inv.to(device), windows=B * nw * nw)
+        geom[k] = geo
+        return geo
+
     def _engine_forward(self, img):
         return self._engine_tokens(img).permute(0, 3, 1, 2)  # NCHW view over NHWC memory (channels_last)
 
     def _engine_tokens(self, img):
+        if not self._variant_l:
+            return self._engine_tokens_raster(img)
         B, _, Hh, Ww = img.shape
         ps = self.patch_embed.proj.kernel_size[0]
         g = Hh // ps
@@ -394,6 +433,49 @@ class ViT(nn.Module):
                 x = ops.linear_tc(hbuf2[:, :p["hid"]], p["w3"][:, :p["hid"]], p["b3"], residual=x, out_dtype=torch.float32)
         # back to raster order: [B, g, g, C] tokens (NHWC memory), 16-bit operand of the pyramid GEMMs
         return x.to(dtype).view(B, g * g, C)[:, geo["inv"]].view(B, g, g, C)
+
+    def _engine_tokens_raster(self, img):
+        """APE-Ti blocks (vit_eva02.py: fused qkv, packed SwiGLU, no sub-LayerNorms) with the fp32 residual stream in raster
+        order.  A window block's norm1 scatters the tokens into a zero-initialised buffer of padded ws x ws windows (pad rows
+        are never written, so they stay the zeros window_partition pads with and attend as keys k = 0, v = v_bias), and its
+        attention writes each real query row straight back to its raster row; global blocks attend over the raster rows."""
+        B, _, Hh, _ = img.shape
+        ps = self.patch_embed.proj.kernel_size[0]
+        g = Hh // ps
+        ws = next((b.window_size for b in self.blocks if b.window_size > 0), 0)
+        dtype, dev = img.dtype, img.device
+        pk = self._pack(dtype, dev)
+        geo = self._raster_geometry(B, g, ws, dev)
+        C = self.pos_embed.shape[-1]
+        heads = self.blocks[0].attn.num_heads
+        hd = C // heads
+        M = B * g * g
+        cols = img.view(B, 3, g, ps, g, ps).permute(0, 2, 4, 1, 3, 5).reshape(M, 3 * ps * ps)  # raster im2col rows
+        x = ops.linear_tc(cols, pk["patch_w"], pk["patch_b"], residual=geo["pos"], out_dtype=torch.float32)
+        rope_win = (self.rope_win.freqs_cos.float().contiguous(), self.rope_win.freqs_sin.float().contiguous())
+        rope_glb = (self.rope_glb.freqs_cos.float().contiguous(), self.rope_glb.freqs_sin.float().contiguous())
+        hid, hid_p = pk["blocks"][0]["hid"], pk["blocks"][0]["hid_p"]
+        hbuf = torch.empty((M, hid_p), dtype=dtype, device=dev)[:, :hid]
+        hwin = torch.zeros((geo["windows"] * ws * ws, C), dtype=dtype, device=dev) if ws else None
+        pad128 = lambda n: -(-n // 128) * 128  # the attention kernel's sequence length: 128-row query tiles
+        for blk, p in zip(self.blocks, pk["blocks"]):
+            if blk.window_size > 0:
+                ops.layernorm(x, p["n1w"], p["n1b"], eps=1e-6, row_map=geo["win_map"], out=hwin)
+                qkv = ops.linear_tc(hwin, p["wqkv"], p["bqkv"])  # pad rows: q_bias, 0, v_bias
+                ops.rope_qk_(qkv, rope_win[0], rope_win[1], C, hd)  # position = row % (ws * ws) = index inside the window
+                o = torch.empty((M, C), dtype=dtype, device=dev)
+                ops.attention_qkv(qkv, geo["windows"], pad128(ws * ws), heads, hd, blk.attn.scale, n_valid=ws * ws,
+                                  seq_stride=ws * ws, out_row_map=geo["win_out_map"], out=o)
+            else:
+                h = ops.layernorm(x, p["n1w"], p["n1b"], eps=1e-6, out_dtype=dtype)
+                qkv = ops.linear_tc(h, p["wqkv"], p["bqkv"])
+                ops.rope_qk_(qkv, rope_glb[0], rope_glb[1], C, hd)  # position = row % (g * g)
+                o = ops.attention_qkv(qkv, B, pad128(g * g), heads, hd, blk.attn.scale, n_valid=g * g, seq_stride=g * g)
+            x = ops.linear_tc(o, p["wproj"], p["bproj"], residual=x, out_dtype=torch.float32)
+            h = ops.layernorm(x, p["n2w"], p["n2b"], eps=1e-6, out_dtype=dtype)
+            ops.linear_tc(h, p["w12"], p["b12"], act="swiglu", out=hbuf)
+            x = ops.linear_tc(hbuf, p["w3"][:, :hid], p["b3"], residual=x, out_dtype=torch.float32)
+        return x.to(dtype).view(B, g, g, C)  # [B, g, g, C] tokens (NHWC memory), 16-bit operand of the pyramid GEMMs
 
 
 def _convT_as_gemm(ct, dtype):

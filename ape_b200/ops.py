@@ -426,26 +426,42 @@ def attention_supported(n, head_dim, dtype):
     return head_dim == 64 and n % 128 == 0 and dtype in (torch.float16, torch.bfloat16)
 
 
-def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_out=False, seq_stride=None, causal=False):
+def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_out=False, seq_stride=None, causal=False,
+                  out_row_map=None, out=None):
     """softmax(q k^T * scale) v for every (sequence, head) straight from the fused qkv buffer [num_seq*n, 3*heads*64]
     (ape_attn_fwd: flash attention on the wgmma tensor cores).  Returns [num_seq*n, heads*64].
     n_valid: sequences are padded to n rows and only the first n_valid keys count (rows beyond must be finite).
     stats_out=True: also returns fp32 [rows, heads, 2] (sum, sum of squares of each row's stored values per head).
     seq_stride: rows between sequences when they are packed tighter than n (then n_valid <= seq_stride < n; rows of a tile
-    past n_valid are not written); causal: key t attends to keys <= t."""
+    past n_valid are not written); causal: key t attends to keys <= t.
+    out_row_map: int32 [qkv rows] (ape_attn_fwd_mapped): query row r is stored at row out_row_map[r] of `out` (required
+    then, [rows, heads*64] in qkv's dtype) and of the statistics ([out rows, heads, 2]); -1 stores nothing.  The mapped rows
+    must be distinct rows of `out`; rows no query maps to keep what `out` held."""
     _require(qkv.is_cuda and qkv.dim() == 2 and qkv.stride(1) == 1, "attention: qkv must be a 2-D CUDA tensor")
     stride = n if seq_stride is None else int(seq_stride)
     _require(qkv.shape[0] >= (num_seq - 1) * stride + (n_valid or n) and qkv.shape[1] == 3 * heads * head_dim, "attention: qkv shape")
-    # packed sequences leave the rows between n_valid and the stride unwritten; they come back as masked KEYS of the next
-    # layer, and 0 * NaN in P V would poison it: those rows must stay finite
-    alloc = torch.zeros if (stride < n or (n_valid is not None and n_valid < n)) else torch.empty
-    out = alloc((qkv.shape[0], heads * head_dim), dtype=qkv.dtype, device=qkv.device)
-    stats = torch.empty((qkv.shape[0], heads, 2), dtype=torch.float32, device=qkv.device) if stats_out else None
+    C = heads * head_dim
+    if out_row_map is not None:
+        _require(out_row_map.is_cuda and out_row_map.dtype == torch.int32 and out_row_map.dim() == 1 and
+                 out_row_map.is_contiguous() and out_row_map.numel() >= (num_seq - 1) * stride + min(stride, n),
+                 "attention: out_row_map must be a contiguous int32 CUDA vector with one entry per query row")
+        _require(out is not None and out.is_cuda and out.dim() == 2 and out.dtype == qkv.dtype and out.shape[1] == C and
+                 out.stride(1) == 1, "attention: out_row_map needs `out` [rows, heads*head_dim] in qkv's dtype")
+    else:
+        _require(out is None, "attention: `out` is only taken with out_row_map")
+        # packed sequences leave the rows between n_valid and the stride unwritten; they come back as masked KEYS of the next
+        # layer, and 0 * NaN in P V would poison it: those rows must stay finite
+        alloc = torch.zeros if (stride < n or (n_valid is not None and n_valid < n)) else torch.empty
+        out = alloc((qkv.shape[0], C), dtype=qkv.dtype, device=qkv.device)
+    stats = torch.empty((out.shape[0], heads, 2), dtype=torch.float32, device=qkv.device) if stats_out else None
+    args = (qkv.data_ptr(), qkv.stride(0), out.data_ptr(), out.stride(0), int(num_seq), int(n), int(n if n_valid is None else n_valid),
+            int(heads), int(head_dim), float(scale), _lib.dtype_code(qkv.dtype), stats.data_ptr() if stats is not None else None,
+            stride, 1 if causal else 0, int(qkv.shape[0]))
     with torch.cuda.device(qkv.device), _timed(("attention", num_seq, n, heads)):
-        rc = _lib.lib.ape_attn_fwd_ex(qkv.data_ptr(), qkv.stride(0), out.data_ptr(), out.stride(0), int(num_seq), int(n),
-                                      int(n if n_valid is None else n_valid), int(heads), int(head_dim), float(scale),
-                                      _lib.dtype_code(qkv.dtype), stats.data_ptr() if stats is not None else None,
-                                      stride, 1 if causal else 0, int(qkv.shape[0]), _lib.current_stream_ptr())
+        if out_row_map is None:
+            rc = _lib.lib.ape_attn_fwd_ex(*args, _lib.current_stream_ptr())
+        else:
+            rc = _lib.lib.ape_attn_fwd_mapped(*args, out_row_map.data_ptr(), _lib.current_stream_ptr())
     _lib.check(rc, "ape_attn_fwd")
     return (out, stats) if stats_out else out
 

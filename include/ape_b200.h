@@ -263,6 +263,14 @@ int ape_attn_fwd(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_se
 int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
                     int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
                     void *stream);
+/* ape_attn_fwd_ex with a scattered output: out_row_map (int32, device, one entry per query row of the launch, i.e.
+ * (num_seq - 1) * seq_stride + the rows stored per sequence) gives the row of out and of stats_out that query row r is
+ * stored at; -1 leaves nothing written for that row.  Lets the padded 14x14 windows of the APE-Ti ViT (vit_eva02.py)
+ * write their attention output straight back into raster token order, skipping the pad tokens.  Mapped rows must lie
+ * inside out / stats_out and be distinct. */
+int ape_attn_fwd_mapped(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                        int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
+                        const int *out_row_map, void *stream);
 
 /* Kernel structure behind ape_attn_fwd*: 0 = P written to shared memory and read from there by the P.V wgmma, 1 = P kept in
  * registers as the A operand of the P.V wgmma.  set >= 0 selects it for the process; returns the value in force
