@@ -130,6 +130,14 @@ def _declare(lib):
     lib.ape_resample_coeffs_u8.argtypes = [_i, _i, _vp, _vp]
     lib.ape_resample_u8.restype = _i
     lib.ape_resample_u8.argtypes = [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _vp, _vp, _i] + [_i] * 6 + [_vp]
+    lib.ape_semseg_resample.restype = _i
+    lib.ape_semseg_resample.argtypes = [_vp, _vp, _vp, _i64] + [_i] * 13 + [_vp]
+    lib.ape_semseg_keys_init.restype = _i
+    lib.ape_semseg_keys_init.argtypes = [_vp, _i64, ctypes.c_float, _i, _vp]
+    lib.ape_gemm_tn_argmax.restype = _i
+    lib.ape_gemm_tn_argmax.argtypes = [_vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp]
+    lib.ape_semseg_keys_decode.restype = _i
+    lib.ape_semseg_keys_decode.argtypes = [_vp, _i64, _vp, _vp, _vp]
 
 
 
@@ -181,6 +189,10 @@ EXPORTS = (
     "ape_resample_ksize",
     "ape_resample_coeffs_u8",
     "ape_resample_u8",
+    "ape_semseg_resample",
+    "ape_semseg_keys_init",
+    "ape_gemm_tn_argmax",
+    "ape_semseg_keys_decode",
 )
 
 

@@ -107,6 +107,21 @@ __device__ __forceinline__ void stg_stream_v4(uint4 *p, uint4 v) {
                : "memory");
 }
 
+// ---- class-argmax keys (semantic label maps: gemm_tc.cu EpiArgmax, semseg.cu) ---------------------
+// (order-preserving bits of the fp32 value) << 32 | (0xFFFFFFFF - column): the unsigned maximum of such keys is the largest
+// value and, among equal values, the lowest column, i.e. torch.argmax.  -0 is folded into +0 (argmax compares them equal).
+__host__ __device__ __forceinline__ unsigned long long argmax_key_bits(uint32_t u, uint32_t col) {
+  const uint32_t o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)o << 32) | (0xFFFFFFFFu - col);
+}
+__device__ __forceinline__ unsigned long long argmax_key(float v, int col) {
+  return argmax_key_bits(__float_as_uint(v + 0.f), (uint32_t)col);
+}
+__device__ __forceinline__ float argmax_key_value(unsigned long long key) {
+  const uint32_t o = (uint32_t)(key >> 32);
+  return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
+}
+
 // element traits: conversion of packed 16-bit pairs to fp32 and back.
 template <typename T>
 struct Elem;

@@ -76,6 +76,8 @@ struct GemmParams {
   // development aid (ape_gemm_set_trace): 8 clock64 stamps per CTA — 0 entry, 1 set-up done, 2 first operands landed,
   // 3 last MMA issued, 4 first accumulator complete, 5 last accumulator complete, 6 epilogue drained, 7 exit
   long long *trace;
+  // class-argmax epilogue (EpiArgmax): C is the u64 key per row; output column n stands for class n + argmax_col_base
+  int argmax_col_base;
 };
 
 __device__ __forceinline__ void trace_stamp(const GemmParams &p, int slot) {
@@ -235,6 +237,44 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
   }
 }
 
+// Class-argmax epilogue of the semantic label maps (semseg.cu): rows are pixels, columns classes, and nothing is stored but
+// the running maximum of each row.  A thread takes the first maximum over its 2 x BN/8 columns of a row, the quad (the four
+// threads that share the row) combines by shuffles, and one 64-bit atomicMax per (row, tile) merges it into the u64 key of
+// the row (argmax_key: larger value first, then lower class, so the key is torch.argmax over all column tiles).
+struct EpiArgmax {
+  static constexpr bool out32 = true, ln = false, rope = false, stats = false;
+  static constexpr int act = ACT_NONE, res = RES_NONE;
+};
+template <class E>
+constexpr bool kArgmax = std::is_same<E, EpiArgmax>::value;
+
+template <int BN>
+__device__ __forceinline__ void argmax_epilogue(const GemmParams &p, const float *acc, int m_blk, int n_blk, int wg, int lane) {
+  const int warp4 = (threadIdx.x >> 5) & 3, tq = lane & 3;
+  const int c_base = n_blk * BN + 2 * tq;
+  unsigned long long *keys = reinterpret_cast<unsigned long long *>(p.C);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m_blk * BM + wg * 64 + warp4 * 16 + (lane >> 2) + 8 * h;
+    float best = -INFINITY;
+    int col = -1;  // -1: no column of this thread lies inside N
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {  // columns in increasing order, strict >: the first maximum
+      const int n = c_base + 8 * j;
+      const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (n < p.N && (col < 0 || v0 > best)) { best = v0; col = n; }
+      if (n + 1 < p.N && v1 > best) { best = v1; col = n + 1; }
+    }
+#pragma unroll
+    for (int s = 1; s <= 2; s <<= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, s);
+      const int oc = __shfl_xor_sync(0xffffffffu, col, s);
+      if (oc >= 0 && (col < 0 || ob > best || (ob == best && oc < col))) { best = ob; col = oc; }
+    }
+    if (tq == 0 && col >= 0 && m < p.M) atomicMax(keys + m, argmax_key(best, col + p.argmax_col_base));
+  }
+}
+
 // CL = cluster size along M (1 or 2).  With CL == 2 the two CTAs of a cluster work on vertically adjacent 128-row tiles
 // of the same BN-column block: each loads half of the B (weight) tile and TMA-multicasts it into both CTAs' shared
 // memory, which halves the weight traffic from L2 per CTA.  A stage may only be refilled when the consumers of BOTH CTAs
@@ -356,7 +396,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if (t == 0) trace_stamp(p, 4);
         trace_stamp(p, 5);
       }
-      if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) epilogue<E, TI, BN, true>(p, acc, m_blk, n_blk, wg, lane);
+      if constexpr (kArgmax<E>) argmax_epilogue<BN>(p, acc, m_blk, n_blk, wg, lane);
+      else if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) epilogue<E, TI, BN, true>(p, acc, m_blk, n_blk, wg, lane);
       else epilogue<E, TI, BN, false>(p, acc, m_blk, n_blk, wg, lane);
     }
     if (threadIdx.x == 0) trace_stamp(p, 6);
@@ -672,6 +713,35 @@ extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const flo
   p.conv_W = W; p.conv_H = H;
   const EpiKey key{false, act, RES_NONE, false, false, false};
   return launch_any(bn, cluster, dtype, key, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// keys[m] = max over n of argmax_key((A W^T)[m, n], n + col_base): the class argmax of every pixel row, merged into keys that
+// the caller initialised (ape_semseg_keys_init).  Single-CTA BN = 128 kernel; K is the padded number of kept queries.
+extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, int N, int K,
+                                  int col_base, int in_dtype, void *stream) {
+  if (in_dtype != APE_DTYPE_F16 && in_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_INVALID_ARG, "gemm_argmax: operands must be fp16 or bf16 (got dtype %d)", in_dtype);
+  if (M < 0 || N <= 0 || K <= 0 || col_base < 0 || (long long)col_base + N > 0x7fffffffLL)
+    return fail(APE_ERR_INVALID_ARG, "gemm_argmax: bad sizes M=%d N=%d K=%d col_base=%d", M, N, K, col_base);
+  if (M == 0) return APE_OK;
+  if (!A || !W || !keys) return fail(APE_ERR_NULL_PTR, "gemm_argmax: null pointer argument");
+  if ((lda * 2) % 16 || (ldw * 2) % 16 || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15))
+    return fail(APE_ERR_INVALID_ARG, "gemm_argmax: A/W base and row pitch must be 16-byte aligned (TMA)");
+  if (lda < K || ldw < K) return fail(APE_ERR_INVALID_ARG, "gemm_argmax: row pitch smaller than K");
+  if (reinterpret_cast<uintptr_t>(keys) & 7) return fail(APE_ERR_INVALID_ARG, "gemm_argmax: keys must be 8-byte aligned");
+  constexpr int bn = 128;
+  CUtensorMap ma, mb;
+  if (int rc = make_map(&ma, A, in_dtype, M, K, lda, BM)) return rc;
+  if (int rc = make_map(&mb, W, in_dtype, N, K, ldw, bn)) return rc;
+  GemmParams p{};
+  p.C = keys; p.M = M; p.N = N; p.K = K;
+  p.m_blocks = (M + BM - 1) / BM;
+  p.k_blocks = (K + BK - 1) / BK;
+  p.trace = g_gemm_trace;
+  p.argmax_col_base = col_base;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiArgmax>(ma, mb, p, st);
+  return launch_gemm<bn, 6, 1, __half, EpiArgmax>(ma, mb, p, st);
 }
 
 extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,

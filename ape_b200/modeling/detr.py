@@ -283,6 +283,10 @@ class DeformableDETRSegmVL(nn.Module):
         # computed on the device from the 128 x 128 masks (what the evaluators encode every mask into: d3_evaluation.py:466-468),
         # 314 MB of booleans per 300 detections at 1024^2 that are never written or copied
         self.mask_format = "bitmask"
+        # "maps": `sem_seg` [N_classes, H, W] fp32 scores as the reference returns them; "label": `sem_seg_label` int64 [H, W] (the
+        # first argmax over classes of that map, all SemSegEvaluator keeps) and `sem_seg_score` fp32 [H, W] (its value).  On CUDA
+        # with a 16-bit engine_dtype the map is never formed (csrc/semseg.cu: 5 GB per image at 1203 classes and 1024^2)
+        self.sem_seg_format = "maps"
         self.semantic_post_nms = semantic_post_nms
         self.panoptic_post_nms = panoptic_post_nms
         self.panoptic_configs = panoptic_configs if panoptic_configs is not None else {
@@ -577,7 +581,7 @@ class DeformableDETRSegmVL(nn.Module):
         shared_keep = [r.query_index for r in results] if (instance_on and det_cls is box_cls and results is not None) else None
         if semantic_on:
             for o, sem in zip(out, self._semantic(box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep)):
-                o["sem_seg"] = sem
+                o.update(sem)
         if panoptic_on:
             for o, pan in zip(out, self._panoptic(box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep)):
                 o["panoptic_seg"] = pan
@@ -757,7 +761,11 @@ class DeformableDETRSegmVL(nn.Module):
 
     def _semantic(self, box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep=None):
         """Semantic branch (:628-666, `_postprocess_semantic` :875-918): class scores of the queries that survive the
-        detection NMS, softmax(sigmoid / 0.06) over classes, times the sigmoid masks at padded-image resolution."""
+        detection NMS, softmax(sigmoid / 0.06) over classes, times the sigmoid masks at padded-image resolution.  One dict per
+        image: {"sem_seg"} or, with sem_seg_format "label", {"sem_seg_label", "sem_seg_score"} (see __init__)."""
+        fmt = getattr(self, "sem_seg_format", "maps")
+        if fmt not in ("maps", "label"):
+            raise ValueError(f"ape_b200: sem_seg_format must be 'maps' or 'label' (got {fmt!r})")
         name = self.dataset_names[self.eval_dataset_id] if self.dataset_names else None
         things, stuff, entity = self.dataset_stuff.get(name, (None, None, "thing"))
         sem_cls = get_stuff_score(box_cls, things or [], stuff or [], entity)
@@ -770,7 +778,19 @@ class DeformableDETRSegmVL(nn.Module):
             keep = [torch.arange(sem_cls.shape[1], device=sem_cls.device)] * sem_cls.shape[0]
         for b, (qi, size, inp) in enumerate(zip(keep, image_sizes, batched_inputs)):
             cls = F.softmax(sem_cls[b, qi].float().sigmoid() / 0.06, dim=-1)
-            if self.engine_dtype in (torch.float16, torch.bfloat16) and mask_pred.is_cuda and len(qi) > 0:
+            h, w = inp.get("height", size[0]), inp.get("width", size[1])
+            class0 = None  # (:655-664) the "things" column of a stuff dataset is a constant
+            if entity == "stuff" and stuff and stuff[0] == "things" and self.stuff_prob_thing > 0:
+                class0 = math.log(self.stuff_prob_thing / (1 - self.stuff_prob_thing))
+            engine = self.engine_dtype in (torch.float16, torch.bfloat16) and mask_pred.is_cuda
+            if fmt == "label" and engine:
+                # engine: resample the kept masks once at the output size and take the class argmax in the GEMM epilogue
+                # (csrc/semseg.cu); the [N, H, W] map below is never formed
+                label, score = ops.semseg_label(mask_pred[b].contiguous(), qi, cls.to(self.engine_dtype), padded_hw, size, (h, w),
+                                                class0)
+                outs.append({"sem_seg_label": label, "sem_seg_score": score})
+                continue
+            if engine and len(qi) > 0:
                 # engine: einsum("qc,qhw->chw") (757 GFLOP at K = 300 kept queries x 1203 names x 1024^2) as ONE wgmma GEMM:
                 # the resize runs channels_last so that the sigmoid masks come out pixel-major [H*W, K] = the K-major operand
                 dt = self.engine_dtype
@@ -788,11 +808,13 @@ class DeformableDETRSegmVL(nn.Module):
             else:
                 m = F.interpolate(mask_pred[b, qi][None].float(), size=padded_hw, mode="bilinear", align_corners=False)[0].sigmoid()
                 result = torch.einsum("qc,qhw->chw", cls, m)  # stays on the GPU (the reference moves >1000 classes to the CPU, :896-898)
-            h, w = inp.get("height", size[0]), inp.get("width", size[1])
             sem = sem_seg_postprocess(result, size, h, w)
-            if entity == "stuff" and stuff and stuff[0] == "things" and self.stuff_prob_thing > 0:
-                sem[0, ...] = math.log(self.stuff_prob_thing / (1 - self.stuff_prob_thing))
-            outs.append(sem)
+            if class0 is not None:
+                sem[0, ...] = class0
+            if fmt == "label":  # the reference definition of the label map (first maximal class, as torch.argmax)
+                outs.append({"sem_seg_label": sem.argmax(0), "sem_seg_score": sem.amax(0)})
+            else:
+                outs.append({"sem_seg": sem})
         return outs
 
     def _panoptic(self, box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep=None):

@@ -704,6 +704,69 @@ def paste_masks_rle(masks, boxes, image_shape, threshold=0.5):
     return out
 
 
+SEMSEG_BAND_BYTES = 256 << 20  # bound of the resampled-operand workspace of semseg_label
+
+
+def semseg_label(mask_logits, query_index, cls, padded_hw, img_hw, out_hw, class0_const=None, band_bytes=None):
+    """Semantic label map of one image without the class-score maps: (label int64 [out_h, out_w], score fp32 [out_h, out_w]) =
+    the argmax over classes, and its value, of
+
+        sem_seg_postprocess(einsum("qc,qhw->chw", cls, F.interpolate(mask_logits[query_index][None], padded_hw,
+                            "bilinear").sigmoid()[0]), img_hw, *out_hw)          (class 0 set to class0_const if given)
+
+    (deformable_detr_segm_vl.py:875-918 + detectron2 sem_seg_postprocess + the evaluator's argmax).  Both resizes are linear,
+    so the class contraction runs at the output resolution: bands of output rows are resampled once into a pixel-major 16-bit
+    operand (ape_semseg_resample, at most `band_bytes`, default SEMSEG_BAND_BYTES) and contracted with cls^T by the wgmma GEMM
+    whose epilogue keeps only the per-pixel argmax (ape_gemm_tn_argmax).  Nothing of size classes x pixels is ever written.
+
+    mask_logits [Q, h, w] CUDA fp32 / fp16 / bf16; query_index int64 [K]; cls [K, N] fp16 / bf16 (the operand dtype: the
+    class weights of the kept queries); class0_const: the constant of class 0 (stuff_prob_thing), which then stays out of the
+    GEMM.  Ties resolve to the lowest class, as torch.argmax.  The band workspace comes from PyTorch's caching allocator, so a
+    captured CUDA graph keeps it in the graph's own pool."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 3 and mask_logits.is_contiguous(), "semseg_label: contiguous CUDA logits [Q,h,w]")
+    _require(cls.dim() == 2 and cls.dtype in (torch.float16, torch.bfloat16), "semseg_label: cls must be fp16 / bf16 [K, N]")
+    dev = mask_logits.device
+    K, N = int(cls.shape[0]), int(cls.shape[1])
+    _require(int(query_index.numel()) == K and N >= 1, "semseg_label: query_index [K] and cls [K, N >= 1] disagree")
+    Hp, Wp = int(padded_hw[0]), int(padded_hw[1])
+    ih, iw = int(img_hw[0]), int(img_hw[1])
+    oh, ow = int(out_hw[0]), int(out_hw[1])
+    _require(0 < ih <= Hp and 0 < iw <= Wp and oh > 0 and ow > 0, "semseg_label: bad image / output size")
+    P = oh * ow
+    keys = torch.empty((P,), dtype=torch.int64, device=dev)  # u64 keys (common.cuh argmax_key)
+    label = torch.empty((oh, ow), dtype=torch.int64, device=dev)
+    score = torch.empty((oh, ow), dtype=torch.float32, device=dev)
+    col_base = 0 if class0_const is None else 1
+    init = (float("-inf"), 0) if class0_const is None else (float(class0_const), 0)
+    if K == 0 and N > col_base and (class0_const is None or float(class0_const) < 0.0):
+        init = (0.0, col_base)  # no kept query: every class the GEMM would cover scores 0
+    stream = _lib.current_stream_ptr()
+    with torch.cuda.device(dev), _timed(("semseg_label", K, N, P)):
+        _lib.check(_lib.lib.ape_semseg_keys_init(keys.data_ptr(), P, init[0], init[1], stream), "ape_semseg_keys_init")
+        if K > 0:
+            Kp = (K + 7) // 8 * 8
+            dt = cls.dtype
+            w = torch.zeros((N - col_base, Kp), dtype=dt, device=dev)
+            w[:, :K] = cls[:, col_base:].t()
+            index = query_index.to(device=dev, dtype=torch.int64).contiguous()
+            budget = SEMSEG_BAND_BYTES if band_bytes is None else int(band_bytes)
+            rows = max(1, min(oh, budget // (ow * Kp * 2)))
+            ws = torch.empty((rows * ow, Kp), dtype=dt, device=dev)
+            for r0 in range(0, oh, rows):
+                nr = min(rows, oh - r0)
+                rc = _lib.lib.ape_semseg_resample(mask_logits.data_ptr(), index.data_ptr(), ws.data_ptr(), Kp, K,
+                                                  mask_logits.shape[1], mask_logits.shape[2], Hp, Wp, ih, iw, oh, ow, r0, nr,
+                                                  _lib.dtype_code(mask_logits.dtype), _lib.dtype_code(dt), stream)
+                _lib.check(rc, "ape_semseg_resample")
+                if N > col_base:
+                    rc = _lib.lib.ape_gemm_tn_argmax(ws.data_ptr(), Kp, w.data_ptr(), Kp, keys[r0 * ow:].data_ptr(), nr * ow,
+                                                     N - col_base, Kp, col_base, _lib.dtype_code(dt), stream)
+                    _lib.check(rc, "ape_gemm_tn_argmax")
+        _lib.check(_lib.lib.ape_semseg_keys_decode(keys.data_ptr(), P, label.data_ptr(), score.data_ptr(), stream),
+                   "ape_semseg_keys_decode")
+    return label, score
+
+
 _RESAMPLE_TABLES = {}
 
 

@@ -385,6 +385,31 @@ int ape_mask_paste_rle(const uint8_t *masks, const float *boxes, int N, int S, i
                        int *col_count, const int64_t *col_offset, int *positions, void *stream);
 int ape_rle_to_string(const uint32_t *counts, int m, char *out);
 
+/*
+ * Semantic label maps without the [N,H,W] class-score maps.  Replaces, for one image, the semantic tail of
+ * deformable_detr_segm_vl.py:875-918 (`_postprocess_semantic`: bilinear upsample of the kept mask logits to the padded size,
+ * sigmoid, einsum("qc,qhw->chw") with the class scores) + detectron2 sem_seg_postprocess (crop to the image, bilinear resize
+ * to the output size) + the evaluator's argmax over classes.  Both resizes are linear, so the class contraction runs at the
+ * output resolution on operands resampled once:
+ *   ape_semseg_resample     A [rows*out_w, lda] (a_dtype fp16 / bf16) for output rows [row0, row0+rows):
+ *                           A[p, k] = resize2(crop(sigmoid(resize1(logits[index[k]]))))(p), k < K; columns K..Kp-1 zero,
+ *                           Kp = K rounded up to 8 <= lda, lda a multiple of 8, A 16-byte aligned.  logits [Q,h,w]
+ *                           (logit_dtype fp32 / fp16 / bf16), index [K] int64; resize1 h x w -> Hp x Wp, crop img_h x img_w,
+ *                           resize2 -> out_h x out_w, both upsample_bilinear2d (align_corners=False) arithmetic in fp32.
+ *   ape_semseg_keys_init    keys [n] <- the key of (value, column): value = -INFINITY for "no class yet", or the constant
+ *                           class 0 takes (stuff_prob_thing, deformable_detr_segm_vl.py:655-664) with the GEMM started at class 1.
+ *   ape_gemm_tn_argmax      keys[m] = max(keys[m], max_n key((A W^T)[m, n], col_base + n)), A [M,K], W [N,K] (classes x
+ *                           padded queries) 16-bit of one dtype, same alignment rules as ape_gemm_tn; nothing else is stored.
+ *   ape_semseg_keys_decode  label [n] int64 = the class of keys[i], score [n] fp32 = its value.
+ * key(v, c) = (order-preserving bits of v) << 32 | (0xFFFFFFFF - c): ties resolve to the lowest class, as torch.argmax.
+ */
+int ape_semseg_resample(const void *logits, const int64_t *index, void *A, int64_t lda, int K, int h, int w, int Hp, int Wp,
+                        int img_h, int img_w, int out_h, int out_w, int row0, int rows, int logit_dtype, int a_dtype, void *stream);
+int ape_semseg_keys_init(uint64_t *keys, int64_t n, float value, int column, void *stream);
+int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, int N, int K, int col_base,
+                       int in_dtype, void *stream);
+int ape_semseg_keys_decode(const uint64_t *keys, int64_t n, int64_t *label, float *score, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
