@@ -6,6 +6,7 @@ APE_L_D   configs/LVISCOCOCOCOSTUFF_O365_OID_VGR_SA1B_REFCOCO_GQA_PhraseCut_Flic
           configs/COCO_InstanceSegmentation/ape_deta/models/ape_deta_r50.py:24-155 and
           configs/common/backbone/vitl_eva02_clip.py:9-48
 MINI      same architecture, toy sizes: used for golden fixtures small enough to commit.
+APE_L_B   APE-L_B and APE-L_C (vit_eva02.py ViT-L, no neck); MINI_EVA02L is its toy-size twin.
 """
 import copy
 
@@ -50,6 +51,25 @@ APE_TI["backbone"] = dict(
     out_channels=256, scale_factors=(4.0, 2.0, 1.0, 0.5), square_pad=1024,
 )
 
+# APE-L_B: configs/LVISCOCOCOCOSTUFF_O365_OID_VGR_REFCOCO/ape_deta/ape_deta_vitl_eva02_vlf_lsj1024_cp_1080k.py on top of
+# …_vlf_lsj1024_cp_720k.py:12-47 (VL classes, fusion layer), …_lsj1024_cp_720k.py:16-53 (1256 classes, top-300, no neck),
+# LVIS_InstanceSegmentation/ape_deta/ape_deta_vitl_eva02_lsj1024_cp_24ep.py and
+# COCO_InstanceSegmentation/ape_deta/ape_deta_vitl_eva02_lsj1024_cp_12ep.py:9-29,83-86 (backbone, neck = None, EVA01-CLIP
+# text features of width 1024) over models/ape_deta_r50.py.  APE-L_C (LVISCOCOCOCOSTUFF_O365_OID_VGR_SA1B_REFCOCO/…_1080k.py)
+# imports that model unchanged; only its criterion list (7 entries) differs, which shapes nothing but the non-persistent
+# features_phrase_bank.  Both configs also set semantic_on=True and stuff_prob_thing=0.9 (…_lsj1024_cp_720k.py:47-51):
+# the semantic branch is switched per run with `model.semantic_on`.
+APE_L_B = copy.deepcopy(APE_L_D)
+APE_L_B["name"] = "APE-L_B"
+APE_L_B["backbone"] = dict(
+    variant="eva02_subln",              # vit_eva02.py: subln=True, naiveswiglu=True (q/k/v projections, ffn_ln, no inner_attn_ln)
+    img_size=1024, patch_size=16, embed_dim=1024, depth=24, num_heads=16,
+    window_size=16, mlp_ratio=4 * 2 / 3, window_block_indexes=_window_blocks(24, every=6),  # vitl_eva02.py:10-27
+    pretrain_img_size=224, pt_hw_seq_len=16,  # vit_eva02.ViT defaults (:468-498): not set by the config
+    out_channels=256, scale_factors=(4.0, 2.0, 1.0, 0.5), square_pad=1024,  # vitl_eva02.py:35-40
+)
+APE_L_B.update(neck=None, num_classes=1256, proposal_ambiguous=0)  # …_lsj1024_cp_720k.py:16,53; deformable_transformer_vl.py:280
+
 MINI = dict(
     name="MINI",
     backbone=dict(
@@ -67,6 +87,13 @@ MINI = dict(
     test_topk=10, test_nms_thresh=0.7, test_score_thresh=0.0,
     pixel_mean=(123.675, 116.280, 103.530), pixel_std=(58.395, 57.120, 57.375),
 )
+
+# APE-L_B's structure at MINI sizes (no neck, proposal_ambiguous = 0, the vit_eva02.py sub-LN blocks): golden fixtures.
+# The pyramid's 64 channels are the encoder's width here, so embed_dim follows out_channels = 256 as in APE-L_B.
+MINI_EVA02L = copy.deepcopy(MINI)
+MINI_EVA02L["name"] = "MINI-EVA02L"
+MINI_EVA02L["backbone"].update(variant="eva02_subln", out_channels=256)
+MINI_EVA02L.update(neck=None, proposal_ambiguous=0)
 
 
 def level_shapes(spec):

@@ -10,6 +10,8 @@ from .detr import ChannelMapper, DeformableDETRSegmVL, PositionEmbeddingSine, So
 from .text import EVA02CLIP, TextTransformer  # noqa: F401
 from .transformer import (DeformableDetrTransformerDecoderVL, DeformableDetrTransformerEncoderVL,
                           DeformableDetrTransformerVL)
+from . import vit_eva02  # noqa: F401  (ape_b200.modeling.vit_eva02.ViT: drop-in for vit_eva02.py configs)
+from .vit_eva02 import ViT as VitEva02
 
 
 class SyntheticTextModel:
@@ -29,22 +31,27 @@ def build_model(spec, num_text=None):
     what detectron2's `instantiate(cfg.model.model_vision)` does from the LazyConfig tree, with
     `_target_`s pointing at this package (INTEGRATION.md)."""
     b = spec["backbone"]
-    net = ViT(img_size=b["img_size"], patch_size=b["patch_size"], embed_dim=b["embed_dim"], depth=b["depth"],
-              num_heads=b["num_heads"], drop_path_rate=0.0, window_size=b["window_size"], mlp_ratio=b["mlp_ratio"],
-              qkv_bias=True, norm_layer=partial(nn.LayerNorm, eps=1e-6), window_block_indexes=b["window_block_indexes"],
-              residual_block_indexes=[], use_rel_pos=True, out_feature="last_feat", use_act_checkpoint=False,
-              xattn=False, rope=True, pt_hw_seq_len=b["pt_hw_seq_len"], intp_freq=True,
-              naiveswiglu=b.get("variant", "eva_clip") == "eva_clip", subln=b.get("variant", "eva_clip") == "eva_clip",
-              swiglu=b.get("variant", "eva_clip") == "eva02",
-              pretrain_img_size=b["pretrain_img_size"], pretrain_use_cls_token=True)
+    variant = b.get("variant", "eva_clip")
+    # "eva_clip": vit_eva_clip.py (APE-L_D); "eva02": vit_eva02.py packed SwiGLU (APE-Ti); "eva02_subln": vit_eva02.py sub-LN
+    # blocks (APE-L_B / L_C), whose `subln` means no inner_attn_ln: the vit_eva02 class reads it so
+    vit_cls = VitEva02 if variant == "eva02_subln" else ViT
+    net = vit_cls(img_size=b["img_size"], patch_size=b["patch_size"], embed_dim=b["embed_dim"], depth=b["depth"],
+                  num_heads=b["num_heads"], drop_path_rate=0.0, window_size=b["window_size"], mlp_ratio=b["mlp_ratio"],
+                  qkv_bias=True, norm_layer=partial(nn.LayerNorm, eps=1e-6), window_block_indexes=b["window_block_indexes"],
+                  residual_block_indexes=[], use_rel_pos=True, out_feature="last_feat", use_act_checkpoint=False,
+                  xattn=False, rope=True, pt_hw_seq_len=b["pt_hw_seq_len"], intp_freq=True,
+                  naiveswiglu=variant != "eva02", subln=variant != "eva02", swiglu=variant == "eva02",
+                  pretrain_img_size=b["pretrain_img_size"], pretrain_use_cls_token=True)
     backbone = SimpleFeaturePyramid(net=net, in_feature="last_feat", out_channels=b["out_channels"],
                                     scale_factors=b["scale_factors"], top_block=LastLevelMaxPool(), norm="LN",
                                     square_pad=b["square_pad"])
     E = spec["embed_dim"]
     feats = ["p2", "p3", "p4", "p5", "p6"]
     shapes = {f: ShapeSpec(channels=b["out_channels"]) for f in feats}
-    neck = ChannelMapper(input_shapes=shapes, in_features=feats, out_channels=E, num_outs=5, kernel_size=1,
-                         norm_layer=nn.GroupNorm(num_groups=spec["gn_groups"], num_channels=E))
+    neck = None
+    if spec.get("neck", "ChannelMapper") is not None:
+        neck = ChannelMapper(input_shapes=shapes, in_features=feats, out_channels=E, num_outs=5, kernel_size=1,
+                             norm_layer=nn.GroupNorm(num_groups=spec["gn_groups"], num_channels=E))
     vl_layer = VisionLanguageFusion(v_dim=E, l_dim=spec["lang_dim"], embed_dim=spec["vlf_embed"],
                                     num_heads=spec["vlf_heads"], dropout=0.1, drop_path=0.0,
                                     init_values=spec["vlf_init"], stable_softmax_2d=True,

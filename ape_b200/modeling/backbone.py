@@ -1,4 +1,4 @@
-"""EVA-02 ViT backbone + SimpleFeaturePyramid of APE-L_D and APE-Ti.
+"""EVA-02 ViT backbone + SimpleFeaturePyramid of APE-L_D, APE-L_B / L_C (ape_b200.modeling.vit_eva02.ViT) and APE-Ti.
 
 Mirror of ape/modeling/backbone/vit_eva_clip.py (`ViT` :570-754, `Block` :383-567, `Attention`
 :135-319, `SwiGLU` :101-132, `SimpleFeaturePyramid` :757-922) and utils_eva02.py (`PatchEmbed`
@@ -115,15 +115,17 @@ class PackedSwiGLU(nn.Module):
 
 
 class Attention(nn.Module):
-    """subln=True: vit_eva_clip.py:135-319 (separate q/k/v projections + inner_attn_ln, APE-L);
-    subln=False: vit_eva02.py `Attention` (fused `qkv` projection, no inner norm, APE-Ti)."""
+    """subln=True: separate q/k/v projections; inner_ln=True adds vit_eva_clip.py's inner_attn_ln (:135-319, APE-L_D), which
+    vit_eva02.py's sub-LN Attention does not have (:206-291, APE-L_B / L_C); subln=False: vit_eva02.py's fused `qkv`
+    projection, no inner norm (APE-Ti).  inner_ln defaults to subln (the vit_eva_clip.py reading)."""
 
-    def __init__(self, dim, num_heads, rope, norm_layer, subln=True):
+    def __init__(self, dim, num_heads, rope, norm_layer, subln=True, inner_ln=None):
         super().__init__()
         self.num_heads = num_heads
         head_dim = dim // num_heads
         self.scale = head_dim ** -0.5
         self.subln = subln
+        self.inner_ln = subln if inner_ln is None else inner_ln
         if subln:
             self.q_proj = nn.Linear(dim, dim, bias=False)
             self.k_proj = nn.Linear(dim, dim, bias=False)
@@ -132,7 +134,7 @@ class Attention(nn.Module):
             self.qkv = nn.Linear(dim, dim * 3, bias=False)
         self.q_bias = nn.Parameter(torch.zeros(dim))
         self.v_bias = nn.Parameter(torch.zeros(dim))
-        if subln:
+        if self.inner_ln:
             self.inner_attn_ln = norm_layer(dim)
         self.proj = nn.Linear(dim, dim)
         self.rope = rope
@@ -156,16 +158,17 @@ class Attention(nn.Module):
         k = self.rope(k).type_as(v)
         o = F.scaled_dot_product_attention(q, k, v, dropout_p=0.0, scale=self.scale)
         o = o.permute(0, 2, 1, 3).reshape(B, N, -1)
-        if self.subln:
+        if self.inner_ln:
             o = self.inner_attn_ln(o)
         return self.proj(o).view(B, H, W, C)
 
 
 class Block(nn.Module):
-    def __init__(self, dim, num_heads, mlp_ratio, norm_layer, window_size, rope, subln=True, packed_swiglu=False):
+    def __init__(self, dim, num_heads, mlp_ratio, norm_layer, window_size, rope, subln=True, packed_swiglu=False,
+                 inner_ln=None):
         super().__init__()
         self.norm1 = norm_layer(dim)
-        self.attn = Attention(dim, num_heads, rope, norm_layer, subln=subln)
+        self.attn = Attention(dim, num_heads, rope, norm_layer, subln=subln, inner_ln=inner_ln)
         self.norm2 = norm_layer(dim)
         self.mlp = PackedSwiGLU(dim, int(dim * mlp_ratio)) if packed_swiglu else SwiGLU(dim, int(dim * mlp_ratio), norm_layer)
         self.window_size = window_size
@@ -184,6 +187,10 @@ class Block(nn.Module):
 
 
 class ViT(nn.Module):
+    # reference file whose meaning of `subln` this class follows: vit_eva_clip.py (inner_attn_ln) here, vit_eva02.py (none)
+    # in ape_b200.modeling.vit_eva02.ViT
+    _reference_file = "vit_eva_clip"
+
     def __init__(self, img_size=1024, patch_size=16, in_chans=3, embed_dim=768, depth=12, num_heads=12,
                  mlp_ratio=4.0, qkv_bias=False, qk_scale=None, drop_rate=0.0, attn_drop_rate=0.0, drop_path_rate=0.0,
                  norm_layer=partial(nn.LayerNorm, eps=1e-6), init_values=None, use_abs_pos=True, use_rel_pos=False,
@@ -192,13 +199,16 @@ class ViT(nn.Module):
                  pretrain_img_size=224, pretrain_use_cls_token=True, out_feature="last_feat", xattn=False,
                  frozen_stages=-1, swiglu=False):
         super().__init__()
-        variant_l = naiveswiglu and subln and not swiglu        # vit_eva_clip.py (APE-L_*: sub-LN, naive SwiGLU)
-        variant_ti = swiglu and not naiveswiglu and not subln   # vit_eva02.py   (APE-Ti: packed SwiGLU, fused qkv)
-        if not (rope and (variant_l or variant_ti) and qkv_bias and use_abs_pos and intp_freq) or postnorm or init_values \
-                or len(residual_block_indexes) or qk_scale is not None:
-            raise NotImplementedError("ape_b200.ViT implements the two EVA-02 configurations APE uses "
+        naive_subln = naiveswiglu and subln and not swiglu
+        variant_l = naive_subln and self._reference_file == "vit_eva_clip"  # APE-L_D: sub-LN with inner_attn_ln, naive SwiGLU
+        variant_lb = naive_subln and self._reference_file == "vit_eva02"    # APE-L_B / L_C: q/k/v projections, ffn_ln only
+        variant_ti = swiglu and not naiveswiglu and not subln                # APE-Ti: packed SwiGLU, fused qkv
+        if not (rope and (variant_l or variant_lb or variant_ti) and qkv_bias and use_abs_pos and intp_freq) or postnorm \
+                or init_values or len(residual_block_indexes) or qk_scale is not None:
+            raise NotImplementedError("ape_b200.ViT implements the three EVA-02 configurations APE uses "
                                       "(rope, qkv_bias, abs pos, intp_freq, pre-norm; naiveswiglu + subln, or packed swiglu)")
         self._variant_l = variant_l
+        self._flavour = "eva_clip" if variant_l else "eva02_subln" if variant_lb else "eva02_swiglu"
         self.pretrain_use_cls_token = pretrain_use_cls_token
         self.patch_embed = PatchEmbed((patch_size, patch_size), (patch_size, patch_size), in_chans=in_chans,
                                       embed_dim=embed_dim)
@@ -209,7 +219,8 @@ class ViT(nn.Module):
         self.rope_glb = VisionRotaryEmbeddingFast(half, pt_hw_seq_len, img_size // patch_size)
         self.blocks = nn.ModuleList([
             Block(embed_dim, num_heads, mlp_ratio, norm_layer, window_size if i in window_block_indexes else 0,
-                  self.rope_win if i in window_block_indexes else self.rope_glb, subln=variant_l, packed_swiglu=variant_ti)
+                  self.rope_win if i in window_block_indexes else self.rope_glb, subln=not variant_ti, packed_swiglu=variant_ti,
+                  inner_ln=variant_l)
             for i in range(depth)])
         # RoPE in the qkv GEMM's epilogue (ape_gemm_tn_rope) instead of the in-place ape_rope_qk pass: measured slower twice
         # (+26 us per GEMM with the general epilogue, +27 us with a lean one: per-thread cos / sin rows are 32 different lines per
@@ -266,6 +277,9 @@ class ViT(nn.Module):
         g = x.shape[-1] // ps
         if self._variant_l:
             return x.shape[-1] == x.shape[-2] and (ws == 0 or g % ws == 0)
+        if self._flavour == "eva02_subln":  # window-major path of APE-L_D, RoPE tables of this grid
+            return x.shape[-1] == x.shape[-2] and x.shape[-1] % ps == 0 and (ws == 0 or g % ws == 0) and \
+                self.rope_glb.freqs_cos.shape[0] == g * g
         # APE-Ti raster path: any window size (windows are padded), 64-channel heads for the attention kernel, and the global
         # RoPE table of this grid
         C, heads = self.pos_embed.shape[-1], self.blocks[0].attn.num_heads
@@ -274,7 +288,7 @@ class ViT(nn.Module):
 
     def _pack(self, dtype, device):
         """Weights re-laid out once for the kernels (fused qkv, interleaved SwiGLU pairs, K padded to 8)."""
-        key = (str(device), tuple(p._version for p in self.parameters()))
+        key = (str(device), self.fold_sub_layernorms, tuple(p._version for p in self.parameters()))
         packs = self.__dict__.setdefault("_packs", {})  # one entry per engine dtype, never evicted (ops.cached)
         if dtype in packs and packs[dtype][0] == key:
             return packs[dtype][1]
@@ -286,6 +300,9 @@ class ViT(nn.Module):
             packed["patch_b"] = self.patch_embed.proj.bias.to(**f32).contiguous()
             for blk in self.blocks:
                 a, m = blk.attn, blk.mlp
+                if self._flavour == "eva02_subln":
+                    packed["blocks"].append(self._pack_block_eva02_subln(blk, dtype, device))
+                    continue
                 if self._variant_l:
                     wqkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0)
                     w1, w2, b1, b2 = m.w1.weight, m.w2.weight, m.w1.bias, m.w2.bias
@@ -323,6 +340,33 @@ class ViT(nn.Module):
                          b3_ln=(m.w3.weight.float() @ m.ffn_ln.bias.float() + m.w3.bias.float()).to(**f32).contiguous())
         packs[dtype] = (key, packed)
         return packed
+
+    def _pack_block_eva02_subln(self, blk, dtype, device):
+        """vit_eva02.py sub-LN block (APE-L_B / L_C): fused [q; k; v] weight, plain proj (no inner_attn_ln), interleaved
+        SwiGLU pairs, and w3 with ffn_ln folded in (or ffn_ln and w3 apart when fold_sub_layernorms is off)."""
+        f32 = dict(dtype=torch.float32, device=device)
+        a, m = blk.attn, blk.mlp
+        hid = m.w1.weight.shape[0]
+        hid_p = (hid + 7) // 8 * 8
+        w12 = torch.stack([m.w1.weight, m.w2.weight], 1).reshape(2 * hid, -1)  # rows (w1_j, w2_j)
+        b12 = torch.stack([m.w1.bias, m.w2.bias], 1).reshape(2 * hid)
+        d = dict(
+            n1w=blk.norm1.weight.to(**f32), n1b=blk.norm1.bias.to(**f32),
+            wqkv=torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0).to(device, dtype).contiguous(),
+            bqkv=torch.cat([a.q_bias, torch.zeros_like(a.v_bias), a.v_bias]).to(**f32).contiguous(),
+            wproj=a.proj.weight.to(device, dtype).contiguous(), bproj=a.proj.bias.to(**f32).contiguous(),
+            n2w=blk.norm2.weight.to(**f32), n2b=blk.norm2.bias.to(**f32),
+            w12=w12.to(device, dtype).contiguous(), b12=b12.to(**f32).contiguous(), hid=hid, hid_p=hid_p)
+        w3 = torch.zeros(m.w3.weight.shape[0], hid_p, dtype=dtype, device=device)
+        if self.fold_sub_layernorms:  # gamma .* W3 as the operand, its row sums, beta W3^T + b3 as the bias
+            w3[:, :hid] = (m.w3.weight.float() * m.ffn_ln.weight.float()[None, :]).to(dtype)
+            d.update(w3_ln=w3, s3=w3.float().sum(1).contiguous(),
+                     b3_ln=(m.w3.weight.float() @ m.ffn_ln.bias.float() + m.w3.bias.float()).to(**f32).contiguous())
+        else:
+            w3[:, :hid] = m.w3.weight
+            d.update(w3=w3, b3=m.w3.bias.to(**f32).contiguous(),
+                     fw=m.ffn_ln.weight.to(**f32).contiguous(), fb=m.ffn_ln.bias.to(**f32).contiguous())
+        return d
 
     def _geometry(self, B, g, ws, dtype, device):
         """Per input geometry: window-major token permutation, abs-pos table, RoPE position maps."""
@@ -362,7 +406,7 @@ class ViT(nn.Module):
         return self._engine_tokens(img).permute(0, 3, 1, 2)  # NCHW view over NHWC memory (channels_last)
 
     def _engine_tokens(self, img):
-        if not self._variant_l:
+        if self._flavour == "eva02_swiglu":
             return self._engine_tokens_raster(img)
         B, _, Hh, Ww = img.shape
         ps = self.patch_embed.proj.kernel_size[0]
@@ -407,10 +451,11 @@ class ViT(nn.Module):
                     ops.rope_qk_(qkv, rope_glb[0], rope_glb[1], C, hd, pos_map=geo["glb_map"])
                 nb, n = B, g * g
             fold = self.fold_sub_layernorms
+            stats = fold and self._variant_l  # statistics only feed the inner_attn_ln fold
             if self.engine_attention and ops.attention_supported(n, hd, qkv.dtype):
-                # wgmma flash attention, no head-split copies; with `fold` it also leaves per-(row, head) statistics
-                o = ops.attention_qkv(qkv, nb, n, heads, hd, blk.attn.scale, stats_out=fold)
-                o, st = o if fold else (o, None)
+                # wgmma flash attention, no head-split copies; with `stats` it also leaves per-(row, head) statistics
+                o = ops.attention_qkv(qkv, nb, n, heads, hd, blk.attn.scale, stats_out=stats)
+                o, st = o if stats else (o, None)
             else:
                 q5 = qkv.view(nb, n, 3, heads, hd)
                 o = F.scaled_dot_product_attention(q5[:, :, 0].transpose(1, 2), q5[:, :, 1].transpose(1, 2),
@@ -419,6 +464,8 @@ class ViT(nn.Module):
             if st is not None:  # inner_attn_ln folded into proj: the raw attention output is the GEMM operand
                 x = ops.linear_tc(o, p["wproj_ln"], p["bproj_ln"], residual=x, out_dtype=torch.float32,
                                   ln_fold=(st, p["sproj"], C, 1e-6))
+            elif not self._variant_l:  # vit_eva02.py sub-LN block: no inner_attn_ln
+                x = ops.linear_tc(o, p["wproj"], p["bproj"], residual=x, out_dtype=torch.float32)
             else:
                 a = ops.layernorm(o, p["lnw"], p["lnb"], eps=1e-6)
                 x = ops.linear_tc(a, p["wproj"], p["bproj"], residual=x, out_dtype=torch.float32)
@@ -562,6 +609,11 @@ class SimpleFeaturePyramid(nn.Module):
         self._square_pad = square_pad
         # 3x3 convolutions on the repo's implicit-GEMM kernel (ape_conv3x3_nhwc) instead of cuDNN
         self.conv3x3_engine = os.environ.get("APE_CONV3X3", "1") == "1"
+        # Engine path for a model without a neck (DeformableDETRSegmVL(neck=None) sets it): every level's final LayerNorm, and
+        # the p6 subsample, write into their slice of one [B, S, C] buffer (`last_flat`), the flattened levels the encoder
+        # consumes (deformable_transformer_vl.py:435-452); the returned levels are views of it
+        self.flat_output = False
+        self.last_flat = None
 
     @property
     def size_divisibility(self):
@@ -588,12 +640,28 @@ class SimpleFeaturePyramid(nn.Module):
             cache[key] = (b * (4 * g * g) + (2 * y + dy) * (2 * g) + 2 * x + dx).reshape(-1).to(device, torch.int32)
         return cache[key]
 
+    def _flat_map(self, B, S, start, n, device):
+        """LayerNorm output rows of one level in the flat [B*S, C] buffer: row (b, r) -> b * S + start + r."""
+        key = ("flat", B, S, start, n, str(device))
+        cache = self.__dict__.setdefault("_maps", {})
+        if key not in cache:
+            b, r = torch.meshgrid(torch.arange(B), torch.arange(n), indexing="ij")
+            cache[key] = (b * S + start + r).reshape(-1).to(device, torch.int32)
+        return cache[key]
+
     def _engine_forward(self, img):
         tok = self.net._engine_tokens(img)  # [B, g, g, C]
         B, g, _, C = tok.shape
         dt, dev = tok.dtype, tok.device
         results = {}
-        for scale, seq, name in zip(self.scale_factors, self.stages, self._out_features):
+        flat = None
+        if self.flat_output:
+            sides = [int(g * s) for s in self.scale_factors]
+            sides.append((sides[-1] + 1) // 2)  # LastLevelMaxPool: kernel 1, stride 2
+            starts = [sum(h * h for h in sides[:i]) for i in range(len(sides) + 1)]
+            flat = torch.empty((B, starts[-1], self._out_feature_channels[self._out_features[0]]), dtype=dt, device=dev)
+        self.last_flat = flat
+        for li, (scale, seq, name) in enumerate(zip(self.scale_factors, self.stages, self._out_features)):
             mods = list(seq)
             if scale == 4.0:
                 ct1, ln, _, ct2, c1, c3 = mods
@@ -632,8 +700,20 @@ class SimpleFeaturePyramid(nn.Module):
             ch = y.shape[-1]
             z = conv3x3_tokens(c3, y, B, hw, hw, self.conv3x3_engine)
             nw, nb = ops.packed(c3.norm, dt)
+            if flat is not None:
+                s0, n = starts[li], hw * hw
+                ops.layernorm(z.view(-1, ch), nw, nb, eps=c3.norm.eps, row_map=self._flat_map(B, starts[-1], s0, n, dev),
+                              out=flat.view(-1, ch))
+                results[name] = flat[:, s0:s0 + n].view(B, hw, hw, ch).permute(0, 3, 1, 2)
+                continue
             z = ops.layernorm(z.view(-1, ch), nw, nb, eps=c3.norm.eps)
             results[name] = z.view(B, hw, hw, ch).permute(0, 3, 1, 2)
+        if flat is not None:  # p6 = p5[::2, ::2] into the last slice
+            h5, h6 = sides[-2], sides[-1]
+            p6 = flat[:, starts[-2]:starts[-1]].view(B, h6, h6, -1)
+            p6.copy_(flat[:, starts[-3]:starts[-2]].view(B, h5, h5, -1)[:, ::2, ::2])
+            results[self._out_features[len(self.stages)]] = p6.permute(0, 3, 1, 2)
+            return {n: results[n] for n in self._out_features}
         top = self.top_block(results[self.top_block.in_feature])
         for n, t in zip(self._out_features[len(self.stages):], top):
             results[n] = t
@@ -643,6 +723,7 @@ class SimpleFeaturePyramid(nn.Module):
         if x.is_cuda and x.dtype in (torch.float16, torch.bfloat16) and hasattr(self.net, "_engine_ok") \
                 and self.net._engine_ok(x) and isinstance(self.top_block, LastLevelMaxPool):
             return self._engine_forward(x)
+        self.last_flat = None
         feats = self.net(x)
         f = feats[self.in_feature]
         results = [stage(f) for stage in self.stages]

@@ -232,6 +232,10 @@ class DeformableDETRSegmVL(nn.Module):
                 or last_class_embed_use_mlp:
             raise NotImplementedError("ape_b200: only the two-stage, box-refine, VisionLanguageAlign configuration")
         self.backbone, self.position_embedding, self.neck, self.transformer = backbone, position_embedding, neck, transformer
+        if neck is None and hasattr(backbone, "flat_output"):
+            # no neck (APE-L_B / L_C, …_lsj1024_cp_720k.py:53): the backbone's levels are the encoder input, so its engine
+            # path writes them straight into the flattened [B, S, C] buffer the encoder consumes
+            backbone.flat_output = True
         self.num_queries, self.num_classes = num_queries, num_classes
         self.embed_dim_language = embed_dim_language
         nd = transformer.decoder.num_layers
@@ -598,7 +602,8 @@ class DeformableDETRSegmVL(nn.Module):
         key = (tuple(batch_shape), tuple(image_sizes))
         geo = self._geo_cache.get(key)
         if geo is None:
-            strides = [self.backbone._out_feature_strides[f] for f in self.neck.in_features]
+            levels = self.neck.in_features if self.neck is not None else self.backbone._out_features  # (:375-378)
+            strides = [self.backbone._out_feature_strides[f] for f in levels]
             H, W = batch_shape[-2], batch_shape[-1]
             shapes = [(-(-H // s), -(-W // s)) for s in strides]
             masks = [F.interpolate(img_masks[None], size=sh).to(torch.bool).squeeze(0) for sh in shapes]
@@ -625,9 +630,14 @@ class DeformableDETRSegmVL(nn.Module):
 
     def _stage_encode(self, images, fusion, geo, mask_prompt_flatten=None):
         features = self.backbone(images.to(self.engine_dtype))
-        feats = self.neck({f: features[f] for f in self.neck.in_features})
+        if self.neck is not None:
+            feats = self.neck({f: features[f] for f in self.neck.in_features})
+            flat = getattr(self.neck, "last_flat", None)
+        else:  # (:375-378) the levels are the backbone's output dict in order
+            feats = tuple(features.values())
+            flat = getattr(self.backbone, "last_flat", None)
         memory, fusion_out, output_memory, enc_cls, enc_coord = self.transformer.stage_encode(
-            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=getattr(self.neck, "last_flat", None))
+            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=flat)
         mask_features = None
         if self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on):
             mask_features = self.maskdino_mask_features(memory, features, geo)

@@ -64,11 +64,14 @@ class _SelfAttention(nn.Module):
             NP = (N + 127) // 128 * 128
             C = nh * 64
             # padded rows must be finite (zeros): they are never written, so one zero-filled buffer per geometry serves every call
-            # (a fresh torch.zeros here was a fill kernel per layer inside the captured graph)
+            # (a fresh torch.zeros here was a fill kernel per layer inside the captured graph).  Never evicted: a captured graph
+            # reads its buffer without owning it, so replacing the entry when the dtype or batch changed freed memory that the
+            # graph of the previous geometry still replays on
             bk = (B, NP, C, x.dtype, str(x.device))
-            if getattr(self, "_qkv_buf", (None,))[0] != bk:
-                self._qkv_buf = (bk, torch.zeros((B, NP, 3 * C), dtype=x.dtype, device=x.device))
-            buf = self._qkv_buf[1]
+            bufs = self.__dict__.setdefault("_qkv_bufs", {})
+            if bk not in bufs:
+                bufs[bk] = torch.zeros((B, NP, 3 * C), dtype=x.dtype, device=x.device)
+            buf = bufs[bk]
             xp = x + pos.to(x.dtype)
             for b in range(B):
                 ops.linear_tc(xp[b], wqk, bqk, out=buf[b, :N, : 2 * C])
