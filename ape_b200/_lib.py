@@ -71,6 +71,8 @@ def _declare(lib):
     lib.ape_conv3x3_nhwc.argtypes = [_vp, _vp, _vp, _vp] + [_i] * 7 + [_vp]
     lib.ape_gemm_set_trace.restype = None
     lib.ape_gemm_set_trace.argtypes = [_vp]
+    lib.ape_ffn_fused.restype = _i
+    lib.ape_ffn_fused.argtypes = [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64] + [_i] * 5 + [_vp]
     lib.ape_gemm_tn_rope.restype = _i
     lib.ape_gemm_tn_rope.argtypes = [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp]
 
@@ -161,6 +163,7 @@ EXPORTS = (
     "ape_gemm_tn_fused",
     "ape_conv3x3_nhwc",
     "ape_gemm_tn_rope",
+    "ape_ffn_fused",
     "ape_gemm_set_trace",
     "ape_layernorm",
     "ape_layernorm_ex",

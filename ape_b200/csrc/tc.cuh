@@ -99,6 +99,12 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
 }
 
+// ---- register reallocation between warpgroups (every thread of the warpgroup executes it) ----------
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- wgmma ------------------------------------------------------------------------------------------
 // A warpgroup (4 consecutive warps, the first with warp index % 4 == 0) issues D (+)= A * B with M = 64.  The fp32
 // accumulator fragment of m64nN: thread (warp w of the group, lane l) holds d[4 j + e] = D[16 w + l/4 + 8 (e >> 1)]

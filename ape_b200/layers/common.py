@@ -75,9 +75,15 @@ class FFN(nn.Module):
         if x.is_cuda and x.dtype in (torch.float16, torch.bfloat16):
             from .. import ops  # tensor-core path: ReLU and the residual add live in the GEMM epilogues
 
-            h = ops.linear_module_tc(self.layers[0][0], x, act="relu")
+            fc1, fc2 = self.layers[0][0], self.layers[1]
+            if out_dtype == torch.float32 and x.shape[-1] == 256 and fc1.out_features % 64 == 0:
+                # one kernel, the [tokens, feedforward_dim] hidden activation never reaches memory; same bits as below
+                w1, b1 = ops.packed(fc1, x.dtype)
+                w2, b2 = ops.packed(fc2, x.dtype)
+                return ops.ffn_fused(x, w1, b1, w2, b2)
+            h = ops.linear_module_tc(fc1, x, act="relu")
             # out_dtype float32: the sum x + ffn(x) leaves the epilogue unrounded (it feeds a LayerNorm)
-            return ops.linear_module_tc(self.layers[1], h, residual=x.contiguous(), out_dtype=out_dtype)
+            return ops.linear_module_tc(fc2, h, residual=x.contiguous(), out_dtype=out_dtype)
         return x + self.layers[1](F.relu(self.layers[0][0](x)))
 
 

@@ -255,6 +255,42 @@ def linear_tc(x, weight, bias=None, act=None, out_dtype=None, residual=None, til
     return (res, stats) if stats_out else res
 
 
+def ffn_fused(x, w1, b1, w2, b2, out=None, variant=0):
+    """x + relu(x @ w1.T + b1) @ w2.T + b2 in one launch (ape_ffn_fused), fp32 [..., 256]; the hidden activation stays on chip.
+
+    x [..., 256] and w1 [F, 256], w2 [256, F] (nn.Linear layouts) fp16/bf16 of one dtype, F a multiple of 64; b1 / b2 fp32 or
+    None.  The result is bit-identical to linear_tc(x, w1, b1, act="relu") followed by linear_tc(h, w2, b2, residual=x,
+    out_dtype=float32).  out: optional fp32 [M, 256] with unit inner stride (any even row pitch).  variant: 0 default,
+    1 single CTA, 2 cluster of two (A/B runs)."""
+    _require(x.is_cuda and w1.is_cuda and w2.is_cuda, "ffn_fused: CUDA tensors only")
+    _require(x.dtype in (torch.float16, torch.bfloat16) and w1.dtype == x.dtype and w2.dtype == x.dtype,
+             "ffn_fused: fp16/bf16 operands of one dtype")
+    E = x.shape[-1]
+    F = w1.shape[0]
+    _require(w1.dim() == 2 and w2.dim() == 2 and tuple(w1.shape) == (F, E) and tuple(w2.shape) == (E, F) and
+             w1.stride(1) == 1 and w2.stride(1) == 1, "ffn_fused: w1 must be [F, E] and w2 [E, F] with unit inner stride")
+    for b, n in ((b1, F), (b2, E)):
+        _require(b is None or (b.dtype == torch.float32 and b.is_contiguous() and b.numel() == n), "ffn_fused: biases fp32 [F] / [E]")
+    x2 = x.reshape(-1, E)
+    if x2.stride(1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
+        x2 = x2.contiguous()
+    M = x2.shape[0]
+    if out is None:
+        out = torch.empty((M, E), dtype=torch.float32, device=x.device)
+        res = out.view(*x.shape[:-1], E)
+    else:
+        _require(out.dtype == torch.float32 and out.dim() == 2 and tuple(out.shape) == (M, E) and out.stride(1) == 1 and out.is_cuda,
+                 "ffn_fused: out must be fp32 [M, E] with unit inner stride")
+        res = out
+    with torch.cuda.device(x.device), _timed(("ffn_fused", M, E, F)):
+        rc = _lib.lib.ape_ffn_fused(x2.data_ptr(), x2.stride(0), w1.data_ptr(), w1.stride(0),
+                                    b1.data_ptr() if b1 is not None else None, w2.data_ptr(), w2.stride(0),
+                                    b2.data_ptr() if b2 is not None else None, out.data_ptr(), out.stride(0), M, E, F,
+                                    _lib.dtype_code(x.dtype), int(variant), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_ffn_fused")
+    return res
+
+
 def conv3x3_supported(H, W, Cin, Cout, dtype):
     if dtype not in (torch.float16, torch.bfloat16) or Cin % 64 or Cout % 8:
         return False

@@ -193,6 +193,19 @@ int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, voi
                      const int *pos_map, int npos, int head_dim, int rope_cols, int tile_n, void *stream);
 
 /*
+ * The transformer FFN block (detrex FFN(num_fcs=2): Linear -> ReLU -> Linear + identity) in one launch:
+ *   out[M, E] (fp32) = relu(x w1^T + b1) w2^T + b2 + x
+ * x [M, E] (pitch ldx), w1 [F, E] (pitch ldw1), w2 [E, F] (pitch ldw2) 16-bit of one dtype in nn.Linear's layouts, 16-byte
+ * aligned bases and pitches; b1 fp32 [F], b2 fp32 [E] (NULL = no bias); out fp32, pitch ldo (0 = E), 8-byte pairs.
+ * E must be 256 and F a multiple of 64 (APE_ERR_UNSUPPORTED otherwise).  The [M, F] hidden activation stays on chip; the
+ * result equals ape_gemm_tn_ex(x, w1, act relu, 16-bit out) followed by ape_gemm_tn_ex(h, w2, + b2, 16-bit residual x, fp32 out)
+ * bit for bit.  variant: 0 = default (= 1), 1 = one CTA per 128-row tile, 2 = clusters of two row tiles sharing the weight
+ * chunks by TMA multicast (A/B runs).
+ */
+int ape_ffn_fused(const void *x, int64_t ldx, const void *w1, int64_t ldw1, const float *b1, const void *w2, int64_t ldw2,
+                  const float *b2, float *out, int64_t ldo, int M, int E, int F, int dtype, int variant, void *stream);
+
+/*
  * Development aid (no reference counterpart): when device_buffer is not NULL, every CTA of the following ape_gemm_tn*
  * launches writes 8 clock64() stamps to device_buffer[8 * blockIdx.x ..]:
  * entry, set-up done, first operands landed, last MMA issued, first / last accumulator complete, epilogue drained, exit.
