@@ -15,6 +15,8 @@
 //                          then bias / activation / residual / rotary / LayerNorm fold in registers and direct stores
 //   warp 8     producer  : STAGES-deep ring of {A 128x64, B BNx64} 16-bit tiles, mbarrier full/empty; it runs ahead
 //                          into the next tile's k-blocks while the consumers finish the epilogue of the current one
+// gemm_pp_kernel is the ping-pong form of the same kernel for single-CTA BN = 128 GEMMs with many tiles: each consumer
+// warpgroup owns whole tiles, and their main loops alternate so that one's epilogue runs under the other's MMAs.
 #include <stdlib.h>
 
 #include <type_traits>
@@ -407,6 +409,149 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) trace_stamp(p, 7);
 }
 
+// Ping-pong variant (single CTA, BN = 128, 384 threads): the same operand ring and the same epilogues, but each consumer
+// warpgroup owns whole 128 x 128 tiles — warpgroup g takes the CTA's tiles t with t % 2 == g — so one warpgroup's epilogue
+// runs while the other's MMAs keep the tensor cores busy.
+//   warps 0-7   consumers : warpgroup g, 128 accumulators per thread (two m64n128 halves: tile rows 0-63 and 64-127)
+//   warps 8-11  producer  : one thread issues TMA; the warpgroup gives its registers to the consumers (setmaxnreg works
+//                           per warpgroup, hence a whole warpgroup)
+// Synchronisation rules:
+//  1. mbar_wait(bar, parity) passes as soon as the barrier is not in phase `parity`, so a wait for a phase one ahead of
+//     the barrier's current one passes on a stage TMA has not written.  Each warpgroup skips the other's k-blocks (K = 256
+//     with 6 stages: warpgroup 1's first tile uses stages 4, 5, 0, 1), so (stage, phase) come from the CTA's running
+//     k-block index t * k_blocks + kb, never from a counter per warpgroup, and the order handoff (rule 2) makes a
+//     warpgroup wait on the full barriers of tile t only after the other has passed its waits of tile t - 1: every
+//     earlier fill of the stage has then landed, and the next one needs this warpgroup's release.
+//  2. Order handoff on named barriers kOrderBar + g (256 threads: one warpgroup waits with bar.sync, the other arrives):
+//     warpgroup g starts the main loop of tile t only after the other warpgroup has issued the last MMA of tile t - 1.
+//     Every arrive (after tile t, if tile t + 1 exists) is matched by the sync before tile t + 1.
+//  3. empty[i] counts 4 arrivals, one per warp of the single warpgroup that reads the stage.
+//  4. The epilogue takes warp4 from threadIdx.x (consumers keep warps 0-7) and the row half from its `wg` argument.
+//     trace_stamp slots keep their meaning; thread 0 belongs to warpgroup 0.
+//  5. PDL as in gemm_tc_kernel: launch_dependents at entry, griddepcontrol.wait before the first TMA load and store.
+constexpr int kPpThreads = 32 * kConsumerWarps + 128;
+constexpr int kOrderBar = 1;  // named barriers 1 and 2
+
+template <typename TI, class E>
+__global__ void __launch_bounds__(kPpThreads, 1)
+gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+  constexpr int BN = 128, STAGES = 6;
+  extern __shared__ uint8_t smem_raw[];
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) trace_stamp(p, 0);
+  using Smem = GemmSmem<BN, STAGES>;
+  Smem &s = *reinterpret_cast<Smem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr uint32_t STAGE_BYTES = (BM + BN) * BK * 2;
+
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  // the tile order of gemm_tc_kernel with CL = 1 (grouped raster in bands of p.band row blocks, row block fastest)
+  const int num_tiles = p.m_blocks * p.n_blocks;
+  auto tile_at = [&](int t, int &m_blk, int &n_blk) -> bool {
+    const int tile = blockIdx.x + t * gridDim.x;
+    if (tile >= num_tiles) return false;
+    const int per_band = p.band * p.n_blocks;
+    const int band = tile / per_band, r = tile - band * per_band;
+    const int rows = min(p.band, p.m_blocks - band * p.band);
+    n_blk = r / rows;
+    m_blk = band * p.band + r - n_blk * rows;
+    return true;
+  };
+
+  if (warp == kConsumerWarps && lane == 0) {
+    tc::prefetch_tensormap(&map_a);
+    tc::prefetch_tensormap(&map_b);
+#pragma unroll
+    for (int i = 0; i < STAGES; ++i) {
+      tc::mbar_init(&s.full[i], 1);
+      tc::mbar_init(&s.empty[i], 4);  // rule 3
+    }
+    tc::fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  if (threadIdx.x == 0) trace_stamp(p, 1);
+
+  if (warp >= kConsumerWarps) {
+    // ===================== TMA producer: every tile of the CTA in order, one ring =====================
+    tc::setmaxnreg_dec<40>();  // 40 x 128 + 232 x 256 <= the 168 x 384 registers of the launch
+    if (warp == kConsumerWarps && lane == 0) {
+      uint32_t stage = 0, phase = 0;
+      int m_blk, n_blk;
+      for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
+        for (int kb = 0; kb < p.k_blocks; ++kb) {
+          tc::mbar_wait(&s.empty[stage], phase ^ 1);
+          tc::mbar_expect_tx(&s.full[stage], STAGE_BYTES);
+          tc::tma_load_2d(s.a[stage], &map_a, &s.full[stage], kb * BK, m_blk * BM);
+          tc::tma_load_2d(s.b[stage], &map_b, &s.full[stage], kb * BK, n_blk * BN);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else {
+    // ===================== consumers: warpgroup wg, tiles wg, wg + 2, ... =====================
+    tc::setmaxnreg_inc<232>();  // 128 accumulators
+    const int wg = warp / 4;
+    float acc[BN];  // acc[0, 64): tile rows 0-63, acc[64, 128): rows 64-127
+#pragma unroll
+    for (int i = 0; i < BN; ++i) acc[i] = 0.f;
+    auto release = [&](uint32_t st) {  // the MMAs that read stage `st` have completed (in this warp's view of the group)
+      if (lane == 0) tc::mbar_arrive(&s.empty[st]);
+    };
+    int m_blk, n_blk;
+    for (int t = wg; tile_at(t, m_blk, n_blk); t += 2) {
+      if (t > 0) tc::named_bar_sync(kOrderBar + wg, 256);  // rule 2: the other warpgroup issued tile t - 1
+      const uint32_t g0 = (uint32_t)t * p.k_blocks;       // rule 1: the CTA's running k-block index
+      uint32_t stage = g0 % STAGES, phase = (g0 / STAGES) & 1, prev = 0;
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        tc::mbar_wait(&s.full[stage], phase);
+        if (kb == 0 && t == 0 && threadIdx.x == 0) trace_stamp(p, 2);
+        const uint64_t da = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage]));
+        const uint64_t da_hi = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage] + 64 * BK * 2));
+        const uint64_t db = tc::make_smem_desc_sw128(tc::smem_u32(s.b[stage]));
+        tc::fence_regs<BN>(acc);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WG_K; ++k) {
+          tc::Wgmma<BN, TI>::template ss<0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+          tc::Wgmma<BN, TI>::template ss<0>(acc + 64, da_hi + 2 * k, db + 2 * k, (kb | k) != 0);
+        }
+        tc::wgmma_commit();
+        tc::fence_regs<BN>(acc);
+        if (kb > 0) {
+          tc::wgmma_wait<1>();
+          release(prev);
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      int m_nx, n_nx;
+      if (tile_at(t + 1, m_nx, n_nx)) tc::named_bar_arrive(kOrderBar + (wg ^ 1), 256);  // rule 2: hand over
+      tc::wgmma_wait<0>();
+      tc::fence_regs<BN>(acc);
+      release(prev);
+      if (threadIdx.x == 0) {
+        trace_stamp(p, 3);
+        if (t == 0) trace_stamp(p, 4);
+        trace_stamp(p, 5);
+      }
+      if constexpr (kArgmax<E>) {
+        argmax_epilogue<BN>(p, acc, m_blk, n_blk, 0, lane);
+        argmax_epilogue<BN>(p, acc + 64, m_blk, n_blk, 1, lane);
+      } else if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) {
+        epilogue<E, TI, BN, true>(p, acc, m_blk, n_blk, 0, lane);
+        epilogue<E, TI, BN, true>(p, acc + 64, m_blk, n_blk, 1, lane);
+      } else {
+        epilogue<E, TI, BN, false>(p, acc, m_blk, n_blk, 0, lane);
+        epilogue<E, TI, BN, false>(p, acc + 64, m_blk, n_blk, 1, lane);
+      }
+    }
+    if (threadIdx.x == 0) trace_stamp(p, 6);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) trace_stamp(p, 7);
+}
+
 // ---- host ----------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -452,11 +597,13 @@ int num_sms() {
   return n;
 }
 
-template <int BN, int STAGES, int CL, typename TI, class E>
+// PP: the ping-pong kernel (BN = 128, STAGES = 6, CL = 1 only)
+template <int BN, int STAGES, int CL, typename TI, class E, bool PP = false>
 int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+  static_assert(!PP || (BN == 128 && STAGES == 6 && CL == 1), "gemm_pp_kernel is BN = 128, 6 stages, single CTA");
   using Smem = GemmSmem<BN, STAGES>;
   const size_t smem = sizeof(Smem) + 1024;
-  auto k = gemm_tc_kernel<BN, STAGES, CL, TI, E>;
+  auto k = PP ? gemm_pp_kernel<TI, E> : gemm_tc_kernel<BN, STAGES, CL, TI, E>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -473,7 +620,7 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cud
   p.band = std::min(m_groups, (clusters + p.n_blocks - 1) / p.n_blocks);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(clusters * CL));
-  cfg.blockDim = dim3(kThreads);
+  cfg.blockDim = dim3(PP ? kPpThreads : kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
@@ -491,9 +638,12 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cud
 }
 
 // 4 stages of 48 KB (BN = 256) or 6 of 32 KB (BN = 128): 192 KB of the 227 KB a block may use.
+// pp: the ping-pong kernel (gemm_impl selects it only for bn = 128 without a cluster)
 template <int CL, typename TI, class E>
-int launch_bn(int bn, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+int launch_bn(int bn, bool pp, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
   if (bn == 256) return launch_gemm<256, 4, CL, TI, E>(ma, mb, p, st);
+  if constexpr (CL == 1)
+    if (pp) return launch_gemm<128, 6, 1, TI, E, true>(ma, mb, p, st);
   return launch_gemm<128, 6, CL, TI, E>(ma, mb, p, st);
 }
 
@@ -527,22 +677,26 @@ struct EpiKey {
   X(true, ACT_NONE, RES_16, false, false, false) X(true, ACT_NONE, RES_F32, true, false, false)
 
 template <int CL, typename TI>
-int launch_epi(int bn, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
+int launch_epi(int bn, bool pp, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cudaStream_t st) {
 #define APE_EPI_CASE(o, a, r, l, ro, s)                                                                                  \
   if (k.out32 == o && k.act == a && k.res == r && k.ln == l && k.rope == ro && k.stats == s)                           \
-    return launch_bn<CL, TI, Epi<o, a, r, l, ro, s>>(bn, ma, mb, p, st);
+    return launch_bn<CL, TI, Epi<o, a, r, l, ro, s>>(bn, pp, ma, mb, p, st);
   APE_GEMM_EPILOGUES(APE_EPI_CASE)
 #undef APE_EPI_CASE
   return fail(APE_ERR_UNSUPPORTED, "gemm: no kernel for the epilogue (fp32 out %d, act %d, residual %d, ln %d, rope %d, stats %d)",
               (int)k.out32, k.act, k.res, (int)k.ln, (int)k.rope, (int)k.stats);
 }
 
-int launch_any(int bn, bool cluster, int in_dtype, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p,
-               cudaStream_t st) {
+int launch_any(int bn, bool cluster, bool pp, int in_dtype, const EpiKey &k, const CUtensorMap &ma, const CUtensorMap &mb,
+               GemmParams &p, cudaStream_t st) {
   if (in_dtype == APE_DTYPE_BF16)
-    return cluster ? launch_epi<2, __nv_bfloat16>(bn, k, ma, mb, p, st) : launch_epi<1, __nv_bfloat16>(bn, k, ma, mb, p, st);
-  return cluster ? launch_epi<2, __half>(bn, k, ma, mb, p, st) : launch_epi<1, __half>(bn, k, ma, mb, p, st);
+    return cluster ? launch_epi<2, __nv_bfloat16>(bn, false, k, ma, mb, p, st) : launch_epi<1, __nv_bfloat16>(bn, pp, k, ma, mb, p, st);
+  return cluster ? launch_epi<2, __half>(bn, false, k, ma, mb, p, st) : launch_epi<1, __half>(bn, pp, k, ma, mb, p, st);
 }
+
+// Ping-pong pays off when most CTAs get a tile for each consumer warpgroup; with fewer tiles (the 900-row decoder
+// GEMMs) the cooperative kernel, which splits one tile over both warpgroups, finishes a CTA's single tile sooner.
+bool use_pingpong(int tiles) { return tiles >= 2 * num_sms(); }
 
 }  // namespace
 }  // namespace ape
@@ -595,8 +749,14 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
   // kernel variant: single CTA, or a cluster of 2 along M sharing the weight tile by TMA multicast.  The cluster pays off
   // when the K loop is long (K >= 2048: w3, FFN2, the 3x3 convolutions), where the weight tile is the larger share of the
   // operand traffic; bit 0x1000 forces the single CTA, bit 0x4000 the cluster.
+  // A single-CTA BN = 128 GEMM runs the ping-pong kernel when there are enough tiles (use_pingpong); bit 0x8000 forces
+  // it (single CTA), bit 0x10000 forces the cooperative kernel.
+  const bool force_pp = (tile_n & 0x8000) != 0, force_coop = (tile_n & 0x10000) != 0;
+  if (force_pp && (force_coop || bn != 128 || (tile_n & 0x4000)))
+    return fail(APE_ERR_INVALID_ARG, "gemm: tile_n flag 0x8000 (ping-pong) needs tile width 128, no cluster and no 0x10000");
   const int m_blocks = (M + BM - 1) / BM;
-  const bool cluster = m_blocks >= 2 && (tile_n & 0x1000) == 0 && ((tile_n & 0x4000) != 0 || K >= 2048);
+  const bool cluster = m_blocks >= 2 && !force_pp && (tile_n & 0x1000) == 0 && ((tile_n & 0x4000) != 0 || K >= 2048);
+  const bool pp = !cluster && bn == 128 && !force_coop && (force_pp || use_pingpong(m_blocks * ((N + bn - 1) / bn)));
   CUtensorMap ma, mb;
   if (int rc = make_map(&ma, A, in_dtype, M, K, lda, BM)) return rc;
   if (int rc = make_map(&mb, W, in_dtype, N, K, ldw, cluster ? bn / 2 : bn)) return rc;
@@ -639,7 +799,7 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
       return fail(APE_ERR_INVALID_ARG, "gemm+rope: needs a 16-bit output, no activation, rope_cols a multiple of 64 <= N");
     p.rope_cos = rope->cos; p.rope_sin = rope->sin; p.rope_pos = rope->pos; p.rope_cols = rope->cols; p.rope_npos = rope->npos;
   }
-  return launch_any(bn, cluster, in_dtype, key, ma, mb, p, st);
+  return launch_any(bn, cluster, pp, in_dtype, key, ma, mb, p, st);
 }
 
 extern "C" int ape_gemm_tn(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,
@@ -712,7 +872,7 @@ extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const flo
   p.conv = 1; p.conv_tw = tw; p.conv_th = th; p.conv_tiles_x = W / tw; p.conv_tiles_img = (W / tw) * (H / th); p.conv_cblks = Cin / 64;
   p.conv_W = W; p.conv_H = H;
   const EpiKey key{false, act, RES_NONE, false, false, false};
-  return launch_any(bn, cluster, dtype, key, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_any(bn, cluster, false, dtype, key, ma, mb, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // keys[m] = max over n of argmax_key((A W^T)[m, n], n + col_base): the class argmax of every pixel row, merged into keys that
@@ -740,6 +900,10 @@ extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int
   p.trace = g_gemm_trace;
   p.argmax_col_base = col_base;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (use_pingpong(p.m_blocks * ((N + bn - 1) / bn))) {
+    if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiArgmax, true>(ma, mb, p, st);
+    return launch_gemm<bn, 6, 1, __half, EpiArgmax, true>(ma, mb, p, st);
+  }
   if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiArgmax>(ma, mb, p, st);
   return launch_gemm<bn, 6, 1, __half, EpiArgmax>(ma, mb, p, st);
 }

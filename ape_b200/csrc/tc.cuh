@@ -105,6 +105,16 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
+// ---- named barriers (ID 0 is __syncthreads) ---------------------------------------------------------
+// bar.sync blocks until `threads` threads have arrived (its own warp included); bar.arrive counts the calling warp and
+// returns at once.  `threads` is a multiple of 32.
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ---- wgmma ------------------------------------------------------------------------------------------
 // A warpgroup (4 consecutive warps, the first with warp index % 4 == 0) issues D (+)= A * B with M = 64.  The fp32
 // accumulator fragment of m64nN: thread (warp w of the group, lane l) holds d[4 j + e] = D[16 w + l/4 + 8 (e >> 1)]
