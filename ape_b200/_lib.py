@@ -10,8 +10,9 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libape_b200.so")
 
-APE_DTYPE_F32, APE_DTYPE_F16, APE_DTYPE_BF16 = 0, 1, 2
-_DTYPE_CODE = {torch.float32: APE_DTYPE_F32, torch.float16: APE_DTYPE_F16, torch.bfloat16: APE_DTYPE_BF16}
+APE_DTYPE_F32, APE_DTYPE_F16, APE_DTYPE_BF16, APE_DTYPE_E4M3 = 0, 1, 2, 3
+_DTYPE_CODE = {torch.float32: APE_DTYPE_F32, torch.float16: APE_DTYPE_F16, torch.bfloat16: APE_DTYPE_BF16,
+               torch.float8_e4m3fn: APE_DTYPE_E4M3}
 
 # APE_B200_CONTAINER_ONLY=1: import the package for its parameter containers / configs only (bench.py's CPU reference arm
 # builds the reference-named state_dict this way) WITHOUT mapping the native library; every kernel entry point then raises.
@@ -67,6 +68,8 @@ def _declare(lib):
     lib.ape_gemm_tn_ex.argtypes = [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64] + [_i] * 8 + [_vp]
     lib.ape_gemm_tn_fused.restype = _i
     lib.ape_gemm_tn_fused.argtypes = [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64] + [_i] * 8 + [_vp, _i, _vp, ctypes.c_float, ctypes.c_float, _vp, _i, _vp]
+    lib.ape_gemm_tn_e4m3.restype = _i
+    lib.ape_gemm_tn_e4m3.argtypes = [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]
     lib.ape_conv3x3_nhwc.restype = _i
     lib.ape_conv3x3_nhwc.argtypes = [_vp, _vp, _vp, _vp] + [_i] * 7 + [_vp]
     lib.ape_gemm_set_trace.restype = None
@@ -78,6 +81,8 @@ def _declare(lib):
 
     lib.ape_layernorm.restype = _i
     lib.ape_layernorm.argtypes = [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i, _i, ctypes.c_float, _i, _i, _vp]
+    lib.ape_layernorm_e4m3.restype = _i
+    lib.ape_layernorm_e4m3.argtypes = [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i, _i, ctypes.c_float, _i, _vp]
     lib.ape_layernorm_ex.restype = _i
     lib.ape_layernorm_ex.argtypes = [_vp, _i64, _vp, _i64, _vp, _vp, ctypes.c_float, _vp, _vp, ctypes.c_float, _vp, _i64, _i,
                                      _vp, _i64, _vp, _i64, _i, _i, _i, _i, _vp]
@@ -161,11 +166,13 @@ EXPORTS = (
     "ape_gemm_tn",
     "ape_gemm_tn_ex",
     "ape_gemm_tn_fused",
+    "ape_gemm_tn_e4m3",
     "ape_conv3x3_nhwc",
     "ape_gemm_tn_rope",
     "ape_ffn_fused",
     "ape_gemm_set_trace",
     "ape_layernorm",
+    "ape_layernorm_e4m3",
     "ape_layernorm_ex",
     "ape_rope_qk",
     "ape_attn_fwd",
@@ -203,7 +210,7 @@ def dtype_code(dt: torch.dtype) -> int:
     try:
         return _DTYPE_CODE[dt]
     except KeyError:
-        raise RuntimeError(f"ape_b200: unsupported dtype {dt} (float32 / float16 / bfloat16 only)") from None
+        raise RuntimeError(f"ape_b200: unsupported dtype {dt} (float32 / float16 / bfloat16 / float8_e4m3fn only)") from None
 
 
 def check(status: int, what: str) -> None:

@@ -552,6 +552,114 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) trace_stamp(p, 7);
 }
 
+// FP8 form (ape_gemm_tn_e4m3): e4m3 A [M, K] and W [N, K] with an fp32 scale per row of each, C = (A W^T) * a_scale[m] *
+// w_scale[n], then the epilogue E of the 16-bit kernels (TO: the 16-bit output type).  The shape of gemm_tc_kernel with
+// CL = 1, BN = 128: a 128-byte swizzle row holds 128 e4m3 values, so one k-block is 128 of K, the stage sizes are those of
+// the 16-bit kernel, and a warpgroup issues 4 x m64n128k32 per k-block.
+// Hopper's FP8 MMA does not keep full fp32 precision when it accumulates over a long K, so each k-block's 4 MMAs go into a
+// scratch fragment (the first with scale_d = 0) that is added to the fp32 accumulator in registers once they have
+// completed: one promotion per 128 of K, as CUTLASS's FP8 kernels without "fast accumulation" do.  The second fragment is
+// why this is the cooperative form (64 + 64 accumulators per thread); a ping-pong warpgroup already holds 128.
+constexpr int BK8 = 128;
+
+template <typename TO, class E>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p,
+                const float *__restrict__ a_scale, const float *__restrict__ w_scale) {
+  constexpr int BN = 128, STAGES = 6;
+  extern __shared__ uint8_t smem_raw[];
+  pdl_launch_dependents();
+  using Smem = GemmSmem<BN, STAGES>;  // BK x 16 bit = BK8 x 8 bit per row: the same bytes
+  Smem &s = *reinterpret_cast<Smem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr uint32_t STAGE_BYTES = (BM + BN) * BK8;
+
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int num_tiles = p.m_blocks * p.n_blocks;
+  auto tile_at = [&](int t, int &m_blk, int &n_blk) -> bool {  // gemm_tc_kernel's order with CL = 1
+    const int tile = blockIdx.x + t * gridDim.x;
+    if (tile >= num_tiles) return false;
+    const int per_band = p.band * p.n_blocks;
+    const int band = tile / per_band, r = tile - band * per_band;
+    const int rows = min(p.band, p.m_blocks - band * p.band);
+    n_blk = r / rows;
+    m_blk = band * p.band + r - n_blk * rows;
+    return true;
+  };
+
+  if (warp == kConsumerWarps && lane == 0) {
+    tc::prefetch_tensormap(&map_a);
+    tc::prefetch_tensormap(&map_b);
+#pragma unroll
+    for (int i = 0; i < STAGES; ++i) {
+      tc::mbar_init(&s.full[i], 1);
+      tc::mbar_init(&s.empty[i], kConsumerWarps);
+    }
+    tc::fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == kConsumerWarps) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      uint32_t stage = 0, phase = 0;
+      int m_blk, n_blk;
+      for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
+        for (int kb = 0; kb < p.k_blocks; ++kb) {
+          tc::mbar_wait(&s.empty[stage], phase ^ 1);
+          tc::mbar_expect_tx(&s.full[stage], STAGE_BYTES);
+          tc::tma_load_2d(s.a[stage], &map_a, &s.full[stage], kb * BK8, m_blk * BM);
+          tc::tma_load_2d(s.b[stage], &map_b, &s.full[stage], kb * BK8, n_blk * BN);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else {
+    // ===================== consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of the tile =====================
+    const int wg = warp / 4, warp4 = warp & 3, tq = lane & 3;
+    float acc[BN / 2], part[BN / 2];
+    uint32_t stage = 0, phase = 0;
+    int m_blk, n_blk;
+    for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        tc::mbar_wait(&s.full[stage], phase);
+        const uint64_t da = tc::make_smem_desc_sw128(tc::smem_u32(s.a[stage] + wg * 64 * BK8));
+        const uint64_t db = tc::make_smem_desc_sw128(tc::smem_u32(s.b[stage]));
+        tc::fence_regs<BN / 2>(part);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK8 / 32; ++k)  // 32 elements (32 B) along K per instruction
+          tc::Wgmma<BN, __nv_fp8_e4m3>::template ss<0>(part, da + 2 * k, db + 2 * k, k != 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::fence_regs<BN / 2>(part);
+        if (lane == 0) tc::mbar_arrive(&s.empty[stage]);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];  // promotion into the fp32 accumulator
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // dequantise: acc * a_scale[m] * w_scale[n] in fp32 (rows past M read row M - 1, columns past N scale by 0)
+      const int m0 = m_blk * BM + wg * 64 + warp4 * 16 + (lane >> 2);
+      const float sa0 = __ldg(a_scale + min(m0, p.M - 1)), sa1 = __ldg(a_scale + min(m0 + 8, p.M - 1));
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n_blk * BN + 8 * j + 2 * tq;
+        const float sw0 = n < p.N ? __ldg(w_scale + n) : 0.f, sw1 = n + 1 < p.N ? __ldg(w_scale + n + 1) : 0.f;
+        acc[4 * j] = acc[4 * j] * sa0 * sw0;
+        acc[4 * j + 1] = acc[4 * j + 1] * sa0 * sw1;
+        acc[4 * j + 2] = acc[4 * j + 2] * sa1 * sw0;
+        acc[4 * j + 3] = acc[4 * j + 3] * sa1 * sw1;
+      }
+      if (p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) epilogue<E, TO, BN, true>(p, acc, m_blk, n_blk, wg, lane);
+      else epilogue<E, TO, BN, false>(p, acc, m_blk, n_blk, wg, lane);
+    }
+  }
+  __syncthreads();
+}
+
 // ---- host ----------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -569,16 +677,18 @@ EncodeTiledFn get_encoder() {
   return fn;
 }
 
-// [rows, K] 16-bit row-major matrix with pitch `ld` elements; box = 64 (K) x box_rows, 128 B swizzle.
+// [rows, K] 16-bit row-major matrix with pitch `ld` elements; box = 64 (K) x box_rows, 128 B swizzle.  An e4m3 matrix
+// (APE_DTYPE_E4M3) is mapped as bytes, and its box of box_cols = BK8 elements is the same 128-byte row.
 int make_map(CUtensorMap *map, const void *base, int dtype, long long rows, long long K, long long ld, int box_rows,
              int box_cols = BK) {
   EncodeTiledFn enc = get_encoder();
   if (!enc) return fail(APE_ERR_UNSUPPORTED, "gemm: cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * (dtype == APE_DTYPE_F32 ? 4 : 2)};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * (dtype == APE_DTYPE_F32 ? 4 : dtype == APE_DTYPE_E4M3 ? 1 : 2)};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(map, dtype == APE_DTYPE_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                        : dtype == APE_DTYPE_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                         : dtype == APE_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
                    const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -697,6 +807,36 @@ int launch_any(int bn, bool cluster, bool pp, int in_dtype, const EpiKey &k, con
 // Ping-pong pays off when most CTAs get a tile for each consumer warpgroup; with fewer tiles (the 900-row decoder
 // GEMMs) the cooperative kernel, which splits one tile over both warpgroups, finishes a CTA's single tile sooner.
 bool use_pingpong(int tiles) { return tiles >= 2 * num_sms(); }
+
+template <typename TO, class E>
+int launch_fp8(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, const float *a_scale, const float *w_scale,
+               cudaStream_t st) {
+  constexpr int BN = 128;
+  const size_t smem = sizeof(GemmSmem<BN, 6>) + 1024;
+  auto k = gemm_fp8_kernel<TO, E>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail((int)e, "gemm_e4m3: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
+    attr_set = true;
+  }
+  p.n_blocks = (p.N + BN - 1) / BN;
+  const int tiles = p.m_blocks * p.n_blocks;
+  const int ctas = std::min(tiles, num_sms());
+  p.band = std::min(p.m_blocks, (ctas + p.n_blocks - 1) / p.n_blocks);  // raster band as in launch_gemm
+  APE_LAUNCH(k, ctas, kThreads, smem, st, ma, mb, p, a_scale, w_scale);
+  return check_launch("gemm_fp8_kernel");
+}
+
+// The e4m3 epilogues: 16-bit output + bias (ViT qkv), SwiGLU with and without the row statistics (ViT w12).
+template <typename TO>
+int launch_fp8_epi(int act, bool stats, const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, const float *a_scale,
+                   const float *w_scale, cudaStream_t st) {
+  if (act == ACT_NONE && !stats) return launch_fp8<TO, Epi<false, ACT_NONE, RES_NONE>>(ma, mb, p, a_scale, w_scale, st);
+  if (act == ACT_SWIGLU && !stats) return launch_fp8<TO, Epi<false, ACT_SWIGLU, RES_NONE>>(ma, mb, p, a_scale, w_scale, st);
+  if (act == ACT_SWIGLU) return launch_fp8<TO, Epi<false, ACT_SWIGLU, RES_NONE, false, false, true>>(ma, mb, p, a_scale, w_scale, st);
+  return fail(APE_ERR_UNSUPPORTED, "gemm_e4m3: no kernel for activation %d (none or swiglu only)", act);
+}
 
 }  // namespace
 }  // namespace ape
@@ -917,4 +1057,42 @@ extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64
     return fail(APE_ERR_INVALID_ARG, "gemm+rope: cos / sin tables must be 16-byte aligned");
   RopeArgs r{cos_table, sin_table, pos_map, rope_cols, npos};
   return gemm_impl(A, lda, W, ldw, C, ldc, bias, nullptr, 0, out_dtype, M, N, K, in_dtype, out_dtype, ACT_NONE, tile_n, &r, stream);
+}
+
+extern "C" int ape_gemm_tn_e4m3(const void *A, int64_t lda, const void *W, int64_t ldw, const float *a_scale,
+                                const float *w_scale, void *C, int64_t ldc, const float *bias, int M, int N, int K, int out_dtype,
+                                int act, float *stats_out, int stats_nslab, void *stream) {
+  if (out_dtype != APE_DTYPE_F16 && out_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_UNSUPPORTED, "gemm_e4m3: output must be fp16 or bf16 (got dtype %d)", out_dtype);
+  if (act != ACT_NONE && act != ACT_SWIGLU)
+    return fail(APE_ERR_UNSUPPORTED, "gemm_e4m3: no kernel for activation %d (none or swiglu only)", act);
+  if (M < 0 || N <= 0 || K <= 0) return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: bad sizes M=%d N=%d K=%d", M, N, K);
+  if (K % 16) return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: K must be a multiple of 16 (got %d)", K);
+  if (M == 0) return APE_OK;
+  if (!A || !W || !C) return fail(APE_ERR_NULL_PTR, "gemm_e4m3: null pointer argument");
+  if (!a_scale || !w_scale) return fail(APE_ERR_NULL_PTR, "gemm_e4m3: null scale pointer (a_scale [M] and w_scale [N] are required)");
+  if (lda % 16 || ldw % 16 || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15))
+    return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: A/W base and row pitch must be 16-byte aligned (TMA)");
+  if (lda < K || ldw < K) return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: row pitch smaller than K");
+  if ((reinterpret_cast<uintptr_t>(a_scale) | reinterpret_cast<uintptr_t>(w_scale)) & 3)
+    return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: scales must be 4-byte aligned fp32");
+  if (act == ACT_SWIGLU && (N & 1)) return fail(APE_ERR_INVALID_ARG, "gemm_e4m3: swiglu needs even N");
+  const int n_out = act == ACT_SWIGLU ? N / 2 : N;
+  if (stats_out && (act != ACT_SWIGLU || stats_nslab != (n_out + 63) / 64))
+    return fail(APE_ERR_INVALID_ARG, "gemm_e4m3+stats: needs the SwiGLU epilogue and stats_nslab = ceil(N/2/64)");
+  CUtensorMap ma, mb;
+  if (int rc = make_map(&ma, A, APE_DTYPE_E4M3, M, K, lda, BM, BK8)) return rc;
+  if (int rc = make_map(&mb, W, APE_DTYPE_E4M3, N, K, ldw, 128, BK8)) return rc;
+  GemmParams p{};
+  p.C = C; p.bias = bias; p.ldc = ldc;
+  p.M = M; p.N = N; p.K = K;
+  p.m_blocks = (M + BM - 1) / BM;
+  p.k_blocks = (K + BK8 - 1) / BK8;
+  p.vec_out = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) % 4) == 0;
+  p.fast = p.vec_out && reinterpret_cast<uintptr_t>(bias) % 8 == 0;
+  p.stats_out = stats_out;
+  p.stats_nslab = stats_out ? stats_nslab : 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (out_dtype == APE_DTYPE_BF16) return launch_fp8_epi<__nv_bfloat16>(act, stats_out != nullptr, ma, mb, p, a_scale, w_scale, st);
+  return launch_fp8_epi<__half>(act, stats_out != nullptr, ma, mb, p, a_scale, w_scale, st);
 }

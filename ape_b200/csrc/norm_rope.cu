@@ -4,6 +4,8 @@
 //   * 2-D rotary embedding applied in place to the q and k thirds of a fused [M, 3C] qkv buffer
 //     (VisionRotaryEmbeddingFast, utils_eva02.py:307-346; rotate_half :248-252).
 // All HBM-bound: one warp per row, 128-bit loads, data held in registers between the two passes.
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 
 namespace ape {
@@ -104,6 +106,84 @@ layernorm_kernel(const TI *__restrict__ x, long long ldx, TO *__restrict__ y, lo
       store8<TO>(yr + 8 * j, o);
     }
   }
+}
+
+// layernorm_kernel with an e4m3 output (the A operand of ape_gemm_tn_e4m3): the warp holds the whole row, so the row's
+// absolute maximum of t = LN(x) * w + b comes for free; y = e4m3(t / s) with s = max|t| / 448, and scale[out_row] = s.
+template <typename TI, int MAXV>
+__global__ void __launch_bounds__(256)
+layernorm_e4m3_kernel(const TI *__restrict__ x, long long ldx, uint8_t *__restrict__ y, long long ldy, float *__restrict__ scale,
+                      const float *__restrict__ w, const float *__restrict__ b, const int *__restrict__ row_map,
+                      int rows, int C, float eps) {
+  pdl_prologue();
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= rows) return;
+  const TI *xr = x + (size_t)warp * ldx;
+  const int nvec = (C + 7) >> 3;
+  float v[MAXV][8];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    const int j = lane + 32 * i;
+    if (j < nvec) {
+      load8<TI>(xr + 8 * j, v[i]);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        if (8 * j + k >= C) v[i][k] = 0.f;
+        sum += v[i][k];
+      }
+    }
+  }
+  const float mean = warp_sum(sum) / (float)C;
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    const int j = lane + 32 * i;
+    if (j < nvec) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float d = (8 * j + k < C) ? v[i][k] - mean : 0.f;
+        sq += d * d;
+      }
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(sq) / (float)C + eps);
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {  // t in place of x, the same arithmetic as layernorm_kernel
+    const int j = lane + 32 * i;
+    if (j < nvec) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        v[i][k] = (8 * j + k < C) ? (v[i][k] - mean) * rstd * __ldg(w + 8 * j + k) + __ldg(b + 8 * j + k) : 0.f;
+        amax = fmaxf(amax, fabsf(v[i][k]));
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float s = amax / 448.f;  // 448: the largest finite e4m3 value
+  const int orow = row_map ? row_map[warp] : warp;
+  uint8_t *yr = y + (size_t)orow * ldy;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    const int j = lane + 32 * i;
+    if (j < nvec) {
+      uint32_t q[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2 lo = make_float2(0.f, 0.f), hi = make_float2(0.f, 0.f);
+        if (s > 0.f) {
+          lo = make_float2(v[i][4 * h] / s, v[i][4 * h + 1] / s);
+          hi = make_float2(v[i][4 * h + 2] / s, v[i][4 * h + 3] / s);
+        }
+        q[h] = (uint32_t)__nv_cvt_float2_to_fp8x2(lo, __NV_SATFINITE, __NV_E4M3) |
+               ((uint32_t)__nv_cvt_float2_to_fp8x2(hi, __NV_SATFINITE, __NV_E4M3) << 16);
+      }
+      *reinterpret_cast<uint2 *>(yr + 8 * j) = make_uint2(q[0], q[1]);
+    }
+  }
+  if (lane == 0) scale[orow] = s;
 }
 
 // Extended row kernel for the deformable encoder (C <= 256 * MAXV):
@@ -364,6 +444,35 @@ extern "C" int ape_layernorm(const void *x, int64_t ldx, void *y, int64_t ldy, c
   }
 #undef APE_LN
   return fail(APE_ERR_UNSUPPORTED, "layernorm: dtype pair (%d -> %d) not supported", in_dtype, out_dtype);
+}
+
+extern "C" int ape_layernorm_e4m3(const void *x, int64_t ldx, void *y, int64_t ldy, float *scale, const float *weight,
+                                  const float *bias, const int *row_map, int rows, int C, float eps, int in_dtype, void *stream) {
+  if (rows < 0 || C <= 0 || C > 1024) return fail(APE_ERR_INVALID_ARG, "layernorm_e4m3: rows=%d C=%d (C <= 1024)", rows, C);
+  if (ldx < ((C + 7) & ~7) || ldy < ((C + 7) & ~7))
+    return fail(APE_ERR_INVALID_ARG, "layernorm_e4m3: row pitch must cover C rounded up to 8 elements");
+  if (in_dtype != APE_DTYPE_F32 && in_dtype != APE_DTYPE_F16 && in_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_UNSUPPORTED, "layernorm_e4m3: input dtype %d not supported", in_dtype);
+  if (rows == 0) return APE_OK;
+  if (!x || !y || !scale || !weight || !bias) return fail(APE_ERR_NULL_PTR, "layernorm_e4m3: null pointer argument");
+  if ((ldx * dtype_size(in_dtype)) % 16 || ldy % 16 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15))
+    return fail(APE_ERR_INVALID_ARG, "layernorm_e4m3: rows must be 16-byte aligned");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int blocks = (rows + 7) / 8;
+#define APE_LN8(TI)                                                                                                        \
+  do {                                                                                                                     \
+    if (C <= 256)                                                                                                          \
+      APE_LAUNCH((layernorm_e4m3_kernel<TI, 1>), blocks, 256, 0, st, (const TI *)x, ldx, (uint8_t *)y, ldy, scale, weight, bias, \
+                 row_map, rows, C, eps);                                                                                   \
+    else                                                                                                                   \
+      APE_LAUNCH((layernorm_e4m3_kernel<TI, 4>), blocks, 256, 0, st, (const TI *)x, ldx, (uint8_t *)y, ldy, scale, weight, bias, \
+                 row_map, rows, C, eps);                                                                                   \
+  } while (0)
+  if (in_dtype == APE_DTYPE_F32) APE_LN8(float);
+  else if (in_dtype == APE_DTYPE_F16) APE_LN8(__half);
+  else APE_LN8(__nv_bfloat16);
+#undef APE_LN8
+  return check_launch("layernorm_e4m3_kernel");
 }
 
 extern "C" int ape_layernorm_ex(const void *x, int64_t ldx, void *y, int64_t ldy, const float *weight, const float *bias,

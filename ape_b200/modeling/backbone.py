@@ -187,6 +187,9 @@ class Block(nn.Module):
 
 
 class ViT(nn.Module):
+    """EVA-02 ViT of APE.  `fp8_linears=True` (off by default, not a reference keyword) runs the qkv and w12 GEMMs of every
+    block in FP8 on the window-major engine path (APE-L_D, APE-L_B / L_C); the APE-Ti raster path and the fp32 path ignore
+    it and run as without it."""
     # reference file whose meaning of `subln` this class follows: vit_eva_clip.py (inner_attn_ln) here, vit_eva02.py (none)
     # in ape_b200.modeling.vit_eva02.ViT
     _reference_file = "vit_eva_clip"
@@ -197,7 +200,7 @@ class ViT(nn.Module):
                  rope=False, postnorm=False, pt_hw_seq_len=16, intp_freq=False, naiveswiglu=False, subln=False,
                  window_size=0, window_block_indexes=(), residual_block_indexes=(), use_act_checkpoint=False,
                  pretrain_img_size=224, pretrain_use_cls_token=True, out_feature="last_feat", xattn=False,
-                 frozen_stages=-1, swiglu=False):
+                 frozen_stages=-1, swiglu=False, fp8_linears=False):
         super().__init__()
         naive_subln = naiveswiglu and subln and not swiglu
         variant_l = naive_subln and self._reference_file == "vit_eva_clip"  # APE-L_D: sub-LN with inner_attn_ln, naive SwiGLU
@@ -232,6 +235,13 @@ class ViT(nn.Module):
         # inner_attn_ln / ffn_ln folded around proj / w3 (ape_gemm_tn_fused): two LayerNorm launches and two trips of the
         # activations through HBM fewer per block
         self.fold_sub_layernorms = True
+        # Opt-in FP8 (e4m3) for the two GEMMs that follow a LayerNorm in every block, qkv (after norm1) and w12 (after
+        # norm2): the LayerNorm writes e4m3 values with a scale per row (ape_layernorm_e4m3) and the GEMM runs on the FP8
+        # tensor cores (ape_gemm_tn_e4m3) against weights quantised once per output row.  RoPE, attention, proj, w3, the
+        # folds and the fp32 residual stream are unchanged.  Only the window-major engine path (APE-L_D, APE-L_B / L_C)
+        # honours it; the APE-Ti raster path and the fp32 path ignore it.  Off by default: its accuracy on the released
+        # checkpoints has not been measured.
+        self.fp8_linears = bool(fp8_linears)
         self._out_feature_channels = {out_feature: embed_dim}
         self._out_feature_strides = {out_feature: patch_size}
         self._out_features = [out_feature]
@@ -368,6 +378,19 @@ class ViT(nn.Module):
                      fw=m.ffn_ln.weight.to(**f32).contiguous(), fb=m.ffn_ln.bias.to(**f32).contiguous())
         return d
 
+    def _pack_fp8(self, packed, device):
+        """e4m3 copies of the fused qkv and interleaved w12 weights with one scale per output row (ops.quantize_rows_e4m3),
+        quantised from the fp32 parameters and added to the blocks of the 16-bit pack `packed` on first use, so the 16-bit
+        weights of a graph captured without FP8 stay where they are."""
+        for blk, d in zip(self.blocks, packed["blocks"]):
+            if "wqkv_q" in d:
+                continue
+            a, m = blk.attn, blk.mlp
+            wqkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0).to(device)
+            w12 = torch.stack([m.w1.weight, m.w2.weight], 1).reshape(2 * m.w1.weight.shape[0], -1).to(device)
+            d["wqkv_q"], d["sqkv"] = ops.quantize_rows_e4m3(wqkv)
+            d["w12_q"], d["s12"] = ops.quantize_rows_e4m3(w12)
+
     def _geometry(self, B, g, ws, dtype, device):
         """Per input geometry: window-major token permutation, abs-pos table, RoPE position maps."""
         k = (B, g, ws, dtype, str(device), self.pos_embed._version)
@@ -431,23 +454,33 @@ class ViT(nn.Module):
         hid_p = pk["blocks"][0]["hid_p"]
         hbuf = torch.empty((M, hid_p), dtype=dtype, device=dev)
         hbuf2 = torch.empty((M, hid_p), dtype=dtype, device=dev)
+        fp8 = self.fp8_linears
+        if fp8:
+            self._pack_fp8(pk, dev)
         for blk, p in zip(self.blocks, pk["blocks"]):
-            h = ops.layernorm(x, p["n1w"], p["n1b"], eps=1e-6, out_dtype=dtype)
             # RoPE in the qkv GEMM epilogue (ape_gemm_tn_rope) is available but OFF: measured +26 us per qkv GEMM (the 8
-            # epilogue warps wait on the cos/sin rows) against 8.7 us for the separate ape_rope_qk pass
-            fused_rope = self.fused_rope and hd == 64 and C % 8 == 0
+            # epilogue warps wait on the cos/sin rows) against 8.7 us for the separate ape_rope_qk pass; the FP8 qkv GEMM
+            # always leaves RoPE to that pass
+            fused_rope = self.fused_rope and hd == 64 and C % 8 == 0 and not fp8
+            if fp8:  # e4m3 LayerNorm output with a scale per row -> FP8 qkv GEMM
+                hq, hs = ops.layernorm(x, p["n1w"], p["n1b"], eps=1e-6, out_dtype=torch.float8_e4m3fn)
+                qkv = ops.linear_fp8(hq, hs, p["wqkv_q"], p["sqkv"], p["bqkv"], out_dtype=dtype)
+            else:
+                h = ops.layernorm(x, p["n1w"], p["n1b"], eps=1e-6, out_dtype=dtype)
             if blk.window_size > 0:
                 if fused_rope:
                     qkv = ops.linear_rope_tc(h, p["wqkv"], p["bqkv"], rope_win[0], rope_win[1], C, hd)
                 else:
-                    qkv = ops.linear_tc(h, p["wqkv"], p["bqkv"])
+                    if not fp8:
+                        qkv = ops.linear_tc(h, p["wqkv"], p["bqkv"])
                     ops.rope_qk_(qkv, rope_win[0], rope_win[1], C, hd)  # position = index inside the window
                 nb, n = B * nw * nw, w * w
             else:
                 if fused_rope:
                     qkv = ops.linear_rope_tc(h, p["wqkv"], p["bqkv"], rope_glb[0], rope_glb[1], C, hd, pos_map=geo["glb_map"])
                 else:
-                    qkv = ops.linear_tc(h, p["wqkv"], p["bqkv"])
+                    if not fp8:
+                        qkv = ops.linear_tc(h, p["wqkv"], p["bqkv"])
                     ops.rope_qk_(qkv, rope_glb[0], rope_glb[1], C, hd, pos_map=geo["glb_map"])
                 nb, n = B, g * g
             fold = self.fold_sub_layernorms
@@ -469,13 +502,18 @@ class ViT(nn.Module):
             else:
                 a = ops.layernorm(o, p["lnw"], p["lnb"], eps=1e-6)
                 x = ops.linear_tc(a, p["wproj"], p["bproj"], residual=x, out_dtype=torch.float32)
-            h = ops.layernorm(x, p["n2w"], p["n2b"], eps=1e-6, out_dtype=dtype)
+            if fp8:
+                hq, hs = ops.layernorm(x, p["n2w"], p["n2b"], eps=1e-6, out_dtype=torch.float8_e4m3fn)
+                w12 = lambda **kw: ops.linear_fp8(hq, hs, p["w12_q"], p["s12"], p["b12"], act="swiglu", **kw)
+            else:
+                h = ops.layernorm(x, p["n2w"], p["n2b"], eps=1e-6, out_dtype=dtype)
+                w12 = lambda **kw: ops.linear_tc(h, p["w12"], p["b12"], act="swiglu", **kw)
             if fold:  # ffn_ln folded into w3: the SwiGLU epilogue leaves the row statistics of the hidden it writes
-                _, st2 = ops.linear_tc(h, p["w12"], p["b12"], act="swiglu", out=hbuf[:, :p["hid"]], stats_out=True)
+                _, st2 = w12(out=hbuf[:, :p["hid"]], stats_out=True)
                 x = ops.linear_tc(hbuf[:, :p["hid"]], p["w3_ln"][:, :p["hid"]], p["b3_ln"], residual=x, out_dtype=torch.float32,
                                   ln_fold=(st2, p["s3"], p["hid"], 1e-6))
             else:
-                ops.linear_tc(h, p["w12"], p["b12"], act="swiglu", out=hbuf[:, :p["hid"]])
+                w12(out=hbuf[:, :p["hid"]])
                 ops.layernorm(hbuf[:, :p["hid"]], p["fw"], p["fb"], eps=1e-6, out=hbuf2[:, :p["hid"]])
                 x = ops.linear_tc(hbuf2[:, :p["hid"]], p["w3"][:, :p["hid"]], p["b3"], residual=x, out_dtype=torch.float32)
         # back to raster order: [B, g, g, C] tokens (NHWC memory), 16-bit operand of the pyramid GEMMs

@@ -700,7 +700,8 @@ class DeformableDETRSegmVL(nn.Module):
         """Run fn(*tensor_args, *const_args) through a CUDA graph captured once per key: inputs are copied into
         static buffers, the replay reuses the captured launch sequence (about 2 000 kernel launches per image
         otherwise dominate the wall clock).  Outputs are static buffers, valid until the next replay of `key`."""
-        key = (key, self.engine_dtype)
+        # the ViT's opt-in FP8 mode is part of the captured launch sequence: one graph per mode
+        key = (key, self.engine_dtype, bool(getattr(getattr(self.backbone, "net", None), "fp8_linears", False)))
         entry = self._graph_cache.get(key)
         if entry is not None:
             self._graph_cache.move_to_end(key)

@@ -5,7 +5,9 @@ APE-L_B, APE-L_C; `vitt_eva02.py`: APE-Ti).
   swiglu=True                    packed `w12` SwiGLU, fused `qkv`, no sub-LayerNorms (APE-Ti)
   naiveswiglu=True, subln=True   separate q/k/v projections with q/v biases, NO inner_attn_ln, SwiGLU w1, w2, ffn_ln, w3
                                  (:179-291; APE-L_B / L_C)
-It is ape_b200.modeling.ViT with that reading; ape_b200.modeling.ViT keeps vit_eva_clip.py's (subln = inner_attn_ln too)."""
+It is ape_b200.modeling.ViT with that reading; ape_b200.modeling.ViT keeps vit_eva_clip.py's (subln = inner_attn_ln too).
+`fp8_linears` (not in the reference, off by default) is ape_b200.modeling.ViT's opt-in FP8 qkv / w12 mode; the APE-Ti path
+ignores it."""
 from functools import partial
 
 import torch.nn as nn
@@ -22,7 +24,7 @@ class ViT(_backbone.ViT):
                  use_abs_pos=True, use_rel_pos=False, rope=True, pt_hw_seq_len=16, intp_freq=True, window_size=0,
                  window_block_indexes=(), residual_block_indexes=(), use_act_checkpoint=False, pretrain_img_size=224,
                  pretrain_use_cls_token=True, out_feature="last_feat", xattn=True, subln=False, swiglu=False,
-                 naiveswiglu=False, frozen_stages=-1):
+                 naiveswiglu=False, frozen_stages=-1, fp8_linears=False):
         # act_layer is accepted and unused, as in the reference (its blocks use SiLU gates only)
         super().__init__(img_size=img_size, patch_size=patch_size, in_chans=in_chans, embed_dim=embed_dim, depth=depth,
                          num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, drop_path_rate=drop_path_rate,
@@ -31,4 +33,5 @@ class ViT(_backbone.ViT):
                          window_size=window_size, window_block_indexes=window_block_indexes,
                          residual_block_indexes=residual_block_indexes, use_act_checkpoint=use_act_checkpoint,
                          pretrain_img_size=pretrain_img_size, pretrain_use_cls_token=pretrain_use_cls_token,
-                         out_feature=out_feature, xattn=xattn, frozen_stages=frozen_stages, swiglu=swiglu)
+                         out_feature=out_feature, xattn=xattn, frozen_stages=frozen_stages, swiglu=swiglu,
+                         fp8_linears=fp8_linears)

@@ -255,6 +255,51 @@ def linear_tc(x, weight, bias=None, act=None, out_dtype=None, residual=None, til
     return (res, stats) if stats_out else res
 
 
+def quantize_rows_e4m3(w):
+    """(q, scale): per-row e4m3 quantisation of a 2-D tensor, computed in fp32 on its device: scale = max|row| / 448 (1 for
+    an all-zero row), q = e4m3(row / scale) rounded to nearest even.  Weight preparation for linear_fp8, done once."""
+    w = w.detach().float()
+    s = w.abs().amax(1) / 448.0
+    s = torch.where(s > 0, s, torch.ones_like(s))
+    return (w / s[:, None]).clamp(-448.0, 448.0).to(torch.float8_e4m3fn).contiguous(), s.contiguous()
+
+
+def linear_fp8(xq, x_scale, wq, w_scale, bias=None, act=None, stats_out=False, out=None, out_dtype=torch.float16):
+    """act((xq @ wq.T) * x_scale[:, None] * w_scale[None, :] + bias) on the FP8 tensor cores (ape_gemm_tn_e4m3).
+
+    xq [M, K] and wq [N, K] torch.float8_e4m3fn with unit inner stride and 16-byte aligned rows, K a multiple of 16;
+    x_scale fp32 [M], w_scale fp32 [N]; bias fp32 [N] or None.  act None or "swiglu" (interleaved weight rows, N/2 output
+    columns; stats_out=True also returns the fp32 [M, ceil(N/2/64), 2] slab statistics, as linear_tc).  The output is fp16 or
+    bf16: `out` [M, n_out] with unit inner stride, or a new tensor of out_dtype."""
+    _require(xq.is_cuda and wq.is_cuda, "linear_fp8: CUDA tensors only")
+    _require(xq.dtype == torch.float8_e4m3fn and wq.dtype == torch.float8_e4m3fn, "linear_fp8: e4m3 operands")
+    _require(xq.dim() == 2 and wq.dim() == 2 and xq.shape[1] == wq.shape[1] and xq.stride(1) == 1 and wq.stride(1) == 1,
+             "linear_fp8: xq [M, K] and wq [N, K] with unit inner stride")
+    M, K = xq.shape
+    N = wq.shape[0]
+    for s, n, name in ((x_scale, M, "x_scale"), (w_scale, N, "w_scale")):
+        _require(s.dtype == torch.float32 and s.is_contiguous() and s.numel() == n and s.is_cuda, f"linear_fp8: {name} fp32 [{n}]")
+    if bias is not None:
+        _require(bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == N, "linear_fp8: bias must be fp32 [N]")
+    _require(act in (None, "swiglu"), "linear_fp8: act None or 'swiglu'")
+    n_out = N // 2 if act == "swiglu" else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=out_dtype, device=xq.device)
+    _require(out.dim() == 2 and out.shape == (M, n_out) and out.stride(1) == 1 and out.is_cuda, "linear_fp8: bad `out`")
+    stats, nslab = None, 0
+    if stats_out:
+        nslab = (n_out + 63) // 64
+        stats = torch.empty((M, nslab, 2), dtype=torch.float32, device=xq.device)
+    with torch.cuda.device(xq.device), _timed(("gemm_tn_e4m3", M, N, K)):
+        rc = _lib.lib.ape_gemm_tn_e4m3(xq.data_ptr(), xq.stride(0), wq.data_ptr(), wq.stride(0), x_scale.data_ptr(),
+                                       w_scale.data_ptr(), out.data_ptr(), out.stride(0),
+                                       bias.data_ptr() if bias is not None else None, M, N, K, _lib.dtype_code(out.dtype),
+                                       ACT[act], stats.data_ptr() if stats is not None else None, int(nslab),
+                                       _lib.current_stream_ptr())
+    _lib.check(rc, "ape_gemm_tn_e4m3")
+    return (out, stats) if stats_out else out
+
+
 def ffn_fused(x, w1, b1, w2, b2, out=None, variant=0):
     """x + relu(x @ w1.T + b1) @ w2.T + b2 in one launch (ape_ffn_fused), fp32 [..., 256]; the hidden activation stays on chip.
 
@@ -374,15 +419,34 @@ def layernorm_module(module, x, out_dtype=None):
     return layernorm(x, w, b, eps=module.eps, out_dtype=out_dtype)
 
 
-def layernorm(x, weight, bias, eps=1e-5, out_dtype=None, row_map=None, out=None):
+def layernorm(x, weight, bias, eps=1e-5, out_dtype=None, row_map=None, out=None, scale_out=None):
     """LayerNorm over the last dim (ape_layernorm).  x [..., C] with unit inner stride and uniform row
-    pitch; weight / bias fp32.  row_map: int32 [rows] output row of each input row (or None)."""
+    pitch; weight / bias fp32.  row_map: int32 [rows] output row of each input row (or None).
+
+    out_dtype=torch.float8_e4m3fn (or an e4m3 `out`): returns (q [rows, C] e4m3, scale [rows] fp32) with q * scale[:, None]
+    the LayerNorm output, s = max|row| / 448 per row (ape_layernorm_e4m3; C <= 1024); `scale_out` is an optional fp32
+    buffer for the scales, indexed like the output rows."""
     C = x.shape[-1]
     x2 = x.reshape(-1, C) if x.dim() != 2 else x
     _require(x2.is_cuda and x2.stride(1) == 1, "layernorm: CUDA tensor with unit inner stride")
     _require(weight.dtype == torch.float32 and bias.dtype == torch.float32, "layernorm: fp32 weight / bias")
     rows = x2.shape[0]
-    out_dtype = out_dtype or x.dtype
+    out_dtype = out.dtype if out is not None else (out_dtype or x.dtype)
+    if out_dtype == torch.float8_e4m3fn:
+        if out is None:
+            out = torch.empty((rows, (C + 15) // 16 * 16), dtype=out_dtype, device=x.device)[:, :C]
+        _require(out.dim() == 2 and out.stride(1) == 1 and out.is_cuda, "layernorm: bad e4m3 `out`")
+        if scale_out is None:
+            scale_out = torch.empty((out.shape[0],), dtype=torch.float32, device=x.device)
+        _require(scale_out.dtype == torch.float32 and scale_out.is_contiguous() and scale_out.numel() == out.shape[0],
+                 "layernorm: scale_out must be fp32 [output rows]")
+        with torch.cuda.device(x.device), _timed(("layernorm_e4m3", rows, C)):
+            rc = _lib.lib.ape_layernorm_e4m3(x2.data_ptr(), x2.stride(0), out.data_ptr(), out.stride(0), scale_out.data_ptr(),
+                                             weight.data_ptr(), bias.data_ptr(),
+                                             row_map.data_ptr() if row_map is not None else None, rows, C, float(eps),
+                                             _lib.dtype_code(x2.dtype), _lib.current_stream_ptr())
+        _lib.check(rc, "ape_layernorm_e4m3")
+        return out, scale_out
     if out is None:
         out = torch.empty((rows, C), dtype=out_dtype, device=x.device)
     with torch.cuda.device(x.device), _timed(("layernorm", rows, C)):

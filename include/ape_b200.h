@@ -35,6 +35,7 @@ extern "C" {
 #define APE_DTYPE_F32 0
 #define APE_DTYPE_F16 1
 #define APE_DTYPE_BF16 2
+#define APE_DTYPE_E4M3 3 /* FP8 e4m3 (torch.float8_e4m3fn): ape_gemm_tn_e4m3 operands, ape_layernorm_e4m3 output */
 
 /* status codes (<0); positive return values are cudaError_t */
 #define APE_OK 0
@@ -173,6 +174,19 @@ int ape_gemm_tn_fused(const void *A, int64_t lda, const void *W, int64_t ldw, vo
                       float ln_eps, float *stats_out, int stats_nslab, void *stream);
 
 /*
+ * FP8 linear layer: C[M, N] = act((A W^T) * a_scale[m] * w_scale[n] + bias), e4m3 x e4m3 on the wgmma tensor cores.
+ * A [M, K] and W [N, K] are e4m3 bytes (torch.float8_e4m3fn), K contiguous, row pitches lda / ldw in elements (= bytes),
+ * 16-byte aligned; K a multiple of 16.  a_scale fp32 [M] and w_scale fp32 [N] are required (dequantised value = q * scale).
+ * The products of e4m3 values are exact; they are summed in fp32, promoted from the tensor cores' accumulator into an fp32
+ * register accumulator every 128 of K.  The scales are applied first, in fp32, then the epilogue of ape_gemm_tn_fused:
+ * bias fp32 [N] or NULL, and act 0 (none) or 3 (SwiGLU over interleaved column pairs, C [M, N/2]; stats_out as in
+ * ape_gemm_tn_fused, or NULL).  out_dtype fp16 or bf16 (pitch ldc elements).  Other epilogues: APE_ERR_UNSUPPORTED.
+ */
+int ape_gemm_tn_e4m3(const void *A, int64_t lda, const void *W, int64_t ldw, const float *a_scale, const float *w_scale, void *C,
+                     int64_t ldc, const float *bias, int M, int N, int K, int out_dtype, int act, float *stats_out,
+                     int stats_nslab, void *stream);
+
+/*
  * 3x3 convolution (stride 1, zero padding 1) over NHWC activations as an implicit GEMM on the wgmma kernel: the 3x3
  * convolutions of SimpleFeaturePyramid (vit_eva_clip.py:804-847) and of the mask head (deformable_detr_segm_vl.py:741-747).
  * x [B,H,W,Cin], w [Cout,3,3,Cin] (= the Conv2d weight permuted (0,2,3,1)), y [B,H,W,Cout], bias fp32 [Cout] or NULL;
@@ -221,6 +235,15 @@ void ape_gemm_set_trace(long long *device_buffer);
  */
 int ape_layernorm(const void *x, int64_t ldx, void *y, int64_t ldy, const float *weight, const float *bias,
                   const int *row_map, int rows, int C, float eps, int in_dtype, int out_dtype, void *stream);
+
+/*
+ * ape_layernorm with an e4m3 output and a scale per row, the A operand of ape_gemm_tn_e4m3: with t the fp32 LayerNorm output
+ * of row r (after weight and bias, as ape_layernorm computes it), s = max|t| / 448 (0 for an all-zero row) and
+ * y[out_row] = e4m3(t / s), rounded to nearest even and saturating (0 where s = 0), scale[out_row] = s.  C <= 1024; y pitch
+ * ldy bytes, a multiple of 16 covering C rounded up to 8; padding bytes are written as 0.  row_map as in ape_layernorm.
+ */
+int ape_layernorm_e4m3(const void *x, int64_t ldx, void *y, int64_t ldy, float *scale, const float *weight, const float *bias,
+                       const int *row_map, int rows, int C, float eps, int in_dtype, void *stream);
 
 /*
  * Extended LayerNorm for the deformable encoder (C % 8 == 0, C <= 1024); one pass over the activations for
