@@ -7,6 +7,7 @@ APE_L_D   configs/LVISCOCOCOCOSTUFF_O365_OID_VGR_SA1B_REFCOCO_GQA_PhraseCut_Flic
           configs/common/backbone/vitl_eva02_clip.py:9-48
 MINI      same architecture, toy sizes: used for golden fixtures small enough to commit.
 APE_L_B   APE-L_B and APE-L_C (vit_eva02.py ViT-L, no neck); MINI_EVA02L is its toy-size twin.
+APE_L_A   APE-L_B without vision-language fusion; MINI_L_A is its toy-size twin.
 """
 import copy
 
@@ -94,6 +95,19 @@ MINI_EVA02L = copy.deepcopy(MINI)
 MINI_EVA02L["name"] = "MINI-EVA02L"
 MINI_EVA02L["backbone"].update(variant="eva02_subln", out_channels=256)
 MINI_EVA02L.update(neck=None, proposal_ambiguous=0)
+
+
+# APE-L_A: configs/LVISCOCOCOCOSTUFF_O365_OID_VG/ape_deta/ape_deta_vitl_eva02_lsj1024_cp_720k.py:11-53 (1256 classes, top-300,
+# no neck) on the same LVIS / COCO chain as APE-L_B, without the _vlf_ step: DeformableDETRSegm over DeformableDetrTransformer
+# (deformable_detr_segm.py, deformable_transformer.py), i.e. APE-L_B without the fusion fields.  The model builds no fusion
+# layer and no name-prompt fusion feature (ape_deta_r50.py leaves name_prompt_fusion_type at "none").
+_FUSION_FIELDS = ("vlf_embed", "vlf_heads", "vlf_init")
+APE_L_A = {k: copy.deepcopy(v) for k, v in APE_L_B.items() if k not in _FUSION_FIELDS}
+APE_L_A["name"] = "APE-L_A"
+
+# APE-L_A's structure at MINI sizes: golden fixtures.
+MINI_L_A = {k: copy.deepcopy(v) for k, v in MINI_EVA02L.items() if k not in _FUSION_FIELDS}
+MINI_L_A["name"] = "MINI-L_A"
 
 
 def level_shapes(spec):

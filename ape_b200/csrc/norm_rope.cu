@@ -192,7 +192,9 @@ layernorm_e4m3_kernel(const TI *__restrict__ x, long long ldx, uint8_t *__restri
 //   y  = t + col_add[c]            if col_add   (gamma_v * delta_v: one vector per image for "name" prompts)
 //   y2 = y + row_add[row]          if y2        (query + query_pos, the operand of the sampling-offset / attention-weight GEMM)
 // so the activations make one trip through HBM where the module sequence makes four.
-template <typename TI, typename TO, int MAXV>
+// NORM = false (no w): t = x, and y is written only when non-null: the first layer of an encoder without fusion layers, whose
+// input needs nothing but `query + query_pos` (deformable_transformer.py:78-102).
+template <typename TI, typename TO, int MAXV, bool NORM = true>
 __global__ void __launch_bounds__(256)
 layernorm_ex_kernel(const TI *__restrict__ x, long long ldx, TO *__restrict__ y, long long ldy, const float *__restrict__ w,
                     const float *__restrict__ b, float eps, const float *__restrict__ w2, const float *__restrict__ b2,
@@ -214,6 +216,7 @@ layernorm_ex_kernel(const TI *__restrict__ x, long long ldx, TO *__restrict__ y,
       for (int k = 0; k < 8; ++k) sum += v[i][k];
     }
   }
+  if constexpr (NORM) {
   float mean = warp_sum(sum) / (float)C;
   float sq = 0.f;
 #pragma unroll
@@ -266,6 +269,7 @@ layernorm_ex_kernel(const TI *__restrict__ x, long long ldx, TO *__restrict__ y,
       }
     }
   }
+  }  // NORM
   const float *ca = col_add ? col_add + (size_t)(warp / rows_per_image) * col_add_stride : nullptr;
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
@@ -277,7 +281,7 @@ layernorm_ex_kernel(const TI *__restrict__ x, long long ldx, TO *__restrict__ y,
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[i][k] += cc[k];
       }
-      store8<TO>(y + (size_t)warp * ldy + 8 * j, v[i]);
+      if (NORM || y) store8<TO>(y + (size_t)warp * ldy + 8 * j, v[i]);
       if (y2) {
         float a[8], o[8];
         load8<TO>(row_add + (size_t)warp * ld_add + 8 * j, a);
@@ -483,7 +487,10 @@ extern "C" int ape_layernorm_ex(const void *x, int64_t ldx, void *y, int64_t ldy
   if (ldx < C || ldy < C || (y2 && (ldy2 < C || ld_add < C)))
     return fail(APE_ERR_INVALID_ARG, "layernorm_ex: row pitch smaller than C");
   if (rows == 0) return APE_OK;
-  if (!x || !y || !weight || !bias || (weight2 && !bias2) || (y2 && !row_add) || (col_add && rows_per_image <= 0))
+  const bool norm = weight != nullptr;  // no weight: no normalisation (then weight2 must be null too, and y may be)
+  if (!norm && (bias || weight2 || !(y || y2)))
+    return fail(APE_ERR_INVALID_ARG, "layernorm_ex: without weight, bias and weight2 must be null and y or y2 given");
+  if (!x || (norm && (!y || !bias)) || (weight2 && !bias2) || (y2 && !row_add) || (col_add && rows_per_image <= 0))
     return fail(APE_ERR_NULL_PTR, "layernorm_ex: null pointer argument");
   const int ie = dtype_size(in_dtype), oe = dtype_size(out_dtype);
   const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(y2) |
@@ -495,7 +502,15 @@ extern "C" int ape_layernorm_ex(const void *x, int64_t ldx, void *y, int64_t ldy
   const int blocks = (rows + 7) / 8;
 #define APE_LNX(TI, TO)                                                                                                   \
   do {                                                                                                                    \
-    if (C <= 256)                                                                                                         \
+    if (!norm && C <= 256)                                                                                                \
+      APE_LAUNCH((ape::layernorm_ex_kernel<TI, TO, 1, false>), blocks, 256, 0, st, (const TI *)x, ldx, (TO *)y, ldy, weight, bias, eps, \
+          weight2, bias2, eps2, col_add, col_add_stride, rows_per_image > 0 ? rows_per_image : 1, (const TO *)row_add, ld_add, (TO *)y2, \
+          ldy2, rows, C);                                                                                                 \
+    else if (!norm)                                                                                                       \
+      APE_LAUNCH((ape::layernorm_ex_kernel<TI, TO, 4, false>), blocks, 256, 0, st, (const TI *)x, ldx, (TO *)y, ldy, weight, bias, eps, \
+          weight2, bias2, eps2, col_add, col_add_stride, rows_per_image > 0 ? rows_per_image : 1, (const TO *)row_add, ld_add, (TO *)y2, \
+          ldy2, rows, C);                                                                                                 \
+    else if (C <= 256)                                                                                                    \
       APE_LAUNCH((ape::layernorm_ex_kernel<TI, TO, 1>), blocks, 256, 0, st, (const TI *)x, ldx, (TO *)y, ldy, weight, bias, eps, weight2, bias2, eps2, \
           col_add, col_add_stride, rows_per_image > 0 ? rows_per_image : 1, (const TO *)row_add, ld_add, (TO *)y2, ldy2, rows, C);  \
     else                                                                                                                  \

@@ -1,4 +1,4 @@
-"""Meta-architecture of the engine: `DeformableDETRSegmVL` (+ `SomeThing` wrapper).
+"""Meta-architecture of the engine: `DeformableDETRSegmVL`, its fusion-free subclass `DeformableDETRSegm` (+ `SomeThing`).
 
 Mirror of ape/modeling/ape_deta/deformable_detr_segm_vl.py:33-164 (constructor), :166-726
 (forward, inference branch), :728-750 (mask features), :759-810 (inference), :846-872
@@ -497,7 +497,7 @@ class DeformableDETRSegmVL(nn.Module):
         low = self.engine_dtype != torch.float32
         geo = self._geometry(images.shape, image_sizes, img_masks)
         mask_prompt_flatten = self._mask_prompt(batched_inputs, images.shape, geo) if "mask_prompt" in batched_inputs[0] else None
-        graphs = low and self.use_cuda_graphs and fusion is not None and fusion.shape[1] == 1 and mask_prompt_flatten is None
+        graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion) and mask_prompt_flatten is None
         need_masks = self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)
         with torch.autocast("cuda", dtype=self.engine_dtype, enabled=low):
             if graphs and not self.profile_stages:
@@ -644,6 +644,12 @@ class DeformableDETRSegmVL(nn.Module):
         return memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features
 
     @staticmethod
+    def _graph_prompt(prompt, fusion):
+        """Prompts whose step is captured in a CUDA graph: one fusion token ("name" prompts), so the encoder's launch sequence
+        does not depend on the text."""
+        return fusion is not None and fusion.shape[1] == 1
+
+    @staticmethod
     def _mix_text(prompt, features_l, fusion_out):
         if prompt == "name":
             if fusion_out is not None:
@@ -710,7 +716,7 @@ class DeformableDETRSegmVL(nn.Module):
             # each with a private memory pool; evict the least recently used together with its geometry
             while len(self._graph_cache) >= self.graph_cache_size:
                 self._graph_cache.popitem(last=False)
-            static_in = [t.clone() for t in tensor_args]
+            static_in = [None if t is None else t.clone() for t in tensor_args]  # None: no fusion input (DeformableDETRSegm)
             # autocast's weight-cast cache must be off while capturing: cached casts would be freed when the
             # autocast region ends while the graph still reads them
             with torch.autocast("cuda", dtype=self.engine_dtype, cache_enabled=False):
@@ -727,7 +733,8 @@ class DeformableDETRSegmVL(nn.Module):
             self._graph_cache[key] = entry
         graph, static_in, static_out = entry[:3]
         for dst, src in zip(static_in, tensor_args):
-            dst.copy_(src)
+            if dst is not None:
+                dst.copy_(src)
         graph.replay()
         return static_out
 
@@ -971,6 +978,29 @@ class DeformableDETRSegmVL(nn.Module):
                                                               self.test_nms_thresh, self.test_topk_per_image)
             results.append(Instances((h, w), pred_boxes=Boxes(bx), scores=sc, pred_classes=cl, query_index=qi))
         return results
+
+
+class DeformableDETRSegm(DeformableDETRSegmVL):
+    """ape/modeling/ape_deta/deformable_detr_segm.py (APE-L_A): the model of DeformableDETRSegmVL without vision-language
+    fusion, over DeformableDetrTransformer.  Same constructor keywords and forward contract.  Text features of every prompt
+    type go straight to the classifier (no fusion input to the encoder, no `features_l` mix), and region prompts
+    (`mask_prompt`) are not read, as in the reference.  The step is captured in a CUDA graph for "name" prompts: the text
+    enters only the classifier, so the graph key on the shape of the text features covers it."""
+
+    def _text_features(self, batched_inputs):
+        prompt, features_l, _ = super()._text_features(batched_inputs)
+        return prompt, features_l, None
+
+    def _mask_prompt(self, batched_inputs, batch_shape, geo):
+        return None
+
+    @staticmethod
+    def _graph_prompt(prompt, fusion):
+        return prompt == "name"
+
+    @staticmethod
+    def _mix_text(prompt, features_l, fusion_out):
+        return features_l
 
 
 class SomeThing(nn.Module):

@@ -6,7 +6,8 @@ Mirror of ape/modeling/ape_deta/deformable_transformer_vl.py (`DeformableDetrTra
 of the detrex containers it is built from (BaseTransformerLayer / TransformerLayerSequence / FFN /
 MultiheadAttention, SURVEY.md Appendix B): same constructor arguments, same forward signatures,
 same parameter names (`layers.{i}.attentions.{j}`, `layers.{i}.ffns.0.layers.{0.0,1}`,
-`layers.{i}.norms.{k}`, `vl_layers.{i}.b_attn…`, `level_embeds`, `enc_output`, `pos_trans`, …)."""
+`layers.{i}.norms.{k}`, `vl_layers.{i}.b_attn…`, `level_embeds`, `enc_output`, `pos_trans`, …).
+The classes of deformable_transformer.py (no fusion layers, APE-L_A) are subclasses at the end of the file."""
 import copy
 import math
 
@@ -461,6 +462,15 @@ class DeformableDetrTransformerVL(nn.Module):
                     output_proposals=out, proposal_invalid=mask_flatten.unsqueeze(-1) | ~valid,
                     level_ids=torch.cat(level_ids), has_padding=bool(mask_flatten.any()))
 
+    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l):
+        """The encoder call of stage_encode -> (memory, language features after the fusion layers)."""
+        return self.encoder(
+            query=feat_flatten, key=None, value=None, query_l=query_l, attention_mask_l=attention_mask_l,
+            query_pos=pos_flatten, query_key_padding_mask=geo["mask_flatten"] if geo["has_padding"] else None,
+            spatial_shapes=geo["spatial_shapes"], reference_points=geo["reference_points"],
+            level_start_index=geo["level_start_index"], valid_ratios=geo["valid_ratios"],
+            host_shapes=geo["shapes"])
+
     def stage_encode(self, multi_level_feats, geo, query_l, attention_mask_l=None, mask_prompt_flatten=None,
                      feat_flatten=None):
         """feat_flatten: optional [B,S,C] tensor that already holds the flattened levels (the engine neck writes its
@@ -476,12 +486,7 @@ class DeformableDetrTransformerVL(nn.Module):
                                        for i, (h, w) in enumerate(geo["shapes"])], 1)
                 cache[engine_dtype] = (ck, (geo["pos_flatten"] + lvl_embed.float()).to(engine_dtype).contiguous())
         pos_flatten = cache[engine_dtype][1]
-        memory, query_l = self.encoder(
-            query=feat_flatten, key=None, value=None, query_l=query_l, attention_mask_l=attention_mask_l,
-            query_pos=pos_flatten, query_key_padding_mask=geo["mask_flatten"] if geo["has_padding"] else None,
-            spatial_shapes=geo["spatial_shapes"], reference_points=geo["reference_points"],
-            level_start_index=geo["level_start_index"], valid_ratios=geo["valid_ratios"],
-            host_shapes=geo["shapes"])
+        memory, query_l = self._encode(feat_flatten, pos_flatten, geo, query_l, attention_mask_l)
         # gen_encoder_output_proposals (:354-369): zero the memory of invalid anchors, project, normalise
         output_proposals = geo["output_proposals"]
         invalid = geo["proposal_invalid"]
@@ -596,3 +601,92 @@ class DeformableDetrTransformerVL(nn.Module):
         self.last_topk_proposals = topk_proposals  # kept for parity tests (bit-exact index requirement)
         return (inter_states, init_reference_out, inter_references, enc_cls, enc_coord,
                 geo["output_proposals"].sigmoid(), memory, query_l)
+
+
+# -- deformable_transformer.py: the same transformer without vision-language fusion (APE-L_A) ------------------------------
+class DeformableDetrTransformerEncoder(DeformableDetrTransformerEncoderVL):
+    """deformable_transformer.py:19-106: the VL encoder without `vl_layers`; forward returns the memory only."""
+
+    def __init__(self, embed_dim=256, num_heads=8, feedforward_dim=1024, attn_dropout=0.1, ffn_dropout=0.1, num_layers=6,
+                 post_norm=False, num_feature_levels=4, use_act_checkpoint=False, pytorch_attn=False):
+        super().__init__(embed_dim=embed_dim, num_heads=num_heads, feedforward_dim=feedforward_dim, attn_dropout=attn_dropout,
+                         ffn_dropout=ffn_dropout, num_layers=num_layers, post_norm=post_norm,
+                         num_feature_levels=num_feature_levels, vl_layer=None, use_act_checkpoint=use_act_checkpoint,
+                         pytorch_attn=pytorch_attn)
+        del self.vl_layers  # no fusion layers, and no such entry in the state_dict
+
+    def forward(self, query, key, value, query_pos=None, key_pos=None, attn_masks=None, query_key_padding_mask=None,
+                key_padding_mask=None, **kwargs):
+        engine_dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else None
+        if engine_dtype is not None:
+            query, query_pos = query.to(engine_dtype), query_pos.to(engine_dtype)
+            if query.is_cuda and query.shape[-1] % 8 == 0:
+                return self._engine_schedule(query.contiguous(), query_pos.contiguous(), query_key_padding_mask, kwargs)
+        if self.record_taps:
+            self.taps = {}
+        for i, layer in enumerate(self.layers):
+            query = layer(query, query_pos, query_key_padding_mask, kwargs["reference_points"], kwargs["spatial_shapes"],
+                          kwargs["level_start_index"], kwargs.get("host_shapes"))
+            if self.record_taps:
+                self.taps[f"enc{i}"] = query
+        if self.post_norm_layer is not None:
+            query = self.post_norm_layer(query)
+        return query
+
+    def _engine_schedule(self, x, query_pos, key_padding_mask, kwargs):
+        """Engine schedule of the encoder without fusion.  Per layer:
+          deformable self-attention + FFN (wgmma GEMMs, fused gather), the fp32 sum x + ffn(x) left un-normalised
+          -> ONE row kernel: last norm of this layer -> (query, query + pos) for the next layer.
+        The first layer's `query + pos` comes from the same row kernel without the norm; the last layer's norm is a plain
+        LayerNorm.  Same functions as the layer loop; no library kernel between the layers."""
+        dt = x.dtype
+        if self.record_taps:
+            self.taps = {}
+        _, qpos = ops.layernorm_ex(x, None, None, 0.0, row_add=query_pos)
+        last = len(self.layers) - 1
+        for i, layer in enumerate(self.layers):
+            s = layer(x, query_pos, key_padding_mask, kwargs["reference_points"], kwargs["spatial_shapes"],
+                      kwargs["level_start_index"], kwargs.get("host_shapes"), query_with_pos=qpos, defer_last_norm=True)
+            nw, nb = ops.packed(layer.norms[1], dt)
+            if i < last:
+                x, qpos = ops.layernorm_ex(s, nw, nb, layer.norms[1].eps, row_add=query_pos, out_dtype=dt)
+            else:
+                x = ops.layernorm(s, nw, nb, eps=layer.norms[1].eps, out_dtype=dt)
+            if self.record_taps:
+                self.taps[f"enc{i}"] = x
+        if self.post_norm_layer is not None:
+            x = self.post_norm_layer(x)
+        return x
+
+
+class DeformableDetrTransformerDecoder(DeformableDetrTransformerDecoderVL):
+    """deformable_transformer.py:109-235: the VL decoder with `look_forward_twice` off (the reference has no such switch)."""
+
+    def __init__(self, embed_dim=256, num_heads=8, feedforward_dim=1024, attn_dropout=0.1, ffn_dropout=0.1, num_layers=6,
+                 return_intermediate=True, num_feature_levels=4, use_act_checkpoint=False, pytorch_attn=False):
+        super().__init__(embed_dim=embed_dim, num_heads=num_heads, feedforward_dim=feedforward_dim, attn_dropout=attn_dropout,
+                         ffn_dropout=ffn_dropout, num_layers=num_layers, return_intermediate=return_intermediate,
+                         num_feature_levels=num_feature_levels, use_act_checkpoint=use_act_checkpoint,
+                         look_forward_twice=False, pytorch_attn=pytorch_attn)
+
+
+class DeformableDetrTransformer(DeformableDetrTransformerVL):
+    """deformable_transformer.py:238-644: the VL transformer without language features or region prompts.  The encoder
+    returns the memory only, `gen_encoder_output_proposals` takes no prompt mask, forward returns a 7-tuple."""
+
+    def gen_encoder_output_proposals(self, memory, memory_padding_mask, spatial_shapes):
+        return super().gen_encoder_output_proposals(memory, memory_padding_mask, spatial_shapes)
+
+    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l):
+        if query_l is not None or attention_mask_l is not None:
+            raise ValueError("ape_b200.DeformableDetrTransformer has no fusion layers: language features go to the classifier")
+        memory = self.encoder(
+            query=feat_flatten, key=None, value=None, query_pos=pos_flatten,
+            query_key_padding_mask=geo["mask_flatten"] if geo["has_padding"] else None,
+            spatial_shapes=geo["spatial_shapes"], reference_points=geo["reference_points"],
+            level_start_index=geo["level_start_index"], valid_ratios=geo["valid_ratios"], host_shapes=geo["shapes"])
+        return memory, None
+
+    def forward(self, multi_level_feats, multi_level_masks, multi_level_pos_embeds, query_embed, **kwargs):
+        return super().forward(multi_level_feats, multi_level_masks, multi_level_pos_embeds, query_embed, None, None, None,
+                               **kwargs)[:7]

@@ -462,14 +462,21 @@ def layernorm_ex(x, weight, bias, eps, weight2=None, bias2=None, eps2=0.0, col_a
     """One pass over x [B, rows, C] (or [rows, C]) for LN -> optional second LN -> + col_add[image] -> (y, y + row_add)
     (ape_layernorm_ex; the previous encoder layer's last norm, the fusion layer's layer_norm_v, gamma_v * delta_v and
     `query + query_pos` in one kernel).  weights fp32 [C]; col_add fp32 [B, C]; row_add like x in the output dtype.
-    Returns (y, y2) with y2 None when row_add is None."""
+    Returns (y, y2) with y2 None when row_add is None.
+
+    weight None: no normalisation.  With neither weight2 nor col_add, y is x itself (not copied) and the kernel only writes
+    y2 = x + row_add: `query + query_pos` of an encoder's first layer when no fusion layer precedes it."""
     C = x.shape[-1]
     _require(x.is_cuda and x.is_contiguous(), "layernorm_ex: contiguous CUDA tensor")
     x2 = x.view(-1, C)
     rows = x2.shape[0]
     rpi = x.shape[-2] if x.dim() == 3 else rows
     out_dtype = out_dtype or x.dtype
-    y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
+    if weight is None:
+        _require(bias is None and weight2 is None, "layernorm_ex: bias / weight2 without weight")
+    add_only = weight is None and col_add is None and out_dtype == x.dtype
+    _require(not add_only or row_add is not None, "layernorm_ex: nothing to compute")
+    y = x if add_only else torch.empty(x.shape, dtype=out_dtype, device=x.device)
     y2 = None
     if row_add is not None:
         _require(row_add.dtype == out_dtype and row_add.is_contiguous() and row_add.numel() == x.numel(),
@@ -483,7 +490,8 @@ def layernorm_ex(x, weight, bias, eps, weight2=None, bias2=None, eps2=0.0, col_a
         _require(t is None or (t.dtype == torch.float32 and t.is_contiguous()), "layernorm_ex: fp32 weights")
     with torch.cuda.device(x.device), _timed(("layernorm_ex", rows, C, weight2 is not None, row_add is not None)):
         rc = _lib.lib.ape_layernorm_ex(
-            x2.data_ptr(), C, y.data_ptr(), C, weight.data_ptr(), bias.data_ptr(), float(eps),
+            x2.data_ptr(), C, None if add_only else y.data_ptr(), C, weight.data_ptr() if weight is not None else None,
+            bias.data_ptr() if bias is not None else None, float(eps),
             weight2.data_ptr() if weight2 is not None else None, bias2.data_ptr() if bias2 is not None else None, float(eps2),
             col_add.data_ptr() if col_add is not None else None, C, int(rpi),
             row_add.data_ptr() if row_add is not None else None, C, y2.data_ptr() if y2 is not None else None, C,

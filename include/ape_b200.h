@@ -252,6 +252,8 @@ int ape_layernorm_e4m3(const void *x, int64_t ldx, void *y, int64_t ldy, float *
  *   y = t + col_add[image, :]        if col_add  gamma_v * delta_v of that fusion (one fp32 [C] vector per image for
  *                                                "name" prompts; col_add_stride elements between images, rows_per_image rows each)
  *   y2 = y + row_add[row, :]         if y2       query + query_pos (multi_scale_deform_attn.py:262-263); row_add / y2 in out_dtype
+ * weight NULL: no normalisation (t = x; bias and weight2 must be NULL) and y may be NULL, so that only y2 = x + row_add is
+ * written: the first layer of an encoder without fusion layers (deformable_transformer.py:78-102).
  */
 int ape_layernorm_ex(const void *x, int64_t ldx, void *y, int64_t ldy, const float *weight, const float *bias, float eps,
                      const float *weight2, const float *bias2, float eps2, const float *col_add, int64_t col_add_stride,
