@@ -145,6 +145,8 @@ def _declare(lib):
     lib.ape_gemm_tn_argmax.argtypes = [_vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp]
     lib.ape_semseg_keys_decode.restype = _i
     lib.ape_semseg_keys_decode.argtypes = [_vp, _i64, _vp, _vp, _vp]
+    lib.ape_panoptic_winners.restype = _i
+    lib.ape_panoptic_winners.argtypes = [_vp] * 5 + [_i] * 9 + [ctypes.c_float, _i, _vp]
 
 
 
@@ -203,6 +205,7 @@ EXPORTS = (
     "ape_semseg_keys_init",
     "ape_gemm_tn_argmax",
     "ape_semseg_keys_decode",
+    "ape_panoptic_winners",
 )
 
 

@@ -838,8 +838,10 @@ class DeformableDETRSegmVL(nn.Module):
     def _panoptic(self, box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep=None):
         """Panoptic branch (:671-696): queries that survive the detection NMS, merged by
         `postprocess.postprocess_panoptic` (the reference's `_postprocess_panoptic`, :919-998, without its per-segment
-        host round trips).  Needs the thing / stuff split of the evaluated dataset in `self.dataset_stuff`."""
-        from .postprocess import postprocess_panoptic
+        host round trips).  Needs the thing / stuff split of the evaluated dataset in `self.dataset_stuff`.  On CUDA with a
+        16-bit engine_dtype, `postprocess.postprocess_panoptic_winners` makes the same merge from one kernel over the logits
+        (csrc/panoptic.cu) and the [K, H, W] mask stacks are never formed."""
+        from .postprocess import postprocess_panoptic, postprocess_panoptic_winners
 
         name = self.dataset_names[self.eval_dataset_id] if self.dataset_names else None
         if name not in self.dataset_stuff:
@@ -853,12 +855,18 @@ class DeformableDETRSegmVL(nn.Module):
             keep = [r.query_index for r in self.inference(box_cls, box_pred, image_sizes)]
         else:
             keep = [torch.arange(box_cls.shape[1], device=box_cls.device)] * box_cls.shape[0]
+        engine = self.engine_dtype in (torch.float16, torch.bfloat16) and mask_pred.is_cuda
+        stuff_first = bool(stuff) and stuff[0] == "things"
         outs = []
         for b, (qi, size, inp) in enumerate(zip(keep, image_sizes, batched_inputs)):
-            m = F.interpolate(mask_pred[b, qi][None].float(), size=padded_hw, mode="bilinear", align_corners=False)[0]
             h, w = inp.get("height", size[0]), inp.get("width", size[1])
-            outs.append(postprocess_panoptic(box_cls[b, qi].float(), m, size, h, w, thing_ids, len(things),
-                                             bool(stuff) and stuff[0] == "things", self.panoptic_configs))
+            if engine:
+                outs.append(postprocess_panoptic_winners(box_cls[b, qi].float(), mask_pred[b].contiguous(), qi, padded_hw, size, h,
+                                                         w, thing_ids, len(things), stuff_first, self.panoptic_configs))
+                continue
+            m = F.interpolate(mask_pred[b, qi][None].float(), size=padded_hw, mode="bilinear", align_corners=False)[0]
+            outs.append(postprocess_panoptic(box_cls[b, qi].float(), m, size, h, w, thing_ids, len(things), stuff_first,
+                                             self.panoptic_configs))
         return outs
 
     def _inference_static(self, box_cls, box_pred, image_sizes, first_pack=None):

@@ -875,6 +875,42 @@ def semseg_label(mask_logits, query_index, cls, padded_hw, img_hw, out_hw, class
     return label, score
 
 
+def panoptic_winners(mask_logits, query_index, scores, padded_hw, img_hw, out_hw, prob):
+    """Per-pixel winners and segment areas of the panoptic merge of one image without the [K, H, W] mask stacks:
+    (ids int32 [out_h, out_w], counts int32 [3, K]).  With
+
+        p = sem_seg_postprocess(F.interpolate(mask_logits[query_index][None].float(), padded_hw, "bilinear")[0], img_hw,
+                                *out_hw).sigmoid()                                   [K, out_h, out_w]
+        win = (scores[:, None, None] * p).argmax(0)                                  first maximum, as torch.argmax
+
+    ids = win where p[win] >= prob, else -1; counts = (bincount(win), bincount(win[p[win] >= prob]), (p >= prob).sum((1, 2))),
+    each of length K (deformable_detr_segm_vl.py:919-998, the three areas of every kept query).  A query whose score is -inf
+    takes no part: it never wins and its counts are 0, so a keep mask can be applied without compacting the queries.
+
+    mask_logits [Q, h, w] CUDA fp32 / fp16 / bf16; query_index int64 [K]; scores fp32 [K].  One call to ape_panoptic_winners
+    (two kernels, capturable in a CUDA graph); K <= APE_PANOPTIC_MAX_K (4096)."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 3 and mask_logits.is_contiguous(),
+             "panoptic_winners: contiguous CUDA logits [Q,h,w]")
+    dev = mask_logits.device
+    K = int(query_index.numel())
+    _require(query_index.dim() == 1 and scores.dim() == 1 and int(scores.numel()) == K,
+             "panoptic_winners: query_index [K] and scores [K] disagree")
+    Hp, Wp = int(padded_hw[0]), int(padded_hw[1])
+    ih, iw = int(img_hw[0]), int(img_hw[1])
+    oh, ow = int(out_hw[0]), int(out_hw[1])
+    _require(0 < ih <= Hp and 0 < iw <= Wp and oh > 0 and ow > 0, "panoptic_winners: bad image / output size")
+    index = query_index.to(device=dev, dtype=torch.int64).contiguous()
+    sc = scores.to(device=dev, dtype=torch.float32).contiguous()
+    ids = torch.empty((oh, ow), dtype=torch.int32, device=dev)
+    counts = torch.empty((3, K), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev), _timed(("panoptic_winners", K, oh * ow)):
+        rc = _lib.lib.ape_panoptic_winners(mask_logits.data_ptr(), index.data_ptr(), sc.data_ptr(), ids.data_ptr(), counts.data_ptr(),
+                                           K, mask_logits.shape[1], mask_logits.shape[2], Hp, Wp, ih, iw, oh, ow, float(prob),
+                                           _lib.dtype_code(mask_logits.dtype), _lib.current_stream_ptr())
+        _lib.check(rc, "ape_panoptic_winners")
+    return ids, counts
+
+
 _RESAMPLE_TABLES = {}
 
 

@@ -448,6 +448,23 @@ int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, u
                        int in_dtype, void *stream);
 int ape_semseg_keys_decode(const uint64_t *keys, int64_t n, int64_t *label, float *score, void *stream);
 
+/*
+ * Panoptic merge without the [K,H,W] mask stacks.  Replaces, for one image, the per-pixel part of
+ * deformable_detr_segm_vl.py:919-998 (`_postprocess_panoptic`, after the upsample of :569 and detectron2 sem_seg_postprocess):
+ *   v_k = resize2(crop(resize1(logits[index[k]]))), p_k = sigmoid(v_k), id = the first k maximising scores[k] * p_k
+ * with resize1 h x w -> Hp x Wp, crop img_h x img_w, resize2 -> out_h x out_w, both upsample_bilinear2d (align_corners=False)
+ * arithmetic in fp32, the sigmoid after both.  logits [Q,h,w] (logit_dtype fp32 / fp16 / bf16), index [K] int64 in [0, Q),
+ * scores [K] fp32; a query whose score is -INFINITY takes no part (it never wins and its counts stay 0).
+ *   ids    [out_h, out_w] int32: id where p_id >= prob, else -1 (also where no query takes part).
+ *   counts [3, K] int32: mask_area[k] = #{pixels whose id is k}, inter_area[k] = #{... and p_k >= prob},
+ *          original_area[k] = #{pixels with p_k >= prob}.  Zeroed by the call itself.
+ * 0 <= K <= APE_PANOPTIC_MAX_K (per-CTA shared-memory histograms of 3*K int32).  Two kernels, no allocation, no
+ * synchronisation: capturable in a CUDA graph.
+ */
+#define APE_PANOPTIC_MAX_K 4096
+int ape_panoptic_winners(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h, int w,
+                         int Hp, int Wp, int img_h, int img_w, int out_h, int out_w, float prob, int logit_dtype, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
