@@ -9,12 +9,14 @@
 //   VisionLanguageAlign contraction            ape/layers/vision_language_align.py:36-48
 // `W` is consumed in nn.Linear's own [out_features, in_features] layout: both operands are K-major.
 //
-// Kernel shape (persistent, warp-specialised, 288 threads, 1 CTA / SM):
-//   warps 0-7  consumers : warpgroup g owns rows 64g..64g+63 of the 128 x BN tile: 4 x wgmma m64nBNk16 per k-block,
-//                          one k-block in flight (the stage of the previous one is released when it has completed),
-//                          then bias / activation / residual / rotary / LayerNorm fold in registers and direct stores
-//   warp 8     producer  : STAGES-deep ring of {A 128x64, B BNx64} 16-bit tiles, mbarrier full/empty; it runs ahead
-//                          into the next tile's k-blocks while the consumers finish the epilogue of the current one
+// Kernel shape (persistent, warp-specialised, 384 threads, 1 CTA / SM):
+//   warps 0-7   consumers : warpgroup g owns rows 64g..64g+63 of the 128 x BN tile: 4 x wgmma m64nBNk16 per k-block,
+//                           one k-block in flight (the stage of the previous one is released when it has completed),
+//                           then bias / activation / residual / rotary / LayerNorm fold in registers and direct stores
+//   warps 8-11  producer  : one thread keeps a STAGES-deep ring of {A 128x64, B BNx64} 16-bit tiles filled by TMA
+//                           (mbarrier full/empty); it runs ahead into the next tile's k-blocks while the consumers finish
+//                           the epilogue of the current one.  The warpgroup gives its registers to the consumers
+//                           (setmaxnreg 40 / 232), so BN = 256 holds its 128 accumulators per thread without spilling.
 // gemm_pp_kernel is the ping-pong form of the same kernel for single-CTA BN = 128 GEMMs with many tiles: each consumer
 // warpgroup owns whole tiles, and their main loops alternate so that one's epilogue runs under the other's MMAs.
 #include <stdlib.h>
@@ -29,7 +31,9 @@ namespace {
 
 constexpr int BM = 128, BK = 64, WG_K = 16;
 constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 32 * kConsumerWarps + 32;
+// gemm_tc_kernel and gemm_pp_kernel: two consumer warpgroups and a producer warpgroup (setmaxnreg works per warpgroup)
+constexpr int kThreads = 32 * kConsumerWarps + 128;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;  // 40 x 128 + 232 x 256 <= the 168 x 384 registers of the launch
 
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SWIGLU = 3, ACT_CLAMP = 4 };
 enum Res { RES_NONE = 0, RES_F32 = 1, RES_16 = 2 };  // RES_16: a residual of the operand type
@@ -326,9 +330,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   pdl_wait();  // set-up done: operands / residual of the previous kernel may be read, C may be written from here on
   if (threadIdx.x == 0) trace_stamp(p, 1);
 
-  if (warp == kConsumerWarps) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp >= kConsumerWarps) {
+    // ===================== TMA producer (one thread of the producer warpgroup) =====================
+    tc::setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
       uint32_t stage = 0, phase = 0;
       int m_blk, n_blk;
       for (int t = 0; tile_at(t, m_blk, n_blk); ++t) {
@@ -357,6 +362,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     __syncwarp();
   } else {
     // ===================== consumers (two warpgroups) =====================
+    tc::setmaxnreg_inc<kConsumerRegs>();  // BN = 256: 128 accumulators
     const int wg = warp / 4;
     float acc[BN / 2];
 #pragma unroll
@@ -398,9 +404,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if (t == 0) trace_stamp(p, 4);
         trace_stamp(p, 5);
       }
-      if constexpr (kArgmax<E>) argmax_epilogue<BN>(p, acc, m_blk, n_blk, wg, lane);
-      else if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (n_blk + 1) * BN <= p.N) epilogue<E, TI, BN, true>(p, acc, m_blk, n_blk, wg, lane);
-      else epilogue<E, TI, BN, false>(p, acc, m_blk, n_blk, wg, lane);
+      if constexpr (kArgmax<E>) {
+        argmax_epilogue<BN>(p, acc, m_blk, n_blk, wg, lane);
+      } else {
+        // BN = 256 as two 128-column halves, one after the other (as gemm_pp_kernel does with its row halves): a single
+        // epilogue over all 128 accumulators hoists the bias and residual loads of every column ahead of the stores and
+        // spills.  Accumulators 64 h .. 64 h + 63 are columns 128 h .. 128 h + 127 of the tile.
+#pragma unroll
+        for (int h = 0; h < BN / 128; ++h) {
+          const int nb = n_blk * (BN / 128) + h;
+          if (!E::rope && p.fast && (m_blk + 1) * BM <= p.M && (nb + 1) * 128 <= p.N) epilogue<E, TI, 128, true>(p, acc + 64 * h, m_blk, nb, wg, lane);
+          else epilogue<E, TI, 128, false>(p, acc + 64 * h, m_blk, nb, wg, lane);
+        }
+      }
     }
     if (threadIdx.x == 0) trace_stamp(p, 6);
   }
@@ -429,11 +445,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 //  4. The epilogue takes warp4 from threadIdx.x (consumers keep warps 0-7) and the row half from its `wg` argument.
 //     trace_stamp slots keep their meaning; thread 0 belongs to warpgroup 0.
 //  5. PDL as in gemm_tc_kernel: launch_dependents at entry, griddepcontrol.wait before the first TMA load and store.
-constexpr int kPpThreads = 32 * kConsumerWarps + 128;
 constexpr int kOrderBar = 1;  // named barriers 1 and 2
 
 template <typename TI, class E>
-__global__ void __launch_bounds__(kPpThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
   constexpr int BN = 128, STAGES = 6;
   extern __shared__ uint8_t smem_raw[];
@@ -473,7 +488,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
   if (warp >= kConsumerWarps) {
     // ===================== TMA producer: every tile of the CTA in order, one ring =====================
-    tc::setmaxnreg_dec<40>();  // 40 x 128 + 232 x 256 <= the 168 x 384 registers of the launch
+    tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == kConsumerWarps && lane == 0) {
       uint32_t stage = 0, phase = 0;
       int m_blk, n_blk;
@@ -490,7 +505,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     __syncwarp();
   } else {
     // ===================== consumers: warpgroup wg, tiles wg, wg + 2, ... =====================
-    tc::setmaxnreg_inc<232>();  // 128 accumulators
+    tc::setmaxnreg_inc<kConsumerRegs>();  // 128 accumulators
     const int wg = warp / 4;
     float acc[BN];  // acc[0, 64): tile rows 0-63, acc[64, 128): rows 64-127
 #pragma unroll
@@ -553,17 +568,18 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 }
 
 // FP8 form (ape_gemm_tn_e4m3): e4m3 A [M, K] and W [N, K] with an fp32 scale per row of each, C = (A W^T) * a_scale[m] *
-// w_scale[n], then the epilogue E of the 16-bit kernels (TO: the 16-bit output type).  The shape of gemm_tc_kernel with
-// CL = 1, BN = 128: a 128-byte swizzle row holds 128 e4m3 values, so one k-block is 128 of K, the stage sizes are those of
-// the 16-bit kernel, and a warpgroup issues 4 x m64n128k32 per k-block.
+// w_scale[n], then the epilogue E of the 16-bit kernels (TO: the 16-bit output type).  The tiles of gemm_tc_kernel with
+// CL = 1, BN = 128, and a single producer warp (288 threads): a 128-byte swizzle row holds 128 e4m3 values, so one k-block
+// is 128 of K, the stage sizes are those of the 16-bit kernel, and a warpgroup issues 4 x m64n128k32 per k-block.
 // Hopper's FP8 MMA does not keep full fp32 precision when it accumulates over a long K, so each k-block's 4 MMAs go into a
 // scratch fragment (the first with scale_d = 0) that is added to the fp32 accumulator in registers once they have
 // completed: one promotion per 128 of K, as CUTLASS's FP8 kernels without "fast accumulation" do.  The second fragment is
 // why this is the cooperative form (64 + 64 accumulators per thread); a ping-pong warpgroup already holds 128.
 constexpr int BK8 = 128;
+constexpr int kFp8Threads = 32 * kConsumerWarps + 32;  // producer: warp 8
 
 template <typename TO, class E>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kFp8Threads, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p,
                 const float *__restrict__ a_scale, const float *__restrict__ w_scale) {
   constexpr int BN = 128, STAGES = 6;
@@ -730,7 +746,7 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cud
   p.band = std::min(m_groups, (clusters + p.n_blocks - 1) / p.n_blocks);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(clusters * CL));
-  cfg.blockDim = dim3(PP ? kPpThreads : kThreads);
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
@@ -808,6 +824,14 @@ int launch_any(int bn, bool cluster, bool pp, int in_dtype, const EpiKey &k, con
 // GEMMs) the cooperative kernel, which splits one tile over both warpgroups, finishes a CTA's single tile sooner.
 bool use_pingpong(int tiles) { return tiles >= 2 * num_sms(); }
 
+// 128 x 256 tiles on single CTAs for long-K wide GEMMs (the ViT-L w3, 4096 x 1024 x 2730): each CTA's 43-k-block main
+// loop is long against its exposed epilogue, and the 128 tiles fill the SMs in one round; it took 46 us where the 128 x 128
+// cluster of two took 110 (tests/perf_gemm_256.py, DESIGN.md §5).  Elsewhere 128 stays: at K = 512 to 1024 the 128 x 128
+// ping-pong kernel, which hides each epilogue under the other warpgroup's MMAs, beat the cooperative 128 x 256 tile on
+// qkv, w12 and the pyramid deconvolutions, and the cooperative 128 x 128 tile beat it on proj.  A cluster of two was
+// slower than a single CTA at both widths on every shape measured, although it halves the weight traffic from L2.
+bool use_wide(int N, int K) { return N >= 1024 && K >= 2048; }
+
 template <typename TO, class E>
 int launch_fp8(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, const float *a_scale, const float *w_scale,
                cudaStream_t st) {
@@ -824,7 +848,7 @@ int launch_fp8(const CUtensorMap &ma, const CUtensorMap &mb, GemmParams &p, cons
   const int tiles = p.m_blocks * p.n_blocks;
   const int ctas = std::min(tiles, num_sms());
   p.band = std::min(p.m_blocks, (ctas + p.n_blocks - 1) / p.n_blocks);  // raster band as in launch_gemm
-  APE_LAUNCH(k, ctas, kThreads, smem, st, ma, mb, p, a_scale, w_scale);
+  APE_LAUNCH(k, ctas, kFp8Threads, smem, st, ma, mb, p, a_scale, w_scale);
   return check_launch("gemm_fp8_kernel");
 }
 
@@ -880,22 +904,23 @@ static int gemm_impl(const void *A, int64_t lda, const void *W, int64_t ldw, voi
     return fail(APE_ERR_INVALID_ARG, "gemm: A/W base and row pitch must be 16-byte aligned (TMA)");
   if (lda < K || ldw < K) return fail(APE_ERR_INVALID_ARG, "gemm: row pitch smaller than K");
   if (act == ACT_SWIGLU && ((N & 1) || residual)) return fail(APE_ERR_INVALID_ARG, "gemm: swiglu needs even N, no residual");
-  // default tile width 128: a 128 x 256 tile holds 128 fp32 accumulators per consumer thread, more than the 168 registers a
-  // thread of this 288-thread block may use leave room for next to the epilogue (it spills); 256 stays selectable
-  const int bn = (tile_n & 0xfff) > 0 ? (tile_n & 0xfff) : 128;
+  const bool force_pp = (tile_n & 0x8000) != 0, force_coop = (tile_n & 0x10000) != 0;
+  const int m_blocks = (M + BM - 1) / BM;
+  // Tile width: 128, or 128 x 256 on a single CTA where use_wide says so.  An explicit width in tile_n (128 or 256)
+  // overrides the rule, and bits 0x8000 / 0x10000 (below) pin the 128-wide kernels unless a width is given.
+  const bool wide = (tile_n & 0xfff) == 0 && !force_pp && !force_coop && use_wide(N, K);
+  const int bn = (tile_n & 0xfff) > 0 ? (tile_n & 0xfff) : wide ? 256 : 128;
   if (bn != 128 && bn != 256) return fail(APE_ERR_INVALID_ARG, "gemm: tile_n must be 128 or 256");
   if (tile_n & 0x2000) return fail(APE_ERR_UNSUPPORTED, "gemm: tile_n flag 0x2000 (CTA-pair MMA) is not available on sm_90a");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // kernel variant: single CTA, or a cluster of 2 along M sharing the weight tile by TMA multicast.  The cluster pays off
-  // when the K loop is long (K >= 2048: w3, FFN2, the 3x3 convolutions), where the weight tile is the larger share of the
-  // operand traffic; bit 0x1000 forces the single CTA, bit 0x4000 the cluster.
+  // kernel variant: single CTA, or a cluster of 2 along M sharing the weight tile by TMA multicast.  The 128-wide
+  // GEMMs with a long K loop (K >= 2048: FFN2 and the 3x3 convolutions) take the cluster, where the weight tile is the
+  // larger share of the operand traffic; bit 0x1000 forces the single CTA, bit 0x4000 the cluster.
   // A single-CTA BN = 128 GEMM runs the ping-pong kernel when there are enough tiles (use_pingpong); bit 0x8000 forces
   // it (single CTA), bit 0x10000 forces the cooperative kernel.
-  const bool force_pp = (tile_n & 0x8000) != 0, force_coop = (tile_n & 0x10000) != 0;
   if (force_pp && (force_coop || bn != 128 || (tile_n & 0x4000)))
     return fail(APE_ERR_INVALID_ARG, "gemm: tile_n flag 0x8000 (ping-pong) needs tile width 128, no cluster and no 0x10000");
-  const int m_blocks = (M + BM - 1) / BM;
-  const bool cluster = m_blocks >= 2 && !force_pp && (tile_n & 0x1000) == 0 && ((tile_n & 0x4000) != 0 || K >= 2048);
+  const bool cluster = m_blocks >= 2 && !force_pp && (tile_n & 0x1000) == 0 && ((tile_n & 0x4000) != 0 || (!wide && K >= 2048));
   const bool pp = !cluster && bn == 128 && !force_coop && (force_pp || use_pingpong(m_blocks * ((N + bn - 1) / bn)));
   CUtensorMap ma, mb;
   if (int rc = make_map(&ma, A, in_dtype, M, K, lda, BM)) return rc;
