@@ -151,20 +151,29 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
     tc::fence_regs<32>(sc);
     if (lane == 0) tc::mbar_arrive(&s.k_empty[b]);  // K_j may be replaced by K_{j+2}
 
-    // masking: padded keys (>= n_valid) and, causal, keys after the query's own position score -inf: ex2(-inf) = 0
+    // masking: padded keys (>= n_valid) and, causal, keys after the query's own position score -inf: ex2(-inf) = 0.
+    // Only blocks that hold such a key for some row of the warpgroup run the compares (the last partial block of n_valid,
+    // and the causal diagonal); in every other block they would leave all scores as they are.
+    const bool mask = (j + 1) * KN > p.n_valid || (p.causal && (j + 1) * KN - 1 > qblk * QM + g * 64);
+    if (mask) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int kvalid = (p.causal ? min(p.n_valid, qpos[h] + 1) : p.n_valid) - j * KN;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * jj + 2 * tq + e >= kvalid) sc[4 * jj + 2 * h + e] = -INFINITY;
+      }
+    }
     float alpha[2], m_use[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int kvalid = (p.causal ? min(p.n_valid, qpos[h] + 1) : p.n_valid) - j * KN;
       float mx = -INFINITY;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float &x = sc[4 * jj + 2 * h + e];
-          if (8 * jj + 2 * tq + e >= kvalid) x = -INFINITY;
-          mx = fmaxf(mx, x);
-        }
+        for (int e = 0; e < 2; ++e) mx = fmaxf(mx, sc[4 * jj + 2 * h + e]);
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_run[h], mx * p.scale_log2);
