@@ -93,12 +93,19 @@ def _declare(lib):
     lib.ape_rope_qk.restype = _i
     lib.ape_rope_qk.argtypes = [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]
 
+    lib.ape_text_embed_packed.restype = _i
+    lib.ape_text_embed_packed.argtypes = [_vp] * 5 + [_i] * 4 + [_vp]
+    lib.ape_rows_gather.restype = _i
+    lib.ape_rows_gather.argtypes = [_vp, _i64, _vp, _vp, _i64, _i, _i, _vp]
+
     lib.ape_attn_fwd.restype = _i
     lib.ape_attn_fwd.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, ctypes.c_float, _i, _vp]
     lib.ape_attn_fwd_ex.restype = _i
     lib.ape_attn_fwd_ex.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _i, _i64, _vp]
     lib.ape_attn_fwd_mapped.restype = _i
     lib.ape_attn_fwd_mapped.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _i, _i64, _vp, _vp]
+    lib.ape_attn_fwd_seg.restype = _i
+    lib.ape_attn_fwd_seg.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, ctypes.c_float, _i, _vp, _i, _i, _i64, _vp, _vp]
     lib.ape_attn_variant.restype = _i
     lib.ape_attn_variant.argtypes = [_i]
     lib.ape_attn_cross_fwd.restype = _i
@@ -177,9 +184,12 @@ EXPORTS = (
     "ape_layernorm_e4m3",
     "ape_layernorm_ex",
     "ape_rope_qk",
+    "ape_text_embed_packed",
+    "ape_rows_gather",
     "ape_attn_fwd",
     "ape_attn_fwd_ex",
     "ape_attn_fwd_mapped",
+    "ape_attn_fwd_seg",
     "ape_attn_variant",
     "ape_attn_cross_fwd",
     "ape_groupnorm_workspace_bytes",

@@ -44,6 +44,7 @@ struct Params {
   float *stats_out;             // [rows, heads, 2] (sum, sum of squares) of each row's stored output values, or nullptr
   float scale_log2;             // softmax scale * log2(e)
   const int *out_row_map;       // ROW_MAP kernels: query row r is stored at out / stats_out row out_row_map[r]; -1 = not stored
+  const int *seg_start;         // SEG kernels: query row r of the launch also ignores the keys before position seg_start[r]
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -63,7 +64,9 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
   }
 }
 
-template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false>
+// SEG: several short sequences share one tile (the text tower's length-packed prompts).  Query row r attends key k of its
+// tile iff seg_start[r] <= k and k passes the causal / n_valid mask: the causal mask with a lower bound per row.
+template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false, bool SEG = false>
 __global__ void __launch_bounds__(CWG * 128 + 32, NC == 1 ? 2 : 1)
 attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
             const __grid_constant__ CUtensorMap map_v, const Params p) {
@@ -126,6 +129,11 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
   int qpos[2];  // position of the thread's two query rows inside the sequence
 #pragma unroll
   for (int h = 0; h < 2; ++h) qpos[h] = qblk * QM + g * 64 + w4 * 16 + (lane >> 2) + 8 * h;
+  int seg_lo[2] = {0, 0};  // SEG: first key position of the thread's two rows
+  if constexpr (SEG) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) seg_lo[h] = p.seg_start[(size_t)seq * p.q_seq_rows + qpos[h]];
+  }
   float o[NC][32];
 #pragma unroll
   for (int c = 0; c < NC; ++c)
@@ -164,6 +172,21 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
 #pragma unroll
           for (int e = 0; e < 2; ++e)
             if (8 * jj + 2 * tq + e >= kvalid) sc[4 * jj + 2 * h + e] = -INFINITY;
+      }
+    }
+    if constexpr (SEG) {
+      // the lower bound, likewise only where it masks something: a warp runs the compares of a block when one of its 16
+      // rows starts after the block's first key
+      if (__any_sync(0xffffffffu, max(seg_lo[0], seg_lo[1]) > j * KN)) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int klo = seg_lo[h] - j * KN;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (8 * jj + 2 * tq + e < klo) sc[4 * jj + 2 * h + e] = -INFINITY;
+        }
       }
     }
     float alpha[2], m_use[2];
@@ -302,10 +325,10 @@ inline int make_map(CUtensorMap *map, const void *base, int dtype, long long row
 }
 
 // grid = (query rows per sequence / (64 * CWG), heads, sequences)
-template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false>
+template <typename T, int NC, int CWG, bool P_IN_SMEM, bool ROW_MAP = false, bool SEG = false>
 int launch(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const Params &p, dim3 grid, cudaStream_t st) {
   const size_t smem = sizeof(Smem<NC, CWG, P_IN_SMEM>) + 1024;
-  auto k = attn_kernel<T, NC, CWG, P_IN_SMEM, ROW_MAP>;
+  auto k = attn_kernel<T, NC, CWG, P_IN_SMEM, ROW_MAP, SEG>;
   static bool set = false;
   if (!set) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

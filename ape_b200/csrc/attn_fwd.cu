@@ -3,7 +3,9 @@
 // and of the EVA02-CLIP text tower (causal, 77-token prompts packed at a row stride): flash-attention forward with wgmma
 // (attn.cuh), Q/K/V tiles staged by TMA straight out of the fused [M, 3C] qkv buffer the qkv GEMM wrote (no head split
 // copies).  One CTA = 128 queries (two consumer warpgroups) of one (sequence, head).  ape_attn_fwd_mapped stores query rows
-// through a row map (APE-Ti's padded 14x14 windows write straight back to raster token order).
+// through a row map (APE-Ti's padded 14x14 windows write straight back to raster token order).  ape_attn_fwd_seg runs
+// 128-row tiles that hold several short prompts each (the text tower's length-packed mode): causal inside a prompt, nothing
+// across prompts.
 #include <stdlib.h>
 
 #include "attn.cuh"
@@ -38,10 +40,11 @@ extern "C" int ape_attn_fwd(const void *qkv, int64_t ld, void *out, int64_t ldo,
   return ape_attn_fwd_ex(qkv, ld, out, ldo, num_seq, n, n, heads, head_dim, scale, dtype, nullptr, 0, 0, 0, stream);
 }
 
-// ape_attn_fwd_ex / ape_attn_fwd_mapped; out_row_map == nullptr stores query row r at row r
+// ape_attn_fwd_ex / ape_attn_fwd_mapped / ape_attn_fwd_seg; out_row_map == nullptr stores query row r at row r, seg_start ==
+// nullptr is the plain (causal) mask
 static int attn_fwd_impl(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
                          int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
-                         const int *out_row_map, void *stream) {
+                         const int *out_row_map, const int *seg_start, void *stream) {
   if (n_valid <= 0 || n_valid > n) return fail(APE_ERR_INVALID_ARG, "attn: n_valid=%d must be in [1, n=%d]", n_valid, n);
   if (seq_stride <= 0) seq_stride = n;
   if (seq_stride < n_valid) return fail(APE_ERR_INVALID_ARG, "attn: seq_stride=%d smaller than n_valid=%d", seq_stride, n_valid);
@@ -67,9 +70,17 @@ static int attn_fwd_impl(const void *qkv, int64_t ld, void *out, int64_t ldo, in
   p.q_store_rows = seq_stride >= n ? n : n_valid;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out_row_map = out_row_map;
+  p.seg_start = seg_start;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   dim3 grid((unsigned)(n / QM), (unsigned)heads, (unsigned)num_seq);
   const bool p_smem = ape_attn_variant(-1) == 0;
+  if (seg_start) {
+    if (dtype == APE_DTYPE_F16)
+      return p_smem ? attn::launch<__half, 1, 2, true, false, true>(map, map, map, p, grid, st)
+                    : attn::launch<__half, 1, 2, false, false, true>(map, map, map, p, grid, st);
+    return p_smem ? attn::launch<__nv_bfloat16, 1, 2, true, false, true>(map, map, map, p, grid, st)
+                  : attn::launch<__nv_bfloat16, 1, 2, false, false, true>(map, map, map, p, grid, st);
+  }
   if (out_row_map) {
     if (dtype == APE_DTYPE_F16)
       return p_smem ? attn::launch<__half, 1, 2, true, true>(map, map, map, p, grid, st)
@@ -87,7 +98,7 @@ extern "C" int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t l
                                int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
                                void *stream) {
   return attn_fwd_impl(qkv, ld, out, ldo, num_seq, n, n_valid, heads, head_dim, scale, dtype, stats_out, seq_stride, causal,
-                       total_rows, nullptr, stream);
+                       total_rows, nullptr, nullptr, stream);
 }
 
 extern "C" int ape_attn_fwd_mapped(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
@@ -96,5 +107,17 @@ extern "C" int ape_attn_fwd_mapped(const void *qkv, int64_t ld, void *out, int64
   if (!out_row_map) return fail(APE_ERR_NULL_PTR, "attn: out_row_map is required (ape_attn_fwd_ex stores rows in place)");
   if (reinterpret_cast<uintptr_t>(out_row_map) & 3) return fail(APE_ERR_INVALID_ARG, "attn: out_row_map must be int32-aligned");
   return attn_fwd_impl(qkv, ld, out, ldo, num_seq, n, n_valid, heads, head_dim, scale, dtype, stats_out, seq_stride, causal,
-                       total_rows, out_row_map, stream);
+                       total_rows, out_row_map, nullptr, stream);
+}
+
+extern "C" int ape_attn_fwd_seg(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                                int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal,
+                                int64_t total_rows, const int *seg_start, void *stream) {
+  if (!seg_start) return fail(APE_ERR_NULL_PTR, "attn: seg_start is required (ape_attn_fwd_ex runs whole sequences)");
+  if (reinterpret_cast<uintptr_t>(seg_start) & 3) return fail(APE_ERR_INVALID_ARG, "attn: seg_start must be int32-aligned");
+  if (n != QM || n_valid != QM || (seq_stride != 0 && seq_stride != QM) || !causal)
+    return fail(APE_ERR_UNSUPPORTED, "attn: segments need causal tiles with n = n_valid = seq_stride = 128 (n=%d n_valid=%d "
+                "seq_stride=%d causal=%d)", n, n_valid, seq_stride, causal);
+  return attn_fwd_impl(qkv, ld, out, ldo, num_seq, n, n_valid, heads, head_dim, scale, dtype, stats_out, seq_stride, causal,
+                       total_rows, nullptr, seg_start, stream);
 }

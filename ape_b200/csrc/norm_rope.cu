@@ -765,3 +765,70 @@ extern "C" int ape_ref_update(const float *delta, const float *ref, const float 
   APE_LAUNCH(ref_update_kernel, (n + 255) / 256, 256, 0, (cudaStream_t)stream, delta, ref, valid_ratios, new_ref, ref_in, B * Q, Q, L, eps);
   return check_launch("ref_update_kernel");
 }
+
+
+// ---- text tower, length-packed prompts ------------------------------------------------------------------------------------
+// First residual of the packed text tower (TextTransformer: token_embedding(text) + positional_embedding,
+// eva02_clip/transformer.py:722-724) over rows that hold the prompts back to back: x[r] = tok_emb[tok[r]] + pos_emb[pos[r]],
+// one fp32 add as in the module sequence, so real rows carry the same bits.  Pad rows (pos < 0) are zeros; so is a row whose
+// token id or position lies outside its table (nothing is read out of bounds).  One thread per 4 channels.
+namespace ape {
+namespace {
+__global__ void __launch_bounds__(256) text_embed_packed_kernel(const float *__restrict__ tok_emb, const float *__restrict__ pos_emb,
+                                                                const int *__restrict__ tok, const int *__restrict__ pos,
+                                                                float *__restrict__ x, int rows, int D, int vocab, int ctx) {
+  pdl_prologue();
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int vec_per_row = D / 4;
+  if (idx >= (long long)rows * vec_per_row) return;
+  const int r = (int)(idx / vec_per_row), j = (int)(idx % vec_per_row);
+  const int t = tok[r], q = pos[r];
+  float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (q >= 0 && q < ctx && t >= 0 && t < vocab) {
+    const float4 a = __ldg(reinterpret_cast<const float4 *>(tok_emb + (size_t)t * D) + j);
+    const float4 b = __ldg(reinterpret_cast<const float4 *>(pos_emb + (size_t)q * D) + j);
+    o = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+  reinterpret_cast<float4 *>(x + (size_t)r * D)[j] = o;
+}
+
+// out[i] = x[rows[i]]: the end-of-text rows of the packed prompts, ahead of ln_final and the text projection
+__global__ void __launch_bounds__(256) rows_gather_kernel(const float *__restrict__ x, long long ldx, const long long *__restrict__ rows,
+                                                          float *__restrict__ out, long long ldo, int n, int D) {
+  pdl_prologue();
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int vec_per_row = D / 4;
+  if (idx >= (long long)n * vec_per_row) return;
+  const int i = (int)(idx / vec_per_row), j = (int)(idx % vec_per_row);
+  reinterpret_cast<float4 *>(out + (size_t)i * ldo)[j] = reinterpret_cast<const float4 *>(x + (size_t)rows[i] * ldx)[j];
+}
+}  // namespace
+}  // namespace ape
+
+extern "C" int ape_text_embed_packed(const float *token_embedding, const float *positional_embedding, const int *tok, const int *pos,
+                                     float *x, int rows, int D, int vocab, int ctx, void *stream) {
+  using namespace ape;
+  if (rows < 0 || D <= 0 || D % 4 || vocab <= 0 || ctx <= 0)
+    return fail(APE_ERR_INVALID_ARG, "text_embed_packed: rows=%d D=%d (multiple of 4) vocab=%d ctx=%d", rows, D, vocab, ctx);
+  if (rows == 0) return APE_OK;
+  if (!token_embedding || !positional_embedding || !tok || !pos || !x) return fail(APE_ERR_NULL_PTR, "text_embed_packed: null pointer argument");
+  if ((reinterpret_cast<uintptr_t>(token_embedding) | reinterpret_cast<uintptr_t>(positional_embedding) | reinterpret_cast<uintptr_t>(x)) & 15)
+    return fail(APE_ERR_INVALID_ARG, "text_embed_packed: tables and x must be 16-byte aligned");
+  const long long n = (long long)rows * (D / 4);
+  APE_LAUNCH(text_embed_packed_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, token_embedding, positional_embedding,
+             tok, pos, x, rows, D, vocab, ctx);
+  return check_launch("text_embed_packed_kernel");
+}
+
+extern "C" int ape_rows_gather(const float *x, int64_t ldx, const int64_t *rows, float *out, int64_t ldo, int n, int D, void *stream) {
+  using namespace ape;
+  if (n < 0 || D <= 0 || D % 4 || ldx < D || ldo < D) return fail(APE_ERR_INVALID_ARG, "rows_gather: n=%d D=%d (multiple of 4, pitches >= D)", n, D);
+  if (n == 0) return APE_OK;
+  if (!x || !rows || !out) return fail(APE_ERR_NULL_PTR, "rows_gather: null pointer argument");
+  if (ldx % 4 || ldo % 4 || ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15))
+    return fail(APE_ERR_INVALID_ARG, "rows_gather: rows must be 16-byte aligned");
+  const long long nv = (long long)n * (D / 4);
+  APE_LAUNCH(rows_gather_kernel, (unsigned)((nv + 255) / 256), 256, 0, (cudaStream_t)stream, x, (long long)ldx,
+             reinterpret_cast<const long long *>(rows), out, (long long)ldo, n, D);
+  return check_launch("rows_gather_kernel");
+}

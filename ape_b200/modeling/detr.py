@@ -445,7 +445,8 @@ class DeformableDETRSegmVL(nn.Module):
             if cache and key in self._text_cache:
                 features_l = self._text_cache[key]
             else:
-                features_l = self.model_language.forward_text(text_list, cache=cache)["last_hidden_state_eot"]
+                kw = {"need_hidden": False} if getattr(self.model_language, "pack_prompts", False) else {}
+                features_l = self.model_language.forward_text(text_list, cache=cache, **kw)["last_hidden_state_eot"]
                 if cache:
                     self._text_cache[key] = features_l
             if cache and features_l.device != self.device:  # keep cached vocabularies resident on the device
@@ -462,7 +463,9 @@ class DeformableDETRSegmVL(nn.Module):
         # phrase / expression (:284-337)
         if not text_list:
             raise NotImplementedError("ape_b200: phrase prompts need `text_prompt` (or `expressions`) at inference")
-        features_l = self.model_language.forward_text(text_list)["last_hidden_state_eot"].to(self.device)
+        # a text tower that packs its prompts by length reads out the end-of-text rows alone when told that nothing else is wanted
+        kw = {"need_hidden": False} if getattr(self.model_language, "pack_prompts", False) else {}
+        features_l = self.model_language.forward_text(text_list, **kw)["last_hidden_state_eot"].to(self.device)
         if self.text_feature_bank and not self.text_feature_bank_reset and 0 <= dataset_id < len(self.dataset_names):
             n = self.criterion[dataset_id].num_classes
             features_l = torch.cat([features_l, self.features_phrase_bank[dataset_id]], dim=0)[: max(len(text_list), n)]

@@ -535,7 +535,7 @@ def attention_supported(n, head_dim, dtype):
 
 
 def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_out=False, seq_stride=None, causal=False,
-                  out_row_map=None, out=None):
+                  out_row_map=None, out=None, seg_start=None):
     """softmax(q k^T * scale) v for every (sequence, head) straight from the fused qkv buffer [num_seq*n, 3*heads*64]
     (ape_attn_fwd: flash attention on the wgmma tensor cores).  Returns [num_seq*n, heads*64].
     n_valid: sequences are padded to n rows and only the first n_valid keys count (rows beyond must be finite).
@@ -544,11 +544,18 @@ def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_o
     past n_valid are not written); causal: key t attends to keys <= t.
     out_row_map: int32 [qkv rows] (ape_attn_fwd_mapped): query row r is stored at row out_row_map[r] of `out` (required
     then, [rows, heads*64] in qkv's dtype) and of the statistics ([out rows, heads, 2]); -1 stores nothing.  The mapped rows
-    must be distinct rows of `out`; rows no query maps to keep what `out` held."""
+    must be distinct rows of `out`; rows no query maps to keep what `out` held.
+    seg_start: int32 [num_seq * 128] (ape_attn_fwd_seg): every 128-row tile holds several short sequences; query row r
+    attends key k of its tile iff seg_start[r] <= k <= r, with seg_start[r] the position in the tile where r's sequence
+    starts (a pad row: its own position).  Needs n = 128, causal=True and no n_valid / seq_stride / out_row_map."""
     _require(qkv.is_cuda and qkv.dim() == 2 and qkv.stride(1) == 1, "attention: qkv must be a 2-D CUDA tensor")
     stride = n if seq_stride is None else int(seq_stride)
     _require(qkv.shape[0] >= (num_seq - 1) * stride + (n_valid or n) and qkv.shape[1] == 3 * heads * head_dim, "attention: qkv shape")
     C = heads * head_dim
+    if seg_start is not None:
+        _require(seg_start.is_cuda and seg_start.dtype == torch.int32 and seg_start.dim() == 1 and seg_start.is_contiguous() and
+                 seg_start.numel() == num_seq * n, "attention: seg_start must be a contiguous int32 CUDA vector with one entry per query row")
+        _require(out_row_map is None and not stats_out, "attention: seg_start goes with neither out_row_map nor stats_out")
     if out_row_map is not None:
         _require(out_row_map.is_cuda and out_row_map.dtype == torch.int32 and out_row_map.dim() == 1 and
                  out_row_map.is_contiguous() and out_row_map.numel() >= (num_seq - 1) * stride + min(stride, n),
@@ -566,12 +573,46 @@ def attention_qkv(qkv, num_seq, n, heads, head_dim, scale, n_valid=None, stats_o
             int(heads), int(head_dim), float(scale), _lib.dtype_code(qkv.dtype), stats.data_ptr() if stats is not None else None,
             stride, 1 if causal else 0, int(qkv.shape[0]))
     with torch.cuda.device(qkv.device), _timed(("attention", num_seq, n, heads)):
-        if out_row_map is None:
+        if seg_start is not None:
+            rc = _lib.lib.ape_attn_fwd_seg(*args, seg_start.data_ptr(), _lib.current_stream_ptr())
+        elif out_row_map is None:
             rc = _lib.lib.ape_attn_fwd_ex(*args, _lib.current_stream_ptr())
         else:
             rc = _lib.lib.ape_attn_fwd_mapped(*args, out_row_map.data_ptr(), _lib.current_stream_ptr())
     _lib.check(rc, "ape_attn_fwd")
     return (out, stats) if stats_out else out
+
+
+def text_embed_packed(token_embedding, positional_embedding, tok, pos):
+    """x[r] = token_embedding[tok[r]] + positional_embedding[pos[r]] as fp32 [rows, D] (ape_text_embed_packed): the text
+    tower's first residual over length-packed prompts.  Tables fp32 [vocab, D] / [ctx, D]; tok / pos int32 [rows]; rows with
+    pos < 0 (pad rows) are zeros."""
+    for t in (token_embedding, positional_embedding):
+        _require(t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.is_contiguous(), "text_embed_packed: contiguous fp32 CUDA tables")
+    D = token_embedding.shape[1]
+    _require(positional_embedding.shape[1] == D, "text_embed_packed: tables of one width")
+    for t in (tok, pos):
+        _require(t.is_cuda and t.dtype == torch.int32 and t.dim() == 1 and t.is_contiguous() and t.numel() == tok.numel(),
+                 "text_embed_packed: tok / pos must be contiguous int32 CUDA vectors of one length")
+    x = torch.empty((tok.numel(), D), dtype=torch.float32, device=tok.device)
+    with torch.cuda.device(tok.device), _timed(("text_embed_packed", tok.numel(), D)):
+        rc = _lib.lib.ape_text_embed_packed(token_embedding.data_ptr(), positional_embedding.data_ptr(), tok.data_ptr(), pos.data_ptr(),
+                                            x.data_ptr(), tok.numel(), D, token_embedding.shape[0], positional_embedding.shape[0],
+                                            _lib.current_stream_ptr())
+    _lib.check(rc, "ape_text_embed_packed")
+    return x
+
+
+def rows_gather(x, rows):
+    """x[rows] for fp32 x [M, D] (unit inner stride) and int64 rows [n], every entry in [0, M) (ape_rows_gather)."""
+    _require(x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1, "rows_gather: fp32 2-D CUDA tensor")
+    _require(rows.is_cuda and rows.dtype == torch.int64 and rows.dim() == 1 and rows.is_contiguous(), "rows_gather: contiguous int64 CUDA rows")
+    out = torch.empty((rows.numel(), x.shape[1]), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device), _timed(("rows_gather", rows.numel(), x.shape[1])):
+        rc = _lib.lib.ape_rows_gather(x.data_ptr(), x.stride(0), rows.data_ptr(), out.data_ptr(), out.stride(0), rows.numel(),
+                                      x.shape[1], _lib.current_stream_ptr())
+    _lib.check(rc, "ape_rows_gather")
+    return out
 
 
 def attention_cross(q, k, v, num_seq, nq, nkv, n_valid, heads, head_dim, scale):

@@ -281,6 +281,18 @@ int ape_rope_qk(void *qkv, int64_t ld, const float *cos_table, const float *sin_
                 int C, int head_dim, int npos, int dtype, void *stream);
 
 /*
+ * First residual of the text tower over length-packed prompts (TextTransformer.forward, eva02_clip/transformer.py:722-724):
+ * x[r, :] = token_embedding[tok[r], :] + positional_embedding[pos[r], :], all fp32, x [rows, D] contiguous, D % 4 == 0,
+ * tables [vocab, D] / [ctx, D] contiguous and 16-byte aligned; tok / pos int32 [rows] (device).  A row with pos[r] < 0 (a
+ * pad row of a tile) is written as zeros, and so is a row whose token id or position lies outside its table.
+ */
+int ape_text_embed_packed(const float *token_embedding, const float *positional_embedding, const int *tok, const int *pos,
+                          float *x, int rows, int D, int vocab, int ctx, void *stream);
+/* out[i, :] = x[rows[i], :] for i < n: fp32 rows of D elements (D % 4 == 0, pitches ldx / ldo in elements, 16-byte aligned
+ * rows), rows int64 [n] on the device, every entry a row of x.  The text tower reads its end-of-text rows with it. */
+int ape_rows_gather(const float *x, int64_t ldx, const int64_t *rows, float *out, int64_t ldo, int n, int D, void *stream);
+
+/*
  * Softmax attention core of the ViT blocks (Attention.forward, ape/modeling/backbone/vit_eva_clip.py:218-319, the
  * part xformers / F.scaled_dot_product_attention computes there): out = softmax(q k^T * scale) v per (sequence, head),
  * flash-attention style on the wgmma tensor cores.  qkv [num_seq * n, >= 3*heads*64] (pitch ld elements): columns
@@ -309,6 +321,14 @@ int ape_attn_fwd_ex(const void *qkv, int64_t ld, void *out, int64_t ldo, int num
 int ape_attn_fwd_mapped(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
                         int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
                         const int *out_row_map, void *stream);
+/* ape_attn_fwd_ex over tiles that hold several short sequences each (the text tower's length-packed prompts): seg_start
+ * (int32, device, one entry per query row of the launch) gives, for query row r of a tile, the position inside that tile
+ * where r's own sequence starts; r attends key k of its tile iff seg_start[r] <= k <= r.  A pad row carries its own position
+ * and so attends only itself (finite output).  n = n_valid = 128, seq_stride 0 or 128, causal != 0: anything else is
+ * APE_ERR_UNSUPPORTED.  With seg_start[r] = 0 everywhere the result equals ape_attn_fwd_ex(causal = 1) bit for bit. */
+int ape_attn_fwd_seg(const void *qkv, int64_t ld, void *out, int64_t ldo, int num_seq, int n, int n_valid, int heads,
+                     int head_dim, float scale, int dtype, float *stats_out, int seq_stride, int causal, int64_t total_rows,
+                     const int *seg_start, void *stream);
 
 /* Kernel structure behind ape_attn_fwd*: 0 = P written to shared memory and read from there by the P.V wgmma, 1 = P kept in
  * registers as the A operand of the P.V wgmma.  set >= 0 selects it for the process; returns the value in force
