@@ -138,6 +138,10 @@ def _declare(lib):
     lib.ape_mask_paste_rle.argtypes = [_vp, _vp, _i, _i, _i, _i, ctypes.c_float, _vp, _vp, _vp, _vp]
     lib.ape_rle_to_string.restype = _i
     lib.ape_rle_to_string.argtypes = [_vp, _i, _vp]
+    lib.ape_mask_pack_workspace_bytes.restype = _i64
+    lib.ape_mask_pack_workspace_bytes.argtypes = [_i] * 6
+    lib.ape_mask_pack.restype = _i
+    lib.ape_mask_pack.argtypes = [_vp] * 5 + [_i] * 10 + [_vp]
     lib.ape_resample_ksize.restype = _i
     lib.ape_resample_ksize.argtypes = [_i, _i]
     lib.ape_resample_coeffs_u8.restype = _i
@@ -208,6 +212,8 @@ EXPORTS = (
     "ape_mask_paste",
     "ape_mask_paste_rle",
     "ape_rle_to_string",
+    "ape_mask_pack_workspace_bytes",
+    "ape_mask_pack",
     "ape_resample_ksize",
     "ape_resample_coeffs_u8",
     "ape_resample_u8",

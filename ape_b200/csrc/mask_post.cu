@@ -31,11 +31,14 @@ __device__ __forceinline__ float ldf(const T *p) {
 }
 
 // bits[k][Y][X / 32] bit (X % 32) = bilinear_upsample(logits[index[k]])(Y, X) > 0
-template <typename T>
+// SKIP (the packed path, mask_pack_* below): slot k does nothing unless live[k].  The extra parameter comes last so that the
+// other parameters keep their places and the SKIP = false kernels compile to what they were before it existed.
+template <typename T, bool SKIP>
 __global__ void __launch_bounds__(256) mask_binarize_kernel(const T *__restrict__ logits, const long long *__restrict__ index,
                                                             uint32_t *__restrict__ bits, int h, int w, int Hp, int Wp,
-                                                            float scale_h, float scale_w) {
+                                                            float scale_h, float scale_w, const int *__restrict__ live) {
   pdl_prologue();
+  if (SKIP && !__ldg(live + blockIdx.z)) return;
   const int words = (Wp + 31) >> 5;
   const int lane = threadIdx.x & 31;
   const int word = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -64,9 +67,12 @@ __device__ __forceinline__ float bit_at(const uint32_t *m, int words, int y, int
 }
 
 // torchvision roi_align (aligned = true, spatial_scale 1, sampling_ratio 0) of the k-th bit mask over box k, >= 0.5
+template <bool SKIP>
 __global__ void __launch_bounds__(256) mask_roialign_kernel(const uint32_t *__restrict__ bits, const float *__restrict__ boxes,
-                                                            uint8_t *__restrict__ out, int Hp, int Wp, int S) {
+                                                            uint8_t *__restrict__ out, int Hp, int Wp, int S,
+                                                            const int *__restrict__ live) {
   pdl_prologue();
+  if (SKIP && !__ldg(live + blockIdx.y)) return;
   const int k = blockIdx.y;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= S * S) return;
@@ -154,11 +160,14 @@ __global__ void __launch_bounds__(256) mask_paste_kernel(const uint8_t *__restri
 //   (exclusive scan of the per-column numbers, on the caller's side)
 //   pass 2  the positions j = x * H + y of the boundaries, written in order at the column's offset.
 // Run lengths are the differences of consecutive positions (plus the leading and the trailing run).
-template <bool WRITE>
+// SKIP: mask n does nothing unless live[n] (its counts and positions are then left unwritten).
+template <bool WRITE, bool SKIP>
 __global__ void __launch_bounds__(256) mask_rle_kernel(const uint8_t *__restrict__ masks, const float *__restrict__ boxes, int S,
                                                        int img_h, int img_w, float threshold, int *__restrict__ col_count,
-                                                       const long long *__restrict__ col_offset, int *__restrict__ positions) {
+                                                       const long long *__restrict__ col_offset, int *__restrict__ positions,
+                                                       const int *__restrict__ live) {
   pdl_prologue();
+  if (SKIP && !__ldg(live + blockIdx.y)) return;
   const int n = blockIdx.y, x = blockIdx.x;
   const float4 b = __ldg(reinterpret_cast<const float4 *>(boxes) + n);
   const uint8_t *m = masks + (size_t)n * S * S;
@@ -211,6 +220,166 @@ __global__ void __launch_bounds__(256) mask_rle_kernel(const uint8_t *__restrict
   if (!WRITE && threadIdx.x == 0) col_count[(size_t)n * img_w + x] = s_base;
 }
 
+// ---- the kept masks of the packed selection rows as COCO run-length codes in fixed-size slots -----------------------------
+// Input: the rows of DeformableDETRSegmVL.forward_packed, [topk, 13] fp32 per image (x1, y1, x2, y2, score, class, query index,
+// candidates, kept nk, image h, w, output h, w).  Everything the host path reads back (nk, the run totals) stays on the device:
+// every slot gets a CTA, and the slots that hold nothing return after reading a flag.  Output row of a slot (PACK_ROW bytes
+// before the SLOT bytes): the 13 fp32 columns, then int32 kind (0 nothing, 1 "counts" characters, 2 the 128 x 128 mask as bits)
+// and int32 length, then the slot.
+constexpr int PACK_COLS = 13, PACK_HEAD = 4 * PACK_COLS + 8;
+constexpr int SLOT_EMPTY = 0, SLOT_CHARS = 1, SLOT_BITS = 2;
+
+// detector_postprocess (detr.py) on one row: box * (output / image size, a double rounded to fp32), clamped to the output,
+// kept iff width and height are > 0.  live[k] = k < nk and kept; the crop box is the row's box, the paste box the rescaled one.
+__global__ void __launch_bounds__(256) mask_pack_prep_kernel(const float *__restrict__ rows, int topk, long long *__restrict__ index,
+                                                             float4 *__restrict__ crop_box, float4 *__restrict__ paste_box,
+                                                             int *__restrict__ live) {
+  pdl_prologue();
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= topk) return;
+  const float *r = rows + (size_t)k * PACK_COLS;
+  const int nk = (int)r[8];
+  int ok = 0;
+  if (k < nk) {
+    const float h = r[9], w = r[10], oh = r[11], ow = r[12];
+    const float sx = (float)((double)ow / (double)w), sy = (float)((double)oh / (double)h);
+    const float x1 = fminf(fmaxf(__fmul_rn(r[0], sx), 0.f), ow), y1 = fminf(fmaxf(__fmul_rn(r[1], sy), 0.f), oh);
+    const float x2 = fminf(fmaxf(__fmul_rn(r[2], sx), 0.f), ow), y2 = fminf(fmaxf(__fmul_rn(r[3], sy), 0.f), oh);
+    ok = __fsub_rn(x2, x1) > 0.f && __fsub_rn(y2, y1) > 0.f;
+    index[k] = (long long)r[6];
+    crop_box[k] = make_float4(r[0], r[1], r[2], r[3]);
+    paste_box[k] = make_float4(x1, y1, x2, y2);
+  }
+  live[k] = ok;
+}
+
+// block-wide exclusive sum over 256 threads; returns this thread's offset, *sum the total.  s_warp holds 8 ints.
+__device__ __forceinline__ int block_excl_scan_256(int v, int *s_warp, int *sum) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += t;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  int before = 0, total = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    before += i < warp ? s_warp[i] : 0;
+    total += s_warp[i];
+  }
+  __syncthreads();  // s_warp is reused by the next call
+  *sum = total;
+  return before + incl - v;
+}
+
+// One CTA per slot: exclusive scan of the slot's column counts -> col_offset (the slot's positions start at n * slot), the
+// number of boundaries, and chars[n] = whether they fit: m boundaries make m + 1 counts of at least one character each, so a slot
+// with m >= slot boundaries goes straight to bits and the positions workspace stays at slot int32 per slot.
+__global__ void __launch_bounds__(256) mask_pack_scan_kernel(const int *__restrict__ col_count, const int *__restrict__ live, int W,
+                                                             int slot, long long *__restrict__ col_offset, int *__restrict__ total,
+                                                             int *__restrict__ chars) {
+  pdl_prologue();
+  const int n = blockIdx.x;
+  if (!__ldg(live + n)) {
+    if (threadIdx.x == 0) chars[n] = 0;
+    return;
+  }
+  __shared__ int s_warp[8];
+  long long base = 0;
+  for (int x0 = 0; x0 < W; x0 += 256) {
+    const int x = x0 + threadIdx.x;
+    const int v = x < W ? col_count[(size_t)n * W + x] : 0;
+    int sum;
+    const int off = block_excl_scan_256(v, s_warp, &sum);
+    if (x < W) col_offset[(size_t)n * W + x] = (long long)n * slot + base + off;
+    base += sum;
+  }
+  if (threadIdx.x == 0) {
+    total[n] = (int)min(base, 0x7fffffffLL);
+    chars[n] = base < slot;
+  }
+}
+
+// cocoapi rleToString of one count (see ape_rle_to_string): number of characters, and the characters when out != NULL
+__device__ __forceinline__ int rle_chars(long long x, uint8_t *out, int room) {
+  int n = 0;
+  bool more = true;
+  while (more) {
+    int c = (int)(x & 0x1f);
+    x >>= 5;
+    more = (c & 0x10) ? x != -1 : x != 0;
+    if (more) c |= 0x20;
+    if (out && n < room) out[n] = (uint8_t)(c + 48);
+    ++n;
+  }
+  return n;
+}
+
+// One CTA per slot: the row, the slot word and the slot.  Counts from the boundary positions p (c_i = p_i - p_{i-1}, with
+// p_{-1} = 0 and a last boundary at H * W), delta-coded and written at their scanned character offsets; a code longer than the
+// slot is replaced by the slot's 128 x 128 mask, bit (y * S + x) at byte >> 3, bit & 7.  Bytes after the length are zero.
+__global__ void __launch_bounds__(256) mask_pack_encode_kernel(const float *__restrict__ rows, const int *__restrict__ live,
+                                                               const int *__restrict__ chars, const int *__restrict__ total,
+                                                               const int *__restrict__ positions, const uint8_t *__restrict__ masks,
+                                                               int S, int H, int W, int slot, uint8_t *__restrict__ out) {
+  pdl_prologue();
+  const int n = blockIdx.x, tid = threadIdx.x;
+  uint8_t *dst = out + (size_t)n * (PACK_HEAD + slot);
+  uint8_t *body = dst + PACK_HEAD;
+  if (tid < PACK_COLS) reinterpret_cast<float *>(dst)[tid] = rows[(size_t)n * PACK_COLS + tid];
+  __shared__ int s_warp[8];
+  int kind = SLOT_EMPTY, len = 0;
+  if (__ldg(live + n)) {
+    kind = SLOT_BITS;
+    if (__ldg(chars + n)) {
+      const int m = total[n] + 1;
+      const long long HW = (long long)H * W;
+      const int *p = positions + (size_t)n * slot;
+      auto P = [&](int j) -> long long { return j < 0 ? 0 : j >= m - 1 ? HW : (long long)p[j]; };
+      int base = 0;
+      for (int i0 = 0; i0 < m && base <= slot; i0 += 256) {  // base is the same in every thread
+        const int i = i0 + tid;
+        long long x = 0;
+        int nc = 0;
+        if (i < m) {
+          x = P(i) - P(i - 1);
+          if (i > 2) x -= P(i - 2) - P(i - 3);
+          nc = rle_chars(x, nullptr, 0);
+        }
+        int sum;
+        const int off = base + block_excl_scan_256(nc, s_warp, &sum);
+        if (i < m && off < slot) rle_chars(x, body + off, slot - off);
+        base += sum;
+      }
+      if (base <= slot) {
+        kind = SLOT_CHARS;
+        len = base;
+      }
+    }
+    __syncthreads();  // the characters of a code that did not fit are overwritten below
+    if (kind == SLOT_BITS) {
+      const uint8_t *m = masks + (size_t)n * S * S;
+      len = (S * S + 7) / 8;
+      for (int j = tid; j < len; j += blockDim.x) {
+        uint32_t b = 0;
+        for (int t = 0; t < 8; ++t) {
+          const int px = j * 8 + t;
+          if (px < S * S && __ldg(m + px)) b |= 1u << t;
+        }
+        body[j] = (uint8_t)b;
+      }
+    }
+  }
+  for (int j = len + tid; j < slot; j += blockDim.x) body[j] = 0;
+  if (tid == 0) {
+    reinterpret_cast<int *>(dst + 4 * PACK_COLS)[0] = kind;
+    reinterpret_cast<int *>(dst + 4 * PACK_COLS)[1] = len;
+  }
+}
+
 }  // namespace
 }  // namespace ape
 
@@ -234,16 +403,20 @@ extern "C" int ape_mask_crop(const void *logits, const int64_t *index, const flo
   dim3 g1((words + 7) / 8, Hp, K);
   uint32_t *bits = reinterpret_cast<uint32_t *>(workspace);
   if (dtype == APE_DTYPE_F32)
-    APE_LAUNCH(mask_binarize_kernel<float>, g1, 256, 0, st, (const float *)logits, (const long long *)index, bits, h, w, Hp, Wp, sh, sw);
+    APE_LAUNCH((mask_binarize_kernel<float, false>), g1, 256, 0, st, (const float *)logits, (const long long *)index, bits, h, w, Hp, Wp, sh, sw,
+               (const int *)nullptr);
   else if (dtype == APE_DTYPE_F16)
-    APE_LAUNCH(mask_binarize_kernel<__half>, g1, 256, 0, st, (const __half *)logits, (const long long *)index, bits, h, w, Hp, Wp, sh, sw);
+    APE_LAUNCH((mask_binarize_kernel<__half, false>), g1, 256, 0, st, (const __half *)logits, (const long long *)index, bits, h, w, Hp, Wp, sh,
+               sw, (const int *)nullptr);
   else if (dtype == APE_DTYPE_BF16)
-    APE_LAUNCH(mask_binarize_kernel<__nv_bfloat16>, g1, 256, 0, st, (const __nv_bfloat16 *)logits, (const long long *)index, bits, h, w, Hp, Wp, sh, sw);
+    APE_LAUNCH((mask_binarize_kernel<__nv_bfloat16, false>), g1, 256, 0, st, (const __nv_bfloat16 *)logits, (const long long *)index, bits, h, w,
+               Hp, Wp, sh, sw, (const int *)nullptr);
   else
     return fail(APE_ERR_INVALID_ARG, "mask_crop: dtype %d", dtype);
   int rc = check_launch("mask_binarize_kernel");
   if (rc) return rc;
-  APE_LAUNCH(mask_roialign_kernel, dim3((S * S + 255) / 256, K), 256, 0, st, (const uint32_t *)bits, boxes, out, Hp, Wp, S);
+  APE_LAUNCH((mask_roialign_kernel<false>), dim3((S * S + 255) / 256, K), 256, 0, st, (const uint32_t *)bits, boxes, out, Hp, Wp, S,
+             (const int *)nullptr);
   return check_launch("mask_roialign_kernel");
 }
 
@@ -271,14 +444,116 @@ extern "C" int ape_mask_paste_rle(const uint8_t *masks, const float *boxes, int 
   cudaStream_t st = (cudaStream_t)stream;
   if (positions == nullptr) {
     if (!col_count) return fail(APE_ERR_NULL_PTR, "mask_paste_rle: null col_count");
-    APE_LAUNCH(mask_rle_kernel<false>, dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, col_count,
-               (const long long *)nullptr, (int *)nullptr);
+    APE_LAUNCH((mask_rle_kernel<false, false>), dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, col_count,
+               (const long long *)nullptr, (int *)nullptr, (const int *)nullptr);
   } else {
     if (!col_offset) return fail(APE_ERR_NULL_PTR, "mask_paste_rle: null col_offset");
-    APE_LAUNCH(mask_rle_kernel<true>, dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, (int *)nullptr,
-               (const long long *)col_offset, positions);
+    APE_LAUNCH((mask_rle_kernel<true, false>), dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, (int *)nullptr,
+               (const long long *)col_offset, positions, (const int *)nullptr);
   }
   return check_launch("mask_rle_kernel");
+}
+
+namespace {
+// workspace of ape_mask_pack, every part 256-byte aligned; reused image after image
+struct PackWs {
+  long long *index;
+  float4 *crop_box, *paste_box;
+  int *live, *chars, *total, *col_count, *positions;
+  long long *col_offset;
+  uint32_t *bits;
+  uint8_t *masks;
+  int64_t bytes;
+};
+
+PackWs pack_ws(void *base, int topk, int Hp, int Wp, int max_w, int S, int slot) {
+  PackWs w{};
+  int64_t off = 0;
+  auto take = [&](int64_t n) {
+    const int64_t o = off;
+    off += (n + 255) / 256 * 256;
+    return reinterpret_cast<char *>(reinterpret_cast<uintptr_t>(base) + o);
+  };
+  w.index = reinterpret_cast<long long *>(take(8LL * topk));
+  w.crop_box = reinterpret_cast<float4 *>(take(16LL * topk));
+  w.paste_box = reinterpret_cast<float4 *>(take(16LL * topk));
+  w.live = reinterpret_cast<int *>(take(4LL * topk));
+  w.chars = reinterpret_cast<int *>(take(4LL * topk));
+  w.total = reinterpret_cast<int *>(take(4LL * topk));
+  w.col_count = reinterpret_cast<int *>(take(4LL * topk * max_w));
+  w.col_offset = reinterpret_cast<long long *>(take(8LL * topk * max_w));
+  w.positions = reinterpret_cast<int *>(take(4LL * topk * slot));
+  w.bits = reinterpret_cast<uint32_t *>(take(ape_mask_crop_workspace_bytes(topk, Hp, Wp)));
+  w.masks = reinterpret_cast<uint8_t *>(take((int64_t)topk * S * S));
+  w.bytes = off;
+  return w;
+}
+}  // namespace
+
+extern "C" int64_t ape_mask_pack_workspace_bytes(int topk, int Hp, int Wp, int max_w, int S, int slot) {
+  if (topk <= 0 || Hp <= 0 || Wp <= 0 || max_w <= 0 || S <= 0 || slot <= 0) return 0;
+  return pack_ws(nullptr, topk, Hp, Wp, max_w, S, slot).bytes;
+}
+
+extern "C" int ape_mask_pack(const void *logits, const float *rows, const int *out_hw, void *workspace, uint8_t *out, int B, int topk,
+                             int Q, int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream) {
+  if (B == 0 || topk == 0) return APE_OK;
+  if (!logits || !rows || !out_hw || !workspace || !out) return fail(APE_ERR_NULL_PTR, "mask_pack: null pointer");
+  if (B < 0 || topk < 0 || topk > 65535 || Q <= 0 || h <= 0 || w <= 0 || Hp <= 0 || Wp <= 0 || Hp > 65535 || S <= 0 || S > 1024)
+    return fail(APE_ERR_INVALID_ARG, "mask_pack: bad geometry B=%d topk=%d Q=%d %dx%d -> %dx%d, S=%d", B, topk, Q, h, w, Hp, Wp, S);
+  if (slot % 4 != 0 || slot < (S * S + 7) / 8)
+    return fail(APE_ERR_INVALID_ARG, "mask_pack: slot of %d bytes (a multiple of 4 that holds the %d x %d mask as bits)", slot, S, S);
+  if ((reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(out)) & 3)
+    return fail(APE_ERR_INVALID_ARG, "mask_pack: rows and out must be 4-byte aligned");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(APE_ERR_INVALID_ARG, "mask_pack: workspace must be 256-byte aligned");
+  if (dtype != APE_DTYPE_F32 && dtype != APE_DTYPE_F16 && dtype != APE_DTYPE_BF16) return fail(APE_ERR_INVALID_ARG, "mask_pack: dtype %d", dtype);
+  int max_w = 0;
+  for (int b = 0; b < B; ++b) {
+    const int oh = out_hw[2 * b], ow = out_hw[2 * b + 1];
+    if (oh <= 0 || ow <= 0 || (long long)oh * ow > 0x7fffffffLL)
+      return fail(APE_ERR_INVALID_ARG, "mask_pack: bad output size %dx%d of image %d", oh, ow, b);
+    max_w = max(max_w, ow);
+  }
+  const PackWs ws = pack_ws(workspace, topk, Hp, Wp, max_w, S, slot);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int words = (Wp + 31) / 32;
+  const float sh = (float)h / (float)Hp, sw = (float)w / (float)Wp;  // as ape_mask_crop
+  const size_t esize = dtype == APE_DTYPE_F32 ? 4 : 2;
+  int rc;
+  for (int b = 0; b < B; ++b) {
+    const int H = out_hw[2 * b], W = out_hw[2 * b + 1];
+    const float *r = rows + (size_t)b * topk * PACK_COLS;
+    const void *lg = reinterpret_cast<const char *>(logits) + (size_t)b * Q * h * w * esize;
+    APE_LAUNCH(mask_pack_prep_kernel, (topk + 255) / 256, 256, 0, st, r, topk, ws.index, ws.crop_box, ws.paste_box, ws.live);
+    if ((rc = check_launch("mask_pack_prep_kernel"))) return rc;
+    const dim3 g1((words + 7) / 8, Hp, topk);
+    if (dtype == APE_DTYPE_F32)
+      APE_LAUNCH((mask_binarize_kernel<float, true>), g1, 256, 0, st, (const float *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
+                 Wp, sh, sw, (const int *)ws.live);
+    else if (dtype == APE_DTYPE_F16)
+      APE_LAUNCH((mask_binarize_kernel<__half, true>), g1, 256, 0, st, (const __half *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
+                 Wp, sh, sw, (const int *)ws.live);
+    else
+      APE_LAUNCH((mask_binarize_kernel<__nv_bfloat16, true>), g1, 256, 0, st, (const __nv_bfloat16 *)lg, (const long long *)ws.index,
+                 ws.bits, h, w, Hp, Wp, sh, sw, (const int *)ws.live);
+    if ((rc = check_launch("mask_binarize_kernel"))) return rc;
+    APE_LAUNCH((mask_roialign_kernel<true>), dim3((S * S + 255) / 256, topk), 256, 0, st, (const uint32_t *)ws.bits,
+               (const float *)ws.crop_box, ws.masks, Hp, Wp, S, (const int *)ws.live);
+    if ((rc = check_launch("mask_roialign_kernel"))) return rc;
+    APE_LAUNCH((mask_rle_kernel<false, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
+               0.5f, ws.col_count, (const long long *)nullptr, (int *)nullptr, (const int *)ws.live);
+    if ((rc = check_launch("mask_rle_kernel"))) return rc;
+    APE_LAUNCH(mask_pack_scan_kernel, topk, 256, 0, st, (const int *)ws.col_count, (const int *)ws.live, W, slot, ws.col_offset,
+               ws.total, ws.chars);
+    if ((rc = check_launch("mask_pack_scan_kernel"))) return rc;
+    APE_LAUNCH((mask_rle_kernel<true, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
+               0.5f, (int *)nullptr, (const long long *)ws.col_offset, ws.positions, (const int *)ws.chars);
+    if ((rc = check_launch("mask_rle_kernel"))) return rc;
+    APE_LAUNCH(mask_pack_encode_kernel, topk, 256, 0, st, r, (const int *)ws.live, (const int *)ws.chars, (const int *)ws.total,
+               (const int *)ws.positions, (const uint8_t *)ws.masks, S, H, W, slot, out + (size_t)b * topk * (PACK_HEAD + slot));
+    if ((rc = check_launch("mask_pack_encode_kernel"))) return rc;
+  }
+  return APE_OK;
 }
 
 // cocoapi rleToString (maskApi.c): run lengths -> the compressed ASCII string of the "counts" field (HOST function).

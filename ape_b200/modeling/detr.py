@@ -287,6 +287,9 @@ class DeformableDETRSegmVL(nn.Module):
         # computed on the device from the 128 x 128 masks (what the evaluators encode every mask into: d3_evaluation.py:466-468),
         # 314 MB of booleans per 300 detections at 1024^2 that are never written or copied
         self.mask_format = "bitmask"
+        # bytes per detection slot for the run-length code of a mask in `forward_packed` (a code that does not fit travels as
+        # the 128 x 128 mask's 2048 bytes of bits and is encoded on the receiving side); a multiple of 4, at least 2048
+        self.mask_slot_bytes = 4096
         # "maps": `sem_seg` [N_classes, H, W] fp32 scores as the reference returns them; "label": `sem_seg_label` int64 [H, W] (the
         # first argmax over classes of that map, all SemSegEvaluator keeps) and `sem_seg_score` fp32 [H, W] (its value).  On CUDA
         # with a 16-bit engine_dtype the map is never formed (csrc/semseg.cu: 5 GB per image at 1203 classes and 1024^2)
@@ -509,17 +512,25 @@ class DeformableDETRSegmVL(nn.Module):
                 # thresholding touches the host
                 # the final selection (threshold, class-aware NMS, top-k: static shapes) rides in the same graph when boxes are
                 # all that is asked for; its configuration is part of the graph key
-                sel = None
-                if do_postprocess in (True, "packed") and not need_masks and self.static_inference_cap > 0 and \
+                sel, const = None, (geo, prompt)
+                # forward_packed with instance masks: the mask stage (csrc/mask_post.cu, ape_mask_pack) follows the selection in
+                # the graph; the output sizes and the slot size join the key
+                packed_masks = do_postprocess == "packed" and self.instance_on and self.test_mask_on and \
+                    not (self.semantic_on or self.panoptic_on)
+                if do_postprocess in (True, "packed") and (not need_masks or packed_masks) and self.static_inference_cap > 0 and \
                         self.test_topk_per_image >= 0 and self.num_queries <= 1024:
                     ent = self.eval_dataset_entity
                     sel = (tuple(image_sizes), bool(getattr(self, "_static_overflowed", False)), float(self.test_score_thresh),
                            float(self.test_nms_thresh), int(self.test_topk_per_image), int(self.static_inference_cap),
                            self.eval_dataset_id, bool(self.instance_on and not (ent and "thing" not in ent)))
+                    const = (geo, prompt, sel)
+                    if packed_masks:
+                        sel += ((self._output_sizes(batched_inputs, image_sizes), int(self.mask_slot_bytes)),)
+                        const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
                     ("forward", prompt, tuple(images.shape), tuple(image_sizes), tuple(features_l.shape), need_masks, sel),
-                    self._stage_all, (images, fusion, features_l), (geo, prompt, sel))
+                    self._stage_all, (images, fusion, features_l), const)
                 self.transformer.last_topk_proposals = topk
                 mark("encode")
                 mark("select")
@@ -554,7 +565,7 @@ class DeformableDETRSegmVL(nn.Module):
         if do_postprocess == "raw":  # logits / boxes stay on the device, no selection here
             return box_cls, box_pred, image_sizes
         if do_postprocess == "packed":  # forward_packed: the selection computed INSIDE the captured graph when there is one
-            return box_cls, box_pred, image_sizes, graph_pack
+            return box_cls, box_pred, image_sizes, graph_pack, mask_pred, tuple(images.shape[-2:])
         # the three branches are gated by the entity of the evaluated dataset (:575-577, :628-630, :671-673)
         ent = self.eval_dataset_entity
         instance_on = self.instance_on and not (ent and "thing" not in ent)
@@ -660,7 +671,7 @@ class DeformableDETRSegmVL(nn.Module):
             return features_l
         return 0.0 * features_l + 1.0 * fusion_out.float()  # (:448)
 
-    def _stage_all(self, images, fusion, features_l, geo, prompt, sel=None):
+    def _stage_all(self, images, fusion, features_l, geo, prompt, sel=None, size_columns=None):
         memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._stage_encode(images, fusion, geo)
         topk = self.transformer.stage_select(enc_cls, enc_coord, geo)
         features_l = self._mix_text(prompt, features_l, fusion_out)
@@ -670,6 +681,8 @@ class DeformableDETRSegmVL(nn.Module):
         if sel is not None:  # (image sizes, class-wise path?, thresholds ..., instance branch on?) — see forward()
             det_cls = self._detector_box_cls(box_cls) if sel[7] else box_cls
             pack = self._select_device(det_cls, box_pred, sel[0], sel[1])
+            if size_columns is not None:  # sel[8] = (output sizes, slot bytes)
+                pack = self._pack_masks(pack, size_columns, mask_logits, tuple(images.shape[-2:]), *sel[8])
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                 init_reference, inter_references, mask_logits, pack)
 
@@ -950,27 +963,52 @@ class DeformableDETRSegmVL(nn.Module):
         return torch.stack(packs)
 
     def forward_packed(self, batched_inputs):
-        """Detections as ONE device tensor [B, topk, 13] (the 9 columns of `_select_device` + padded image height / width and
-        requested output height / width), without touching the host: the multi-GPU path hands it straight to one NCCL
-        gather on the compute stream (ape_b200.parallel.gather_packed) and only the destination rank copies to the host.
-        Boxes only (instance masks travel separately).  The selection path (candidate list vs class-wise NMS) is the one
-        the last host-synchronised forward found appropriate; the packed rows carry the candidate count so the receiver can
-        tell if that choice was wrong for an image (count > static_inference_cap on the candidate-list path)."""
-        assert not (self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)), "forward_packed: boxes only"
-        box_cls, box_pred, image_sizes, pack = self.forward(batched_inputs, do_postprocess="packed")
+        """Detections as ONE device tensor, without touching the host: the multi-GPU path hands it straight to one NCCL gather
+        on the compute stream (ape_b200.parallel.gather_packed) and only the destination rank copies to the host.
+        Boxes only: fp32 [B, topk, 13], the 9 columns of `_select_device` + image height / width and requested output height /
+        width.  With `instance_on and test_mask_on`: uint8 [B, topk, 60 + mask_slot_bytes], those 13 columns as bytes, then
+        each kept mask as a COCO run-length code in a slot of fixed size (`ops.mask_pack`); `parallel.unpack_packed` turns
+        either into what `model(inputs)` returns (with `mask_format = "rle"` for masks).  The selection path (candidate list
+        vs class-wise NMS) is the one the last host-synchronised forward found appropriate; the packed rows carry the candidate
+        count so the receiver can tell if that choice was wrong for an image (count > static_inference_cap on the
+        candidate-list path)."""
+        assert not (self.semantic_on or self.panoptic_on), "forward_packed: boxes, or boxes and instance masks"
+        masks = self.instance_on and self.test_mask_on
+        box_cls, box_pred, image_sizes, pack, mask_pred, padded_hw = self.forward(batched_inputs, do_postprocess="packed")
+        if pack is not None and masks:  # the mask stage ran in the graph; its output buffer is rewritten by the next replay
+            return pack.clone()
         if pack is None:  # no graph for this call (fp32 mode, phrase prompts ...): the same selection, eagerly
             ent = self.eval_dataset_entity
             det_cls = self._detector_box_cls(box_cls) if (self.instance_on and not (ent and "thing" not in ent)) else box_cls
             pack = self._select_device(det_cls, box_pred, image_sizes, bool(getattr(self, "_static_overflowed", False)))
-        rows = tuple((float(h), float(w), float(inp.get("height", h)), float(inp.get("width", w)))
-                     for (h, w), inp in zip(image_sizes, batched_inputs))
-        cache = self.__dict__.setdefault("_packed_extra", {})  # the four size columns per geometry: no pageable upload per call
-        extra = cache.get((rows, str(pack.device)))
+        cols = self._size_columns(batched_inputs, image_sizes, pack.device)
+        if masks:
+            return self._pack_masks(pack, cols, mask_pred, padded_hw, self._output_sizes(batched_inputs, image_sizes),
+                                    int(self.mask_slot_bytes))
+        return torch.cat([pack, cols[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
+
+    @staticmethod
+    def _output_sizes(batched_inputs, image_sizes):
+        return tuple((int(inp.get("height", h)), int(inp.get("width", w))) for (h, w), inp in zip(image_sizes, batched_inputs))
+
+    def _size_columns(self, batched_inputs, image_sizes, device=None):
+        """[B, 4] fp32 (image height, width, output height, width) on the device, cached per geometry: no pageable upload per call."""
+        device = self.device if device is None else device
+        rows = tuple((float(h), float(w), float(oh), float(ow))
+                     for (h, w), (oh, ow) in zip(image_sizes, self._output_sizes(batched_inputs, image_sizes)))
+        cache = self.__dict__.setdefault("_packed_extra", {})
+        extra = cache.get((rows, str(device)))
         if extra is None:
             if len(cache) > 64:
                 cache.clear()
-            extra = cache[(rows, str(pack.device))] = torch.tensor(rows, dtype=torch.float32).to(pack.device)
-        return torch.cat([pack, extra[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
+            extra = cache[(rows, str(device))] = torch.tensor(rows, dtype=torch.float32).to(device)
+        return extra
+
+    @staticmethod
+    def _pack_masks(pack, size_columns, mask_logits, padded_hw, out_sizes, slot):
+        """Selection rows [B, topk, 9] + size columns -> uint8 [B, topk, 60 + slot] with the kept masks' run-length codes."""
+        rows = torch.cat([pack, size_columns[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
+        return ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, slot)
 
     def inference(self, box_cls, box_pred, image_sizes):
         """:759-810 + fast_rcnn.py:40-95.  CUDA: the static-shape selection above (device results; bounded memory for any

@@ -853,6 +853,38 @@ def paste_masks_rle(masks, boxes, image_shape, threshold=0.5):
     return out
 
 
+MASK_PACK_HEAD = 60  # bytes before a mask slot: 13 fp32 selection columns, int32 kind, int32 length
+MASK_SLOT_EMPTY, MASK_SLOT_CHARS, MASK_SLOT_BITS = 0, 1, 2
+
+
+def mask_pack(mask_logits, rows, out_sizes, padded_hw, slot, mask_size=128):
+    """The kept masks of the packed selection rows as COCO run-length codes in fixed-size slots (ape_mask_pack), with no host
+    synchronisation: mask_logits [B,Q,h,w] (CUDA fp32 / fp16 / bf16), rows fp32 [B,topk,13] (`forward_packed`'s columns),
+    out_sizes [(H, W)] per image (the rows' output sizes, as host ints) -> uint8 [B, topk, MASK_PACK_HEAD + slot]: each slot's
+    13 columns as bytes, int32 kind (MASK_SLOT_*) and length, then the "counts" characters or, for a code longer than the slot,
+    the mask_size^2 mask as bits (little-endian bit order).  Slots past the kept count and boxes that are empty after the
+    rescale and clip hold no mask."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 4 and mask_logits.is_contiguous(), "mask_pack: contiguous CUDA logits [B,Q,h,w]")
+    B, Q, h, w = (int(v) for v in mask_logits.shape)
+    _require(rows.dtype == torch.float32 and rows.is_contiguous() and rows.dim() == 3 and rows.shape[0] == B and rows.shape[2] == 13
+             and rows.device == mask_logits.device, "mask_pack: rows must be contiguous fp32 [B,topk,13] on the logits' device")
+    _require(len(out_sizes) == B, "mask_pack: one output size per image")
+    topk, slot, S = int(rows.shape[1]), int(slot), int(mask_size)
+    out = torch.empty((B, topk, MASK_PACK_HEAD + slot), dtype=torch.uint8, device=mask_logits.device)
+    if B == 0 or topk == 0:
+        return out
+    Hp, Wp = int(padded_hw[0]), int(padded_hw[1])
+    hw = (ctypes.c_int * (2 * B))(*[int(v) for s in out_sizes for v in s])
+    max_w = max(int(s[1]) for s in out_sizes)
+    ws = torch.empty((max(int(_lib.lib.ape_mask_pack_workspace_bytes(topk, Hp, Wp, max_w, S, slot)), 1),), dtype=torch.uint8,
+                     device=mask_logits.device)
+    with torch.cuda.device(mask_logits.device), _timed(("mask_pack", B, topk, Hp, Wp, slot)):
+        rc = _lib.lib.ape_mask_pack(mask_logits.data_ptr(), rows.data_ptr(), hw, ws.data_ptr(), out.data_ptr(), B, topk, Q, h, w, Hp,
+                                    Wp, S, slot, _lib.dtype_code(mask_logits.dtype), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_mask_pack")
+    return out
+
+
 SEMSEG_BAND_BYTES = 256 << 20  # bound of the resampled-operand workspace of semseg_label
 
 

@@ -63,25 +63,80 @@ def gather_detections(instances: List[Instances], max_det: int, device, dst: int
 
 # ---- device-side path: no host round trip before the collective ---------------------------------------------------
 def unpack_packed(packed: torch.Tensor) -> List[dict]:
-    """Rows of `DeformableDETRSegmVL.forward_packed` ([images, topk, 13], any device) -> the reference's output list
-    [{"instances": Instances}] on the host: the kept detections rescaled to the requested output size, clipped, empty boxes
-    dropped (detectron2 detector_postprocess).  One device->host copy for everything."""
+    """Rows of `DeformableDETRSegmVL.forward_packed` (any device) -> the reference's output list [{"instances": Instances}] on
+    the host: the kept detections rescaled to the requested output size, clipped, empty boxes dropped (detectron2
+    detector_postprocess).  One device->host copy for everything.
+    fp32 [images, topk, 13]: boxes only.  uint8 [images, topk, 60 + slot] (instance masks): the same 13 columns as bytes, and
+    `pred_masks_rle` = [{"size": [H, W], "counts": bytes}] per kept detection, as `model(inputs)` returns with
+    `mask_format = "rle"`.  A slot that holds its mask as bits is pasted and encoded here (`ops.paste_masks_rle`)."""
+    if packed.dtype == torch.uint8:
+        return _unpack_packed_masks(packed)
     host = packed.to("cpu")
+    return [_unpack_rows(p)[0] for p in host]
+
+
+def _unpack_rows(p: torch.Tensor):
+    """One image's [topk, 13] rows -> ({"instances", "num_candidates"}, indices of the kept slots)."""
+    nk = int(p[0, 8])
+    h, w, oh, ow = (float(v) for v in p[0, 9:13])
+    r = p[:nk]
+    b = r[:, :4].clone()
+    if h > 0 and w > 0:
+        b[:, 0::2] *= ow / w
+        b[:, 1::2] *= oh / h
+    b = torch.stack((b[:, 0].clamp(min=0, max=ow), b[:, 1].clamp(min=0, max=oh), b[:, 2].clamp(min=0, max=ow),
+                     b[:, 3].clamp(min=0, max=oh)), dim=-1)
+    keep = ((b[:, 2] - b[:, 0]) > 0) & ((b[:, 3] - b[:, 1]) > 0)
+    return ({"instances": Instances((int(oh), int(ow)), pred_boxes=Boxes(b[keep]), scores=r[keep, 4].clone(),
+                                    pred_classes=r[keep, 5].to(torch.int64), query_index=r[keep, 6].to(torch.int64)),
+             "num_candidates": int(p[0, 7])}, keep.nonzero()[:, 0].tolist())
+
+
+MASK_PACK_HEAD = 60  # = ops.MASK_PACK_HEAD: 13 fp32 columns, int32 slot kind, int32 slot length
+MASK_SLOT_CHARS, MASK_SLOT_BITS = 1, 2  # = ops.MASK_SLOT_*
+
+
+def unpack_mask_bits(slot_bytes) -> torch.Tensor:
+    """The bits form of mask slots (pixel y * S + x at byte >> 3, bit & 7): [..., S*S/8] bytes -> bool [..., S, S]."""
+    import numpy as np
+
+    a = np.frombuffer(bytes(slot_bytes), dtype=np.uint8) if isinstance(slot_bytes, (bytes, bytearray)) else np.asarray(slot_bytes)
+    S = int(round((8 * a.shape[-1]) ** 0.5))
+    bits = np.unpackbits(a, axis=-1, bitorder="little")[..., : S * S]
+    return torch.from_numpy(bits.reshape(a.shape[:-1] + (S, S)).astype(bool))
+
+
+def _unpack_packed_masks(packed: torch.Tensor) -> List[dict]:
+    host = packed.to("cpu")
+    rows = host[..., :52].contiguous().view(torch.float32)                     # [images, topk, 13]
+    words = host[..., 52:MASK_PACK_HEAD].contiguous().view(torch.int32).numpy()  # [images, topk, 2]: kind, length
+    raw = host.numpy()
     out = []
-    for p in host:
-        nk = int(p[0, 8])
-        h, w, oh, ow = (float(v) for v in p[0, 9:13])
-        r = p[:nk]
-        b = r[:, :4].clone()
-        if h > 0 and w > 0:
-            b[:, 0::2] *= ow / w
-            b[:, 1::2] *= oh / h
-        b = torch.stack((b[:, 0].clamp(min=0, max=ow), b[:, 1].clamp(min=0, max=oh), b[:, 2].clamp(min=0, max=ow),
-                         b[:, 3].clamp(min=0, max=oh)), dim=-1)
-        keep = ((b[:, 2] - b[:, 0]) > 0) & ((b[:, 3] - b[:, 1]) > 0)
-        out.append({"instances": Instances((int(oh), int(ow)), pred_boxes=Boxes(b[keep]), scores=r[keep, 4].clone(),
-                                           pred_classes=r[keep, 5].to(torch.int64), query_index=r[keep, 6].to(torch.int64)),
-                    "num_candidates": int(p[0, 7])})
+    for i in range(host.shape[0]):
+        res, kept = _unpack_rows(rows[i])
+        inst = res["instances"]
+        size = [inst.image_size[0], inst.image_size[1]]
+        rles, bits = [], []
+        for j, k in enumerate(kept):
+            kind, n = int(words[i, k, 0]), int(words[i, k, 1])
+            if kind == MASK_SLOT_CHARS:
+                rles.append({"size": size, "counts": raw[i, k, MASK_PACK_HEAD:MASK_PACK_HEAD + n].tobytes()})
+                continue
+            if kind != MASK_SLOT_BITS:
+                raise ValueError(f"unpack_packed: image {i} slot {k} is kept but holds no mask (kind {kind})")
+            rles.append(None)
+            bits.append((j, k, n))
+        if bits:  # masks that travelled as bits: pasted and encoded with the kernels `model(inputs)` uses
+            from . import ops
+
+            n = bits[0][2]
+            masks = unpack_mask_bits(raw[i, [k for _, k, _ in bits], MASK_PACK_HEAD:MASK_PACK_HEAD + n])
+            dev = packed.device if packed.is_cuda else torch.device("cuda")
+            boxes = inst.pred_boxes.tensor[[j for j, _, _ in bits]]
+            for (j, _, _), rle in zip(bits, ops.paste_masks_rle(masks.to(dev), boxes.to(dev), inst.image_size, 0.5)):
+                rles[j] = rle
+        inst.pred_masks_rle = rles
+        out.append(res)
     return out
 
 

@@ -442,6 +442,25 @@ int ape_mask_paste(const uint8_t *masks, const float *boxes, uint8_t *out, int N
 int ape_mask_paste_rle(const uint8_t *masks, const float *boxes, int N, int S, int img_h, int img_w, float threshold,
                        int *col_count, const int64_t *col_offset, int *positions, void *stream);
 int ape_rle_to_string(const uint32_t *counts, int m, char *out);
+/*
+ * The kept instance masks of the packed selection rows as COCO run-length codes in fixed-size slots, with no count read back
+ * by the host: CUDA-graph capturable, and the result is one fixed-shape tensor for one collective.  Replaces, per image, the
+ * reference's paste_masks_in_image (detectron2 detector_postprocess), then mask_util.encode / instances_to_coco_json (the
+ * evaluator's encoding of every pasted mask), then the pickled comm.gather of those codes (lvis_evaluation.py:103-104).
+ *   ape_mask_pack  logits [B,Q,h,w] dtype; rows [B,topk,13] fp32 as DeformableDETRSegmVL.forward_packed writes them (x1, y1,
+ *                  x2, y2 in image pixels, score, class, query index, candidates, kept nk, image h, w, output h, w); out_hw
+ *                  HOST int32 [B,2] = the output sizes (the same as the rows' last two columns).  For each slot < nk whose
+ *                  box is non-empty after detector_postprocess's rescale and clip: ape_mask_crop over the padded size Hp x Wp,
+ *                  then the paste into the rescaled box at threshold 0.5 encoded as cocoapi's rleToString "counts".
+ *                  out [B,topk,60+slot] bytes per slot: the 13 fp32 columns; int32 kind (0 no mask, 1 counts characters,
+ *                  2 the S x S mask as bits: pixel y*S+x at byte >> 3, bit & 7) and int32 length; the slot, zero after the length.
+ *                  A code longer than slot bytes is stored as bits.  slot: a multiple of 4 of at least S*S/8.
+ *                  workspace: ape_mask_pack_workspace_bytes(topk, Hp, Wp, max output width, S, slot), 256-byte aligned;
+ *                  rows and out 4-byte aligned.
+ */
+int64_t ape_mask_pack_workspace_bytes(int topk, int Hp, int Wp, int max_w, int S, int slot);
+int ape_mask_pack(const void *logits, const float *rows, const int *out_hw, void *workspace, uint8_t *out, int B, int topk, int Q,
+                  int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream);
 
 /*
  * Semantic label maps without the [N,H,W] class-score maps.  Replaces, for one image, the semantic tail of
