@@ -156,6 +156,18 @@ def _declare(lib):
     lib.ape_gemm_tn_argmax.argtypes = [_vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp]
     lib.ape_semseg_keys_decode.restype = _i
     lib.ape_semseg_keys_decode.argtypes = [_vp, _i64, _vp, _vp, _vp]
+    lib.ape_label_rle_workspace_bytes.restype = _i64
+    lib.ape_label_rle_workspace_bytes.argtypes = [_i, _i, _i64]
+    lib.ape_label_rle_out_bytes.restype = _i64
+    lib.ape_label_rle_out_bytes.argtypes = [_i, _i]
+    lib.ape_label_rle_sizes.restype = _i
+    lib.ape_label_rle_sizes.argtypes = [_vp, _i, _i, _vp, _vp, _vp]
+    lib.ape_label_rle.restype = _i
+    lib.ape_label_rle.argtypes = [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]
+    lib.ape_label_rle_pack_workspace_bytes.restype = _i64
+    lib.ape_label_rle_pack_workspace_bytes.argtypes = [_i, _i, _i]
+    lib.ape_label_rle_pack.restype = _i
+    lib.ape_label_rle_pack.argtypes = [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]
     lib.ape_panoptic_winners.restype = _i
     lib.ape_panoptic_winners.argtypes = [_vp] * 5 + [_i] * 9 + [ctypes.c_float, _i, _vp]
 
@@ -221,6 +233,12 @@ EXPORTS = (
     "ape_semseg_keys_init",
     "ape_gemm_tn_argmax",
     "ape_semseg_keys_decode",
+    "ape_label_rle_workspace_bytes",
+    "ape_label_rle_out_bytes",
+    "ape_label_rle_sizes",
+    "ape_label_rle",
+    "ape_label_rle_pack_workspace_bytes",
+    "ape_label_rle_pack",
     "ape_panoptic_winners",
 )
 

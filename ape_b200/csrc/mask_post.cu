@@ -21,6 +21,7 @@
 //                          sampling grid exists only in registers.
 // sigmoid(x) > 0.5 is evaluated as x > 0 (identical except for |x| < 6e-8, where fp32 sigmoid rounds to 0.5 exactly).
 #include "common.cuh"
+#include "rle.cuh"
 
 namespace ape {
 namespace {
@@ -253,28 +254,6 @@ __global__ void __launch_bounds__(256) mask_pack_prep_kernel(const float *__rest
   live[k] = ok;
 }
 
-// block-wide exclusive sum over 256 threads; returns this thread's offset, *sum the total.  s_warp holds 8 ints.
-__device__ __forceinline__ int block_excl_scan_256(int v, int *s_warp, int *sum) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int incl = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= d) incl += t;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  int before = 0, total = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    before += i < warp ? s_warp[i] : 0;
-    total += s_warp[i];
-  }
-  __syncthreads();  // s_warp is reused by the next call
-  *sum = total;
-  return before + incl - v;
-}
-
 // One CTA per slot: exclusive scan of the slot's column counts -> col_offset (the slot's positions start at n * slot), the
 // number of boundaries, and chars[n] = whether they fit: m boundaries make m + 1 counts of at least one character each, so a slot
 // with m >= slot boundaries goes straight to bits and the positions workspace stays at slot int32 per slot.
@@ -301,21 +280,6 @@ __global__ void __launch_bounds__(256) mask_pack_scan_kernel(const int *__restri
     total[n] = (int)min(base, 0x7fffffffLL);
     chars[n] = base < slot;
   }
-}
-
-// cocoapi rleToString of one count (see ape_rle_to_string): number of characters, and the characters when out != NULL
-__device__ __forceinline__ int rle_chars(long long x, uint8_t *out, int room) {
-  int n = 0;
-  bool more = true;
-  while (more) {
-    int c = (int)(x & 0x1f);
-    x >>= 5;
-    more = (c & 0x10) ? x != -1 : x != 0;
-    if (more) c |= 0x20;
-    if (out && n < room) out[n] = (uint8_t)(c + 48);
-    ++n;
-  }
-  return n;
 }
 
 // One CTA per slot: the row, the slot word and the slot.  Counts from the boundary positions p (c_i = p_i - p_{i-1}, with

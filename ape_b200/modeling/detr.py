@@ -294,6 +294,10 @@ class DeformableDETRSegmVL(nn.Module):
         # first argmax over classes of that map, all SemSegEvaluator keeps) and `sem_seg_score` fp32 [H, W] (its value).  On CUDA
         # with a 16-bit engine_dtype the map is never formed (csrc/semseg.cu: 5 GB per image at 1203 classes and 1024^2)
         self.sem_seg_format = "maps"
+        # "rle" adds `sem_seg_rle` to what "label" returns: one cocoapi run-length code per label present (ops.label_map_rle), what
+        # SemSegEvaluator.process encodes the map into.  `sem_seg_slot_bytes`: the semantic slot per image of `forward_packed`
+        # (codes, or the map as uint16 when they do not fit: the default holds any map up to 1024 x 1024 exactly); a multiple of 4
+        self.sem_seg_slot_bytes = 1 << 21
         self.semantic_post_nms = semantic_post_nms
         self.panoptic_post_nms = panoptic_post_nms
         self.panoptic_configs = panoptic_configs if panoptic_configs is not None else {
@@ -515,17 +519,20 @@ class DeformableDETRSegmVL(nn.Module):
                 sel, const = None, (geo, prompt)
                 # forward_packed with instance masks: the mask stage (csrc/mask_post.cu, ape_mask_pack) follows the selection in
                 # the graph; the output sizes and the slot size join the key
-                packed_masks = do_postprocess == "packed" and self.instance_on and self.test_mask_on and \
-                    not (self.semantic_on or self.panoptic_on)
-                if do_postprocess in (True, "packed") and (not need_masks or packed_masks) and self.static_inference_cap > 0 and \
-                        self.test_topk_per_image >= 0 and self.num_queries <= 1024:
+                # with semantic_on the semantic stage (ape_label_rle_pack) follows too, and its configuration joins the key
+                packed = do_postprocess == "packed" and not self.panoptic_on
+                packed_masks = packed and self.instance_on and self.test_mask_on
+                packed_sem = self._packed_semantic_config() if packed and self.semantic_on else None
+                if do_postprocess in (True, "packed") and (not need_masks or packed_masks or packed_sem) and \
+                        self.static_inference_cap > 0 and self.test_topk_per_image >= 0 and self.num_queries <= 1024:
                     ent = self.eval_dataset_entity
                     sel = (tuple(image_sizes), bool(getattr(self, "_static_overflowed", False)), float(self.test_score_thresh),
                            float(self.test_nms_thresh), int(self.test_topk_per_image), int(self.static_inference_cap),
                            self.eval_dataset_id, bool(self.instance_on and not (ent and "thing" not in ent)))
                     const = (geo, prompt, sel)
-                    if packed_masks:
-                        sel += ((self._output_sizes(batched_inputs, image_sizes), int(self.mask_slot_bytes)),)
+                    if packed_masks or packed_sem:
+                        sel += ((self._output_sizes(batched_inputs, image_sizes), int(self.mask_slot_bytes) if packed_masks else None,
+                                 packed_sem),)
                         const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
@@ -681,8 +688,9 @@ class DeformableDETRSegmVL(nn.Module):
         if sel is not None:  # (image sizes, class-wise path?, thresholds ..., instance branch on?) — see forward()
             det_cls = self._detector_box_cls(box_cls) if sel[7] else box_cls
             pack = self._select_device(det_cls, box_pred, sel[0], sel[1])
-            if size_columns is not None:  # sel[8] = (output sizes, slot bytes)
-                pack = self._pack_masks(pack, size_columns, mask_logits, tuple(images.shape[-2:]), *sel[8])
+            if size_columns is not None:  # sel[8] = (output sizes, mask slot bytes or None, semantic configuration or None)
+                pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sel[0], tuple(images.shape[-2:]),
+                                       sel[1], *sel[8])
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                 init_reference, inter_references, mask_logits, pack)
 
@@ -798,8 +806,17 @@ class DeformableDETRSegmVL(nn.Module):
         detection NMS, softmax(sigmoid / 0.06) over classes, times the sigmoid masks at padded-image resolution.  One dict per
         image: {"sem_seg"} or, with sem_seg_format "label", {"sem_seg_label", "sem_seg_score"} (see __init__)."""
         fmt = getattr(self, "sem_seg_format", "maps")
-        if fmt not in ("maps", "label"):
-            raise ValueError(f"ape_b200: sem_seg_format must be 'maps' or 'label' (got {fmt!r})")
+        if fmt not in ("maps", "label", "rle"):
+            raise ValueError(f"ape_b200: sem_seg_format must be 'maps', 'label' or 'rle' (got {fmt!r})")
+        if fmt == "rle":
+            self.sem_seg_format = "label"
+            try:
+                outs = self._semantic(box_cls, box_pred, mask_pred, image_sizes, padded_hw, batched_inputs, shared_keep)
+            finally:
+                self.sem_seg_format = "rle"
+            for o in outs:
+                o["sem_seg_rle"] = ops.label_map_rle(o["sem_seg_label"])
+            return outs
         name = self.dataset_names[self.eval_dataset_id] if self.dataset_names else None
         things, stuff, entity = self.dataset_stuff.get(name, (None, None, "thing"))
         sem_cls = get_stuff_score(box_cls, things or [], stuff or [], entity)
@@ -971,20 +988,29 @@ class DeformableDETRSegmVL(nn.Module):
         either into what `model(inputs)` returns (with `mask_format = "rle"` for masks).  The selection path (candidate list
         vs class-wise NMS) is the one the last host-synchronised forward found appropriate; the packed rows carry the candidate
         count so the receiver can tell if that choice was wrong for an image (count > static_inference_cap on the
-        candidate-list path)."""
-        assert not (self.semantic_on or self.panoptic_on), "forward_packed: boxes, or boxes and instance masks"
+        candidate-list path).
+        With `semantic_on`: uint8 [B, 32 + topk * R + sem_seg_slot_bytes] per image, a header of 8 int32 (topk, R, semantic slot
+        kind, its bytes used, output height, width, labels present, 0), then that image's rows of either form above (R = 52, or 60 +
+        mask_slot_bytes), then its semantic label map as one run-length code per label (`ops.semseg_pack`): `unpack_packed` adds
+        `sem_seg_rle` as `model(inputs)` returns it with `sem_seg_format = "rle"`.  Needs a 16-bit engine_dtype on CUDA."""
+        assert not self.panoptic_on, "forward_packed: boxes, instance masks and semantic label maps; panoptic is not packed"
         masks = self.instance_on and self.test_mask_on
+        sem = self._packed_semantic_config() if self.semantic_on else None
+        if sem is not None and not (self.engine_dtype in (torch.float16, torch.bfloat16) and self.device.type == "cuda"):
+            raise ValueError("ape_b200: forward_packed with semantic_on needs a CUDA model with a 16-bit engine_dtype (the semantic "
+                             "label map is built by ops.semseg_label); use model(inputs) with sem_seg_format = 'rle' instead")
         box_cls, box_pred, image_sizes, pack, mask_pred, padded_hw = self.forward(batched_inputs, do_postprocess="packed")
-        if pack is not None and masks:  # the mask stage ran in the graph; its output buffer is rewritten by the next replay
+        if pack is not None and (masks or sem is not None):  # the stages ran in the graph; their buffer is rewritten by the next replay
             return pack.clone()
         if pack is None:  # no graph for this call (fp32 mode, phrase prompts ...): the same selection, eagerly
             ent = self.eval_dataset_entity
             det_cls = self._detector_box_cls(box_cls) if (self.instance_on and not (ent and "thing" not in ent)) else box_cls
             pack = self._select_device(det_cls, box_pred, image_sizes, bool(getattr(self, "_static_overflowed", False)))
         cols = self._size_columns(batched_inputs, image_sizes, pack.device)
-        if masks:
-            return self._pack_masks(pack, cols, mask_pred, padded_hw, self._output_sizes(batched_inputs, image_sizes),
-                                    int(self.mask_slot_bytes))
+        if masks or sem is not None:
+            return self._pack_rows(pack, cols, box_cls, box_pred, mask_pred, tuple(image_sizes), padded_hw,
+                                   bool(getattr(self, "_static_overflowed", False)), self._output_sizes(batched_inputs, image_sizes),
+                                   int(self.mask_slot_bytes) if masks else None, sem)
         return torch.cat([pack, cols[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
 
     @staticmethod
@@ -1004,11 +1030,76 @@ class DeformableDETRSegmVL(nn.Module):
             extra = cache[(rows, str(device))] = torch.tensor(rows, dtype=torch.float32).to(device)
         return extra
 
-    @staticmethod
-    def _pack_masks(pack, size_columns, mask_logits, padded_hw, out_sizes, slot):
-        """Selection rows [B, topk, 9] + size columns -> uint8 [B, topk, 60 + slot] with the kept masks' run-length codes."""
+    def _packed_semantic_config(self):
+        """Everything the packed semantic stage reads from the model, as a graph-key tuple: (slot bytes, branch on for the
+        evaluated dataset, semantic_post_nms, class-0 constant or None, thing classes, stuff classes, entity)."""
+        ent = self.eval_dataset_entity
+        name = self.dataset_names[self.eval_dataset_id] if self.dataset_names else None
+        things, stuff, entity = self.dataset_stuff.get(name, (None, None, "thing"))
+        class0 = None  # as _semantic (:655-664)
+        if entity == "stuff" and stuff and stuff[0] == "things" and self.stuff_prob_thing > 0:
+            class0 = math.log(self.stuff_prob_thing / (1 - self.stuff_prob_thing))
+        slot = int(self.sem_seg_slot_bytes)
+        if slot < 16 or slot % 4:
+            raise ValueError(f"ape_b200: sem_seg_slot_bytes must be a multiple of 4 of at least 16 (got {slot})")
+        return (slot, not (ent and "stuff" not in ent), bool(self.semantic_post_nms), class0, tuple(things or ()), tuple(stuff or ()),
+                entity)
+
+    def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes, mask_slot,
+                   sem):
+        """Selection rows [B, topk, 9] + size columns -> what forward_packed returns: fp32 [B, topk, 13] rows, or uint8
+        [B, topk, 60 + mask_slot] with the kept masks' run-length codes (mask_slot not None); with a semantic configuration
+        (`_packed_semantic_config`) each image's header, those rows as bytes and its semantic slot.  No host synchronisation."""
         rows = torch.cat([pack, size_columns[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
-        return ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, slot)
+        if mask_slot is not None:
+            rows = ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, mask_slot)
+        if sem is None:
+            return rows
+        slot, on, post_nms, class0, things, stuff, entity = sem
+        B, topk = rows.shape[0], rows.shape[1]
+        det = rows.contiguous().view(torch.uint8).reshape(B, -1)
+        R = det.shape[1] // max(topk, 1)
+        out = torch.empty((B, ops.SEM_PACK_HEAD + det.shape[1] + slot), dtype=torch.uint8, device=rows.device)
+        out[:, ops.SEM_PACK_HEAD:ops.SEM_PACK_HEAD + det.shape[1]] = det
+        slots = out[:, ops.SEM_PACK_HEAD + det.shape[1]:]
+        info = torch.zeros((B, 3), dtype=torch.int32, device=rows.device)  # kind, bytes used, labels present
+        if on:
+            sem_cls = get_stuff_score(box_cls, list(things), list(stuff), entity)
+            if post_nms and self.instance_on and not (self.eval_dataset_entity and "thing" not in self.eval_dataset_entity) and \
+                    self._detector_box_cls(box_cls) is box_cls and sem_cls.shape == box_cls.shape:
+                keep = pack  # _semantic reuses the instance branch's kept queries in this case
+            elif post_nms:
+                keep = self._select_device(sem_cls, box_pred, list(image_sizes), classwise)
+            else:
+                keep = None
+            labels = [self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw, image_sizes[b],
+                                                  out_sizes[b], class0) for b in range(B)]
+            ops.semseg_pack(labels, sem_cls.shape[-1], slots, info)
+        else:
+            slots.zero_()
+        hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
+        hdr[:, 0], hdr[:, 1] = topk, R
+        hdr[:, 2:4] = info[:, 0:2]
+        hdr[:, 4:6] = size_columns[:, 2:4].to(torch.int32)
+        hdr[:, 6] = info[:, 2]
+        out[:, :ops.SEM_PACK_HEAD] = hdr.view(torch.uint8)
+        return out
+
+    def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0):
+        """`_semantic`'s label map of one image with K = topk queries whatever the kept count (no host synchronisation): the
+        rows of `keep` ([topk, 9] selection rows, None = every query) at or past the kept count get zero class weights, so the
+        class GEMM adds exact zeros for them."""
+        Q = sem_cls.shape[0]
+        if keep is None:
+            qi, live = torch.arange(Q, device=sem_cls.device), None
+        else:
+            qi = keep[:, 6].to(torch.int64).clamp(0, Q - 1)
+            live = torch.arange(keep.shape[0], device=keep.device) < keep[:, 8].to(torch.int64)
+        cls = F.softmax(sem_cls[qi].float().sigmoid() / 0.06, dim=-1)
+        if live is not None:
+            cls = torch.where(live[:, None], cls, cls.new_zeros(()))
+        label, _ = ops.semseg_label(mask_logits.contiguous(), qi, cls.to(self.engine_dtype), padded_hw, size, out_hw, class0)
+        return label
 
     def inference(self, box_cls, box_pred, image_sizes):
         """:759-810 + fast_rcnn.py:40-95.  CUDA: the static-shape selection above (device results; bounded memory for any

@@ -948,6 +948,102 @@ def semseg_label(mask_logits, query_index, cls, padded_hw, img_hw, out_hw, class
     return label, score
 
 
+def _label_rle_table(raw, P, H, W):
+    """A codes body (P x (int32 label, character offset, length), then the characters) -> the list label_map_rle returns."""
+    import numpy as np
+
+    raw = np.asarray(raw, dtype=np.uint8)
+    table = raw[:12 * P].view(np.int32).reshape(P, 3)
+    chars = raw[12 * P:]
+    return [{"label": int(c), "segmentation": {"size": [H, W], "counts": chars[o:o + n].tobytes()}} for c, o, n in table.tolist()]
+
+
+def label_map_rle(label):
+    """`[{"label": c, "segmentation": mask_util.encode(np.asfortranarray((label == c).astype(np.uint8)))} for c in np.unique(label)]`
+    (detectron2's encode_json_sem_seg without the per-label masks, ape_label_rle): label int64 [H, W] on a CUDA device, values in
+    [0, 65535] -> one cocoapi run-length code per label present, in ascending label order.  One synchronising read of the map's
+    sizes (labels present, boundaries), then the codes are built on the device and copied to the host in one copy."""
+    _require(label.is_cuda and label.dim() == 2 and label.dtype == torch.int64, "label_map_rle: CUDA int64 label map [H, W]")
+    label = label.contiguous()
+    H, W = int(label.shape[0]), int(label.shape[1])
+    dev = label.device
+    stream = _lib.current_stream_ptr()
+    with torch.cuda.device(dev), _timed(("label_rle", H, W)):
+        ws = torch.empty((int(_lib.lib.ape_label_rle_workspace_bytes(W, 0, 0)),), dtype=torch.uint8, device=dev)
+        sizes = torch.empty((3,), dtype=torch.int32, device=dev)
+        _lib.check(_lib.lib.ape_label_rle_sizes(label.data_ptr(), H, W, ws.data_ptr(), sizes.data_ptr(), stream), "ape_label_rle_sizes")
+        host = sizes.cpu()  # P, m, labels out of range
+        P, m = int(host[0]), int(host[1])
+        hs = (ctypes.c_int * 3)(*[int(v) for v in host.tolist()])
+        ws = torch.empty((int(_lib.lib.ape_label_rle_workspace_bytes(W, max(P, 0), 2 * max(m, 0) + 1)),), dtype=torch.uint8, device=dev)
+        out = torch.empty((max(int(_lib.lib.ape_label_rle_out_bytes(max(P, 0), max(m, 0))), 4),), dtype=torch.uint8, device=dev)
+        info = torch.empty((3,), dtype=torch.int32, device=dev)
+        _lib.check(_lib.lib.ape_label_rle(label.data_ptr(), H, W, hs, ws.data_ptr(), out.data_ptr(), info.data_ptr(), stream),
+                   "ape_label_rle")
+        n = int(info[1])
+        raw = out[:n].cpu().numpy()
+    return _label_rle_table(raw, P, H, W)
+
+
+def label_map_from_rle(sem_seg_rle):
+    """The label map back from label_map_rle's list (host, numpy): int64 [H, W], each pixel the label whose code covers it."""
+    import numpy as np
+
+    H, W = sem_seg_rle[0]["segmentation"]["size"]
+    flat = np.zeros((H * W,), dtype=np.int64)  # column-major pixel order, as the codes
+    for entry in sem_seg_rle:
+        s = entry["segmentation"]["counts"]
+        counts, p = [], 0
+        while p < len(s):  # cocoapi rleFrString
+            x, k, more = 0, 0, True
+            while more:
+                c = s[p] - 48
+                x |= (c & 0x1F) << (5 * k)
+                more = bool(c & 0x20)
+                p += 1
+                k += 1
+                if not more and (c & 0x10):
+                    x |= -1 << (5 * k)
+            if len(counts) > 2:
+                x += counts[-2]
+            counts.append(x)
+        ends = np.cumsum(counts)
+        for lo, hi in zip(ends[0::2], ends[1::2]):  # odd runs are the label's pixels
+            flat[lo:hi] = entry["label"]
+    return flat.reshape(W, H).T.copy()
+
+
+SEM_PACK_HEAD = 32  # bytes before an image's detections in forward_packed's semantic form: 8 int32 header fields
+SEM_SLOT_NONE, SEM_SLOT_CODES, SEM_SLOT_MAP, SEM_SLOT_OVER = 0, 1, 2, 3
+
+
+def semseg_pack(labels, num_labels, slots, info):
+    """One semantic slot per image with no host synchronisation (ape_label_rle_pack): labels [int64 [H_b, W_b] CUDA] with values
+    in [0, num_labels); slots uint8 [B, slot] (rows 4-byte aligned, each row contiguous); info int32 [B, 3] <- kind
+    (SEM_SLOT_*), bytes used, labels present.  A slot holds the codes of label_map_rle (a table of P x (int32 label, int32
+    character offset, int32 length), then the characters) when they fit, else the map as uint16 [H, W] when that fits, else
+    nothing."""
+    B = len(labels)
+    _require(slots.dim() == 2 and slots.shape[0] == B and slots.dtype == torch.uint8 and slots.stride(1) == 1,
+             "semseg_pack: slots must be uint8 [B, slot] with contiguous rows")
+    _require(info.dtype == torch.int32 and info.is_contiguous() and tuple(info.shape) == (B, 3), "semseg_pack: info int32 [B, 3]")
+    if B == 0:
+        return
+    dev = slots.device
+    slot = int(slots.shape[1])
+    max_w = max(int(l.shape[1]) for l in labels)
+    ws = torch.empty((max(int(_lib.lib.ape_label_rle_pack_workspace_bytes(max_w, int(num_labels), slot)), 1),), dtype=torch.uint8,
+                     device=dev)
+    stream = _lib.current_stream_ptr()
+    with torch.cuda.device(dev), _timed(("semseg_pack", B, slot)):
+        for b, l in enumerate(labels):
+            _require(l.is_cuda and l.dim() == 2 and l.dtype == torch.int64 and l.is_contiguous() and l.device == dev,
+                     "semseg_pack: contiguous CUDA int64 label maps on the slots' device")
+            rc = _lib.lib.ape_label_rle_pack(l.data_ptr(), int(l.shape[0]), int(l.shape[1]), int(num_labels), slot, ws.data_ptr(),
+                                             slots[b].data_ptr(), info[b].data_ptr(), stream)
+            _lib.check(rc, "ape_label_rle_pack")
+
+
 def panoptic_winners(mask_logits, query_index, scores, padded_hw, img_hw, out_hw, prob):
     """Per-pixel winners and segment areas of the panoptic merge of one image without the [K, H, W] mask stacks:
     (ids int32 [out_h, out_w], counts int32 [3, K]).  With

@@ -68,7 +68,14 @@ def unpack_packed(packed: torch.Tensor) -> List[dict]:
     detector_postprocess).  One device->host copy for everything.
     fp32 [images, topk, 13]: boxes only.  uint8 [images, topk, 60 + slot] (instance masks): the same 13 columns as bytes, and
     `pred_masks_rle` = [{"size": [H, W], "counts": bytes}] per kept detection, as `model(inputs)` returns with
-    `mask_format = "rle"`.  A slot that holds its mask as bits is pasted and encoded here (`ops.paste_masks_rle`)."""
+    `mask_format = "rle"`.  A slot that holds its mask as bits is pasted and encoded here (`ops.paste_masks_rle`).
+    uint8 [images, 32 + topk * R + slot] (semantic label maps): per image a header of 8 int32 (topk, R, semantic slot kind,
+    bytes used, output height, width, labels present, 0), its rows in one of the forms above (R = 52: the 13 fp32 columns), then
+    its semantic slot; the dicts gain `sem_seg_rle` as `model(inputs)` returns it with `sem_seg_format = "rle"` (none when the
+    dataset's entity turned the branch off).  A slot that holds the map as uint16 is encoded here (`ops.label_map_rle`); a slot
+    that holds nothing raises ValueError."""
+    if packed.dtype == torch.uint8 and packed.dim() == 2:
+        return _unpack_packed_semantic(packed)
     if packed.dtype == torch.uint8:
         return _unpack_packed_masks(packed)
     host = packed.to("cpu")
@@ -106,7 +113,7 @@ def unpack_mask_bits(slot_bytes) -> torch.Tensor:
     return torch.from_numpy(bits.reshape(a.shape[:-1] + (S, S)).astype(bool))
 
 
-def _unpack_packed_masks(packed: torch.Tensor) -> List[dict]:
+def _unpack_packed_masks(packed: torch.Tensor, device=None) -> List[dict]:
     host = packed.to("cpu")
     rows = host[..., :52].contiguous().view(torch.float32)                     # [images, topk, 13]
     words = host[..., 52:MASK_PACK_HEAD].contiguous().view(torch.int32).numpy()  # [images, topk, 2]: kind, length
@@ -131,11 +138,46 @@ def _unpack_packed_masks(packed: torch.Tensor) -> List[dict]:
 
             n = bits[0][2]
             masks = unpack_mask_bits(raw[i, [k for _, k, _ in bits], MASK_PACK_HEAD:MASK_PACK_HEAD + n])
-            dev = packed.device if packed.is_cuda else torch.device("cuda")
+            dev = device if device is not None else packed.device if packed.is_cuda else torch.device("cuda")
             boxes = inst.pred_boxes.tensor[[j for j, _, _ in bits]]
             for (j, _, _), rle in zip(bits, ops.paste_masks_rle(masks.to(dev), boxes.to(dev), inst.image_size, 0.5)):
                 rles[j] = rle
         inst.pred_masks_rle = rles
+        out.append(res)
+    return out
+
+
+SEM_PACK_HEAD = 32  # = ops.SEM_PACK_HEAD
+SEM_SLOT_NONE, SEM_SLOT_CODES, SEM_SLOT_MAP, SEM_SLOT_OVER = 0, 1, 2, 3  # = ops.SEM_SLOT_*
+
+
+def _unpack_packed_semantic(packed: torch.Tensor) -> List[dict]:
+    import numpy as np
+
+    host = packed.to("cpu")
+    raw = host.numpy()
+    dev = packed.device if packed.is_cuda else torch.device("cuda")
+    out = []
+    for i in range(raw.shape[0]):
+        topk, R, kind, n, oh, ow, P, _ = raw[i, :SEM_PACK_HEAD].view(np.int32).tolist()
+        det = host[i, SEM_PACK_HEAD:SEM_PACK_HEAD + topk * R].reshape(1, topk, R)
+        if R == 4 * 13:
+            res = _unpack_rows(det[0].contiguous().view(torch.float32))[0]
+        else:
+            res = _unpack_packed_masks(det, dev)[0]
+        slot = raw[i, SEM_PACK_HEAD + topk * R:]
+        if kind == SEM_SLOT_CODES:
+            from . import ops
+
+            res["sem_seg_rle"] = ops._label_rle_table(slot[:n], P, oh, ow)
+        elif kind == SEM_SLOT_MAP:
+            from . import ops
+
+            label = torch.from_numpy(slot[:2 * oh * ow].view(np.uint16).astype(np.int64).reshape(oh, ow))
+            res["sem_seg_rle"] = ops.label_map_rle(label.to(dev))
+        elif kind != SEM_SLOT_NONE:
+            raise ValueError(f"unpack_packed: the semantic label map of image {i} ({oh} x {ow}) needs {n} bytes and did not fit its "
+                             f"slot of {slot.size} bytes; raise model.sem_seg_slot_bytes")
         out.append(res)
     return out
 

@@ -488,6 +488,36 @@ int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, u
 int ape_semseg_keys_decode(const uint64_t *keys, int64_t n, int64_t *label, float *score, void *stream);
 
 /*
+ * A label map as cocoapi run-length codes, one per label present, without a mask per label.  Replaces detectron2's
+ * SemSegEvaluator.process -> encode_json_sem_seg: np.unique, then for each label mask_util.encode(np.array((L == c)[:, :, None],
+ * order="F")).  label int64 [H,W] row-major, H*W <= 2^27, labels in [0, 65535].  A "codes body" is P x (int32 label, int32
+ * character offset from the first character, int32 character length) in ascending label order, then the rleToString
+ * characters of every label.  Deterministic: the output does not depend on the order of atomics.
+ *   ape_label_rle_sizes            sizes (device int32 [3]) <- P labels present, m boundaries (t >= 1 with L(t) != L(t-1) in
+ *                                  column-major order t = x*H + y), number of labels outside [0, 65535] (0 or 1).  workspace:
+ *                                  ape_label_rle_workspace_bytes(W, 0, 0).
+ *   ape_label_rle                  out <- the codes body; sizes is a HOST copy of what ape_label_rle_sizes wrote for this map
+ *                                  (labels outside [0, 65535]: APE_ERR_INVALID_ARG).  out holds ape_label_rle_out_bytes(P, m);
+ *                                  out_info (device int32 [3]) <- 1, bytes written, P.  workspace:
+ *                                  ape_label_rle_workspace_bytes(W, P, 2m+1) (P x W int32 and about 3 int32 per boundary).
+ *   ape_label_rle_pack             one image's semantic slot of `slot` bytes with no host read-back (CUDA-graph capturable):
+ *                                  labels in [0, num_labels).  The slot is zeroed, then holds the codes body (kind 1) when it
+ *                                  fits, else the map as uint16 [H,W] row-major (kind 2) when 2*H*W <= slot, else nothing
+ *                                  (kind 3).  A map whose boundaries alone rule out codes that fit skips their passes.
+ *                                  out_info (device int32 [3]) <- kind, bytes used (kind 3: the bytes the smaller form needs, a
+ *                                  lower bound for codes; 0 for labels outside [0, num_labels)), P.  slot a multiple of 4,
+ *                                  >= 16; workspace: ape_label_rle_pack_workspace_bytes(W, num_labels, slot).
+ * Workspaces 256-byte aligned, out 4-byte aligned.
+ */
+int64_t ape_label_rle_workspace_bytes(int W, int P, int64_t events);
+int64_t ape_label_rle_out_bytes(int P, int m);
+int ape_label_rle_sizes(const int64_t *label, int H, int W, void *workspace, int *sizes, void *stream);
+int ape_label_rle(const int64_t *label, int H, int W, const int *sizes, void *workspace, uint8_t *out, int *out_info, void *stream);
+int64_t ape_label_rle_pack_workspace_bytes(int W, int num_labels, int slot);
+int ape_label_rle_pack(const int64_t *label, int H, int W, int num_labels, int slot, void *workspace, uint8_t *out, int *out_info,
+                       void *stream);
+
+/*
  * Panoptic merge without the [K,H,W] mask stacks.  Replaces, for one image, the per-pixel part of
  * deformable_detr_segm_vl.py:919-998 (`_postprocess_panoptic`, after the upsample of :569 and detectron2 sem_seg_postprocess):
  *   v_k = resize2(crop(resize1(logits[index[k]]))), p_k = sigmoid(v_k), id = the first k maximising scores[k] * p_k
