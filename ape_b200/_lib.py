@@ -170,6 +170,10 @@ def _declare(lib):
     lib.ape_label_rle_pack.argtypes = [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]
     lib.ape_panoptic_winners.restype = _i
     lib.ape_panoptic_winners.argtypes = [_vp] * 5 + [_i] * 9 + [ctypes.c_float, _i, _vp]
+    lib.ape_panoptic_pack_workspace_bytes.restype = _i64
+    lib.ape_panoptic_pack_workspace_bytes.argtypes = [_i, _i]
+    lib.ape_panoptic_pack.restype = _i
+    lib.ape_panoptic_pack.argtypes = [_vp] * 3 + [_i] * 4 + [ctypes.c_double, _i, _i, _vp, _vp, _i, _vp]
 
 
 
@@ -240,6 +244,8 @@ EXPORTS = (
     "ape_label_rle_pack_workspace_bytes",
     "ape_label_rle_pack",
     "ape_panoptic_winners",
+    "ape_panoptic_pack_workspace_bytes",
+    "ape_panoptic_pack",
 )
 
 

@@ -12,7 +12,14 @@
 // histograms, which are added to the global counts with one atomic per non-zero bin when the CTA ends.
 //   panoptic_zero_kernel     counts <- 0 (a kernel, so that the pair is one capturable sequence on the stream)
 //   panoptic_winners_kernel  ids [out_h, out_w] int32, counts [3, K] int32
+//
+// ape_panoptic_pack turns those into one image's panoptic slot of forward_packed without reading anything back to the host
+// (the reference's loop over the kept queries, deformable_detr_segm_vl.py:958-995, and the painting of the map):
+//   panoptic_segments_kernel  one CTA: which queries make a segment, their ids, the lookup table query -> segment id, the slot's
+//                             header and segment table
+//   panoptic_paint_kernel     map [out_h, out_w] uint16 = lut[ids] (0 where ids is -1) into the slot, then zeros to its end
 #include <algorithm>
+#include <climits>
 
 #include "common.cuh"
 #include "resize.cuh"
@@ -91,6 +98,135 @@ void launch_winners(int grid, size_t smem, cudaStream_t st, const void *logits, 
              img_h, img_w, s2h, s2w, out_h, out_w, prob, tiles_x, tiles);
 }
 
+// ---- the panoptic slot ----------------------------------------------------------------------------------------------------
+constexpr int kSegThreads = 1024;
+constexpr int kSegPer = APE_PANOPTIC_MAX_K / kSegThreads;  // consecutive queries per thread, so that the scan runs in query order
+constexpr int kSlotHead = 8;                                // int32 header words
+
+// The reference's loop, for k in order: a query with all three areas > 0 and mask_area / original_area not below the threshold
+// takes part; a thing query, or the first such query of its stuff class, opens the next segment id; a later query of a stuff class
+// joins the segment of that class's first one.  In parallel: the first query of each stuff class is a minimum (atomicMin, so it
+// does not depend on the order of the atomics), the ids a block scan over the openers.
+__global__ void __launch_bounds__(kSegThreads) panoptic_segments_kernel(const int *__restrict__ counts, const int *__restrict__ classes,
+                                                                        int K, int num_classes, int num_things, int stuff_first,
+                                                                        double overlap, int out_h, int out_w, int map_bytes,
+                                                                        int *__restrict__ first, int *__restrict__ lut,
+                                                                        int *__restrict__ slot) {
+  __shared__ int s_id[APE_PANOPTIC_MAX_K];  // segment id of every query that opens one
+  __shared__ int s_warp[kSegThreads / 32];
+  pdl_prologue();
+  for (int c = threadIdx.x; c < num_classes; c += kSegThreads) first[c] = INT_MAX;
+  __syncthreads();
+  const int k0 = threadIdx.x * kSegPer;
+  int cls[kSegPer];
+  bool valid[kSegPer];
+#pragma unroll
+  for (int j = 0; j < kSegPer; ++j) {
+    const int k = k0 + j;
+    valid[j] = false;
+    cls[j] = 0;
+    if (k < K) {
+      const int area = counts[k], inter = counts[K + k], orig = counts[2 * K + k], c = classes[k];
+      // the reference skips a query iff area / orig < threshold, the quotient of two ints correctly rounded to a double: the
+      // same IEEE division here (a NaN threshold then skips nothing, as there); a class outside [0, num_classes) takes no part
+      valid[j] = area > 0 && orig > 0 && inter > 0 && !((double)area / (double)orig < overlap) && c >= 0 && c < num_classes;
+      cls[j] = c;
+      if (valid[j] && c >= num_things) atomicMin(first + c, k);
+    }
+  }
+  __syncthreads();
+  int opens = 0;
+  bool open[kSegPer];
+#pragma unroll
+  for (int j = 0; j < kSegPer; ++j) {
+    open[j] = valid[j] && (cls[j] < num_things || __ldcg(first + cls[j]) == k0 + j);
+    opens += open[j];
+  }
+  // exclusive scan of the openers over the CTA (32 warps)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int incl = opens;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += t;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  int before = 0, segments = 0;
+#pragma unroll 8
+  for (int i = 0; i < kSegThreads / 32; ++i) {
+    const int v = s_warp[i];
+    before += i < warp ? v : 0;
+    segments += v;
+  }
+  int id = before + incl - opens;
+#pragma unroll
+  for (int j = 0; j < kSegPer; ++j) {
+    const int k = k0 + j;
+    if (!open[j]) continue;
+    s_id[k] = ++id;
+    const bool thing = cls[j] < num_things;
+    int *row = slot + kSlotHead + 3 * (id - 1);
+    row[0] = id;
+    row[1] = thing ? 1 : 0;
+    row[2] = thing || !stuff_first ? cls[j] : cls[j] - num_things + 1;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < kSegPer; ++j) {
+    const int k = k0 + j;
+    if (k >= K) break;
+    lut[k] = open[j] ? s_id[k] : valid[j] ? s_id[__ldcg(first + cls[j])] : 0;  // a repeat takes its class's segment
+  }
+  for (int i = kSlotHead + 3 * segments + threadIdx.x; i < kSlotHead + 3 * K; i += kSegThreads) slot[i] = 0;  // unused rows
+  if (threadIdx.x == 0) {
+    slot[0] = 1;
+    slot[1] = segments;
+    slot[2] = out_h;
+    slot[3] = out_w;
+    slot[4] = K;
+    slot[5] = 4 * kSlotHead + 12 * K + map_bytes;
+    slot[6] = 0;
+    slot[7] = 0;
+  }
+}
+
+// lut of the segment ids at two pixels as one little-endian word of two uint16 (0 past the map's end and where ids is -1)
+__device__ __forceinline__ uint32_t paint_pair(const int *__restrict__ ids, const int *__restrict__ lut, long long p, long long HW) {
+  int a = -1, b = -1;
+  if (p + 1 < HW) {
+    const int2 v = __ldg(reinterpret_cast<const int2 *>(ids + p));  // p is even, ids 8-byte aligned
+    a = v.x;
+    b = v.y;
+  } else if (p < HW) {
+    a = __ldg(ids + p);
+  }
+  const uint32_t lo = a >= 0 ? (uint32_t)__ldg(lut + a) & 0xffffu : 0u;
+  const uint32_t hi = b >= 0 ? (uint32_t)__ldg(lut + b) & 0xffffu : 0u;
+  return lo | hi << 16;
+}
+
+// map words w = [0, words) of the slot from its map on (word w = pixels 2w, 2w+1): 16-byte stores from the first 16-byte
+// boundary, single words before it (head < 4) and after the last whole vector
+__global__ void __launch_bounds__(256) panoptic_paint_kernel(const int *__restrict__ ids, const int *__restrict__ lut, long long HW,
+                                                             uint32_t *__restrict__ map, long long words, int head) {
+  pdl_prologue();
+  const long long vecs = (words - head) / 4, tail = head + 4 * vecs;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < vecs; i += (long long)gridDim.x * blockDim.x) {
+    const long long w = head + 4 * i;
+    uint4 v;
+    v.x = paint_pair(ids, lut, 2 * w, HW);
+    v.y = paint_pair(ids, lut, 2 * w + 2, HW);
+    v.z = paint_pair(ids, lut, 2 * w + 4, HW);
+    v.w = paint_pair(ids, lut, 2 * w + 6, HW);
+    *reinterpret_cast<uint4 *>(map + w) = v;
+  }
+  if (blockIdx.x == 0 && threadIdx.x < 8) {
+    const long long w = threadIdx.x < 4 ? (long long)threadIdx.x : tail + threadIdx.x - 4;
+    if ((threadIdx.x < 4 && w < head) || (threadIdx.x >= 4 && w < words)) map[w] = paint_pair(ids, lut, 2 * w, HW);
+  }
+}
+
 }  // namespace
 }  // namespace ape
 
@@ -132,4 +268,47 @@ extern "C" int ape_panoptic_winners(const void *logits, const int64_t *index, co
   else APE_PANOPTIC(__nv_bfloat16);
 #undef APE_PANOPTIC
   return check_launch("panoptic_winners_kernel");
+}
+
+namespace {
+int64_t pan_align(int64_t n) { return (n + 255) / 256 * 256; }
+}  // namespace
+
+// workspace: first valid query per class int32 [num_classes], then the lookup table query -> segment id int32 [K]
+extern "C" int64_t ape_panoptic_pack_workspace_bytes(int K, int num_classes) {
+  if (K < 0 || K > APE_PANOPTIC_MAX_K || num_classes < 0) return 0;
+  return pan_align(4LL * std::max(num_classes, 1)) + pan_align(4LL * std::max(K, 1));
+}
+
+extern "C" int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things,
+                                 int stuff_first, double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot,
+                                 int slot_bytes, void *stream) {
+  if (K < 0 || K > APE_PANOPTIC_MAX_K)
+    return fail(APE_ERR_INVALID_ARG, "panoptic_pack: K=%d outside [0, %d]", K, APE_PANOPTIC_MAX_K);
+  if (num_classes < 0 || num_things < 0) return fail(APE_ERR_INVALID_ARG, "panoptic_pack: num_classes %d, num_things %d", num_classes, num_things);
+  if (out_h <= 0 || out_w <= 0) return fail(APE_ERR_INVALID_ARG, "panoptic_pack: bad output size %dx%d", out_h, out_w);
+  const long long HW = (long long)out_h * out_w, need = 4LL * kSlotHead + 12LL * K + 2 * HW;
+  if (slot_bytes < 0 || slot_bytes % 4 != 0 || need > slot_bytes)
+    return fail(APE_ERR_INVALID_ARG, "panoptic_pack: slot of %d bytes (a multiple of 4 of at least %lld for K=%d and %dx%d)", slot_bytes,
+                need, K, out_h, out_w);
+  if (!ids || !workspace || !slot || (K > 0 && (!counts || !classes))) return fail(APE_ERR_NULL_PTR, "panoptic_pack: null pointer");
+  if ((reinterpret_cast<uintptr_t>(workspace) & 255) || (reinterpret_cast<uintptr_t>(slot) & 3) || (reinterpret_cast<uintptr_t>(ids) & 7))
+    return fail(APE_ERR_INVALID_ARG, "panoptic_pack: workspace must be 256-byte, slot 4-byte and ids 8-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  int *first = reinterpret_cast<int *>(workspace);
+  int *lut = reinterpret_cast<int *>(reinterpret_cast<char *>(workspace) + pan_align(4LL * std::max(num_classes, 1)));
+  APE_LAUNCH(panoptic_segments_kernel, 1, kSegThreads, 0, st, counts, classes, K, num_classes, num_things, stuff_first ? 1 : 0,
+             overlap_threshold, out_h, out_w, (int)(2 * HW), first, lut, reinterpret_cast<int *>(slot));
+  int rc = check_launch("panoptic_segments_kernel");
+  if (rc != APE_OK) return rc;
+  uint8_t *map = slot + 4LL * kSlotHead + 12LL * K;
+  const long long words = (slot_bytes - (map - slot)) / 4;
+  const int head = (int)std::min<long long>(((16 - (reinterpret_cast<uintptr_t>(map) & 15)) & 15) / 4, words);
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const long long blocks = ((words - head) / 4 + 255) / 256;
+  const int grid = (int)std::max(1LL, std::min(blocks, 8LL * std::max(sms, 1)));
+  APE_LAUNCH(panoptic_paint_kernel, grid, 256, 0, st, ids, (const int *)lut, HW, reinterpret_cast<uint32_t *>(map), words, head);
+  return check_launch("panoptic_paint_kernel");
 }

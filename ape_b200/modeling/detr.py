@@ -298,6 +298,9 @@ class DeformableDETRSegmVL(nn.Module):
         # SemSegEvaluator.process encodes the map into.  `sem_seg_slot_bytes`: the semantic slot per image of `forward_packed`
         # (codes, or the map as uint16 when they do not fit: the default holds any map up to 1024 x 1024 exactly); a multiple of 4
         self.sem_seg_slot_bytes = 1 << 21
+        # the panoptic slot per image of `forward_packed`: a 32-byte header, 12 bytes per query of the merge and the map as uint16
+        # (ops.panoptic_pack); the default holds any output up to 1024 x 1024 with up to 1024 queries.  A multiple of 4
+        self.panoptic_slot_bytes = (1 << 21) + (1 << 14)
         self.semantic_post_nms = semantic_post_nms
         self.panoptic_post_nms = panoptic_post_nms
         self.panoptic_configs = panoptic_configs if panoptic_configs is not None else {
@@ -519,20 +522,22 @@ class DeformableDETRSegmVL(nn.Module):
                 sel, const = None, (geo, prompt)
                 # forward_packed with instance masks: the mask stage (csrc/mask_post.cu, ape_mask_pack) follows the selection in
                 # the graph; the output sizes and the slot size join the key
-                # with semantic_on the semantic stage (ape_label_rle_pack) follows too, and its configuration joins the key
-                packed = do_postprocess == "packed" and not self.panoptic_on
+                # with semantic_on the semantic stage (ape_label_rle_pack) follows too, and its configuration joins the key; so
+                # does the panoptic stage (ape_panoptic_winners + ape_panoptic_pack) with panoptic_on
+                packed = do_postprocess == "packed"
                 packed_masks = packed and self.instance_on and self.test_mask_on
                 packed_sem = self._packed_semantic_config() if packed and self.semantic_on else None
-                if do_postprocess in (True, "packed") and (not need_masks or packed_masks or packed_sem) and \
+                packed_pan = self._packed_panoptic_config() if packed and self.panoptic_on else None
+                if do_postprocess in (True, "packed") and (not need_masks or packed_masks or packed_sem or packed_pan) and \
                         self.static_inference_cap > 0 and self.test_topk_per_image >= 0 and self.num_queries <= 1024:
                     ent = self.eval_dataset_entity
                     sel = (tuple(image_sizes), bool(getattr(self, "_static_overflowed", False)), float(self.test_score_thresh),
                            float(self.test_nms_thresh), int(self.test_topk_per_image), int(self.static_inference_cap),
                            self.eval_dataset_id, bool(self.instance_on and not (ent and "thing" not in ent)))
                     const = (geo, prompt, sel)
-                    if packed_masks or packed_sem:
+                    if packed_masks or packed_sem or packed_pan:
                         sel += ((self._output_sizes(batched_inputs, image_sizes), int(self.mask_slot_bytes) if packed_masks else None,
-                                 packed_sem),)
+                                 packed_sem, packed_pan),)
                         const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
@@ -688,7 +693,7 @@ class DeformableDETRSegmVL(nn.Module):
         if sel is not None:  # (image sizes, class-wise path?, thresholds ..., instance branch on?) — see forward()
             det_cls = self._detector_box_cls(box_cls) if sel[7] else box_cls
             pack = self._select_device(det_cls, box_pred, sel[0], sel[1])
-            if size_columns is not None:  # sel[8] = (output sizes, mask slot bytes or None, semantic configuration or None)
+            if size_columns is not None:  # sel[8] = (output sizes, mask slot bytes or None, semantic / panoptic configuration or None)
                 pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sel[0], tuple(images.shape[-2:]),
                                        sel[1], *sel[8])
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
@@ -992,25 +997,34 @@ class DeformableDETRSegmVL(nn.Module):
         With `semantic_on`: uint8 [B, 32 + topk * R + sem_seg_slot_bytes] per image, a header of 8 int32 (topk, R, semantic slot
         kind, its bytes used, output height, width, labels present, 0), then that image's rows of either form above (R = 52, or 60 +
         mask_slot_bytes), then its semantic label map as one run-length code per label (`ops.semseg_pack`): `unpack_packed` adds
-        `sem_seg_rle` as `model(inputs)` returns it with `sem_seg_format = "rle"`.  Needs a 16-bit engine_dtype on CUDA."""
-        assert not self.panoptic_on, "forward_packed: boxes, instance masks and semantic label maps; panoptic is not packed"
+        `sem_seg_rle` as `model(inputs)` returns it with `sem_seg_format = "rle"`.  Needs a 16-bit engine_dtype on CUDA.
+        With `panoptic_on`: the same 2-D form with a panoptic slot of `panoptic_slot_bytes` at the end of each image's row, whose
+        size is header word 7 (0 in every other form; without semantic_on the semantic slot is empty, kind 0).  The slot holds a
+        header of 8 int32 (1, or 0 when the dataset's entity turns the branch off; segments S; output height, width; table rows
+        Kt = topk with panoptic_post_nms, else num_queries; bytes used; 0; 0), Kt rows of int32 (id, isthing, category_id) of
+        which the first S are the segments, then the panoptic map as uint16 (`ops.panoptic_pack`): `unpack_packed` adds
+        `panoptic_seg` as `model(inputs)` returns it.  Needs a 16-bit engine_dtype on CUDA; an output whose slot would not fit
+        raises ValueError before anything runs."""
         masks = self.instance_on and self.test_mask_on
         sem = self._packed_semantic_config() if self.semantic_on else None
+        pan = self._packed_panoptic_config() if self.panoptic_on else None
         if sem is not None and not (self.engine_dtype in (torch.float16, torch.bfloat16) and self.device.type == "cuda"):
             raise ValueError("ape_b200: forward_packed with semantic_on needs a CUDA model with a 16-bit engine_dtype (the semantic "
                              "label map is built by ops.semseg_label); use model(inputs) with sem_seg_format = 'rle' instead")
+        if pan is not None:
+            self._check_panoptic_slot(pan, batched_inputs)
         box_cls, box_pred, image_sizes, pack, mask_pred, padded_hw = self.forward(batched_inputs, do_postprocess="packed")
-        if pack is not None and (masks or sem is not None):  # the stages ran in the graph; their buffer is rewritten by the next replay
-            return pack.clone()
+        if pack is not None and (masks or sem is not None or pan is not None):
+            return pack.clone()  # the stages ran in the graph; their buffer is rewritten by the next replay
         if pack is None:  # no graph for this call (fp32 mode, phrase prompts ...): the same selection, eagerly
             ent = self.eval_dataset_entity
             det_cls = self._detector_box_cls(box_cls) if (self.instance_on and not (ent and "thing" not in ent)) else box_cls
             pack = self._select_device(det_cls, box_pred, image_sizes, bool(getattr(self, "_static_overflowed", False)))
         cols = self._size_columns(batched_inputs, image_sizes, pack.device)
-        if masks or sem is not None:
+        if masks or sem is not None or pan is not None:
             return self._pack_rows(pack, cols, box_cls, box_pred, mask_pred, tuple(image_sizes), padded_hw,
                                    bool(getattr(self, "_static_overflowed", False)), self._output_sizes(batched_inputs, image_sizes),
-                                   int(self.mask_slot_bytes) if masks else None, sem)
+                                   int(self.mask_slot_bytes) if masks else None, sem, pan)
         return torch.cat([pack, cols[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
 
     @staticmethod
@@ -1045,24 +1059,88 @@ class DeformableDETRSegmVL(nn.Module):
         return (slot, not (ent and "stuff" not in ent), bool(self.semantic_post_nms), class0, tuple(things or ()), tuple(stuff or ()),
                 entity)
 
+    def _packed_panoptic_config(self):
+        """Everything the packed panoptic stage reads from the model, as a graph-key tuple: (slot bytes, branch on for the
+        evaluated dataset, panoptic_post_nms, thing classes, stuff classes, prob, pano_temp, transform_eval,
+        object_mask_threshold, overlap_threshold)."""
+        ent = self.eval_dataset_entity
+        on = not (ent and "thing+stuff" not in ent)
+        name = self.dataset_names[self.eval_dataset_id] if self.dataset_names else None
+        if on and name not in self.dataset_stuff:  # as _panoptic
+            raise RuntimeError(f"ape_b200: panoptic_on needs model.dataset_stuff[{name!r}] = (thing_classes, stuff_classes, entity)")
+        things, stuff = self.dataset_stuff.get(name, (None, None))[:2]
+        if not (self.engine_dtype in (torch.float16, torch.bfloat16) and self.device.type == "cuda"):
+            raise ValueError("ape_b200: forward_packed with panoptic_on needs a CUDA model with a 16-bit engine_dtype (the panoptic "
+                             "map is built by ops.panoptic_winners); use model(inputs) instead")
+        slot = int(self.panoptic_slot_bytes)
+        if slot < ops.PAN_PACK_HEAD or slot % 4:
+            raise ValueError(f"ape_b200: panoptic_slot_bytes must be a multiple of 4 of at least {ops.PAN_PACK_HEAD} (got {slot})")
+        c = self.panoptic_configs
+        return (slot, bool(on), bool(self.panoptic_post_nms), tuple(things or ()), tuple(stuff or ()), float(c["prob"]),
+                float(c["pano_temp"]), bool(c["transform_eval"]), float(c["object_mask_threshold"]), float(c["overlap_threshold"]))
+
+    def _check_panoptic_slot(self, pan, batched_inputs):
+        """ValueError, before anything is enqueued, when an image's panoptic map would not fit the slot: its size depends only on
+        the output size and the number of queries of the merge."""
+        slot, on, post_nms = pan[:3]
+        if not on:
+            return
+        if post_nms:  # the top-k that _text_features is about to set for this call
+            d = self.eval_dataset_id
+            prompt = self.dataset_prompts[d] if d >= 0 else batched_inputs[0].get("prompt", "name")
+            K = 1 if prompt == "expression" else int(self.select_box_nums_for_evaluation)
+            if self.select_box_nums_for_evaluation_list is not None:
+                K = int(self.select_box_nums_for_evaluation_list[d])
+        else:
+            K = int(self.num_queries)
+        if K > ops.APE_PANOPTIC_MAX_K:
+            raise ValueError(f"ape_b200: forward_packed merges at most {ops.APE_PANOPTIC_MAX_K} queries per panoptic map (got {K})")
+        for i, inp in enumerate(batched_inputs):
+            h, w = inp["image"].shape[-2:]
+            oh, ow = int(inp.get("height", h)), int(inp.get("width", w))
+            need = ops.panoptic_slot_bytes_needed(K, (oh, ow))
+            if need > slot:
+                raise ValueError(f"ape_b200: the panoptic map of image {i} ({oh} x {ow}, {K} queries) needs {need} bytes; "
+                                 f"model.panoptic_slot_bytes is {slot}")
+
     def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes, mask_slot,
-                   sem):
+                   sem, pan=None):
         """Selection rows [B, topk, 9] + size columns -> what forward_packed returns: fp32 [B, topk, 13] rows, or uint8
         [B, topk, 60 + mask_slot] with the kept masks' run-length codes (mask_slot not None); with a semantic configuration
-        (`_packed_semantic_config`) each image's header, those rows as bytes and its semantic slot.  No host synchronisation."""
+        (`_packed_semantic_config`) or a panoptic one (`_packed_panoptic_config`) each image's header, those rows as bytes, its
+        semantic slot (empty without one) and its panoptic slot (none without one).  No host synchronisation."""
         rows = torch.cat([pack, size_columns[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
         if mask_slot is not None:
             rows = ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, mask_slot)
-        if sem is None:
+        if sem is None and pan is None:
             return rows
-        slot, on, post_nms, class0, things, stuff, entity = sem
         B, topk = rows.shape[0], rows.shape[1]
         det = rows.contiguous().view(torch.uint8).reshape(B, -1)
         R = det.shape[1] // max(topk, 1)
-        out = torch.empty((B, ops.SEM_PACK_HEAD + det.shape[1] + slot), dtype=torch.uint8, device=rows.device)
+        sem_bytes = sem[0] if sem is not None else 0
+        pan_bytes = pan[0] if pan is not None else 0
+        out = torch.empty((B, ops.SEM_PACK_HEAD + det.shape[1] + sem_bytes + pan_bytes), dtype=torch.uint8, device=rows.device)
         out[:, ops.SEM_PACK_HEAD:ops.SEM_PACK_HEAD + det.shape[1]] = det
-        slots = out[:, ops.SEM_PACK_HEAD + det.shape[1]:]
         info = torch.zeros((B, 3), dtype=torch.int32, device=rows.device)  # kind, bytes used, labels present
+        if sem is not None:
+            self._pack_semantic(sem, out[:, ops.SEM_PACK_HEAD + det.shape[1]:ops.SEM_PACK_HEAD + det.shape[1] + sem_bytes], info, pack,
+                                box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes)
+        if pan is not None:
+            self._pack_panoptic(pan, out[:, out.shape[1] - pan_bytes:], pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw,
+                                classwise, out_sizes)
+        hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
+        hdr[:, 0], hdr[:, 1] = topk, R
+        hdr[:, 2:4] = info[:, 0:2]
+        hdr[:, 4:6] = size_columns[:, 2:4].to(torch.int32)
+        hdr[:, 6] = info[:, 2]
+        hdr[:, 7] = pan_bytes
+        out[:, :ops.SEM_PACK_HEAD] = hdr.view(torch.uint8)
+        return out
+
+    def _pack_semantic(self, sem, slots, info, pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes):
+        """The semantic slots [B, slot] of `_pack_rows` and their (kind, bytes used, labels present) in info [B, 3]."""
+        slot, on, post_nms, class0, things, stuff, entity = sem
+        B = slots.shape[0]
         if on:
             sem_cls = get_stuff_score(box_cls, list(things), list(stuff), entity)
             if post_nms and self.instance_on and not (self.eval_dataset_entity and "thing" not in self.eval_dataset_entity) and \
@@ -1077,13 +1155,40 @@ class DeformableDETRSegmVL(nn.Module):
             ops.semseg_pack(labels, sem_cls.shape[-1], slots, info)
         else:
             slots.zero_()
-        hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
-        hdr[:, 0], hdr[:, 1] = topk, R
-        hdr[:, 2:4] = info[:, 0:2]
-        hdr[:, 4:6] = size_columns[:, 2:4].to(torch.int32)
-        hdr[:, 6] = info[:, 2]
-        out[:, :ops.SEM_PACK_HEAD] = hdr.view(torch.uint8)
-        return out
+
+    def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes):
+        """The panoptic slots [B, slot] of `_pack_rows`: `_panoptic`'s merge with K = topk queries whatever the kept count (every
+        query without panoptic_post_nms), no host synchronisation.  The rows of the selection at or past the kept count and the
+        queries under object_mask_threshold get the score -inf, so they take no part (ops.panoptic_winners)."""
+        from .postprocess import _query_scores
+
+        slot, on, post_nms, things, stuff, prob, pano_temp, transform_eval, object_mask_threshold, overlap_threshold = pan
+        if not on:
+            slots.zero_()
+            return
+        cfg = {"prob": prob, "pano_temp": pano_temp, "transform_eval": transform_eval, "object_mask_threshold": object_mask_threshold}
+        ent = self.eval_dataset_entity
+        if post_nms and self.instance_on and not (ent and "thing" not in ent) and self._detector_box_cls(box_cls) is box_cls:
+            keep = pack  # _panoptic reuses the instance branch's kept queries in this case
+        elif post_nms:
+            keep = self._select_device(box_cls, box_pred, list(image_sizes), classwise)
+        else:
+            keep = None
+        B, Q = box_cls.shape[0], box_cls.shape[1]
+        stuff_first = bool(stuff) and stuff[0] == "things"
+        for b in range(B):
+            if keep is None:
+                qi, live = torch.arange(Q, device=box_cls.device), None
+            else:
+                qi = keep[b, :, 6].to(torch.int64).clamp(0, Q - 1)
+                live = torch.arange(keep.shape[1], device=keep.device) < keep[b, :, 8].to(torch.int64)
+            scores, labels, kept = _query_scores(box_cls[b, qi].float(), cfg)
+            if live is not None:
+                kept = kept & live
+            ids, counts = ops.panoptic_winners(mask_logits[b].contiguous(), qi, torch.where(kept, scores, float("-inf")), padded_hw,
+                                               image_sizes[b], out_sizes[b], prob)
+            ops.panoptic_pack(ids, counts, labels.to(torch.int32), box_cls.shape[-1], len(things), stuff_first, overlap_threshold,
+                              slots[b])
 
     def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0):
         """`_semantic`'s label map of one image with K = topk queries whatever the kept count (no host synchronisation): the

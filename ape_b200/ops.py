@@ -1080,6 +1080,42 @@ def panoptic_winners(mask_logits, query_index, scores, padded_hw, img_hw, out_hw
     return ids, counts
 
 
+APE_PANOPTIC_MAX_K = 4096  # = include/ape_b200.h: queries per panoptic merge
+PAN_PACK_HEAD = 32  # bytes before a panoptic slot's segment table: 8 int32 header fields
+PAN_ROW = 12        # bytes per segment table row: int32 id, isthing, category_id
+
+
+def panoptic_slot_bytes_needed(K, out_hw):
+    """Bytes a panoptic slot needs for K queries and an output of out_hw: header, K table rows, the uint16 map."""
+    return PAN_PACK_HEAD + PAN_ROW * int(K) + 2 * int(out_hw[0]) * int(out_hw[1])
+
+
+def panoptic_pack(ids, counts, classes, num_classes, num_things, stuff_first, overlap_threshold, slot):
+    """One image's panoptic slot from `panoptic_winners`' (ids, counts) with no host synchronisation (ape_panoptic_pack):
+    postprocess._segments' decisions over the K queries in order and the painting of the map, on the device.  classes int32 [K]
+    (the label of each query, in [0, num_classes)); slot uint8 [slot_bytes] contiguous, 4-byte aligned, at least
+    panoptic_slot_bytes_needed(K, ids.shape) bytes.  The slot gets a header of 8 int32 (1, segments S, out_h, out_w, K, bytes used,
+    0, 0), K rows of (int32 id, isthing, category_id) of which the first S are the segments in id order, the map as uint16
+    [out_h, out_w] (0 = no segment), and zeros to its end."""
+    _require(ids.is_cuda and ids.dim() == 2 and ids.dtype == torch.int32 and ids.is_contiguous(), "panoptic_pack: CUDA int32 ids [H, W]")
+    K = int(counts.shape[1]) if counts.dim() == 2 else -1
+    _require(counts.dtype == torch.int32 and counts.is_contiguous() and tuple(counts.shape) == (3, K), "panoptic_pack: int32 counts [3, K]")
+    _require(classes.dtype == torch.int32 and classes.is_contiguous() and tuple(classes.shape) == (K,), "panoptic_pack: int32 classes [K]")
+    _require(slot.dtype == torch.uint8 and slot.dim() == 1 and slot.is_contiguous(), "panoptic_pack: contiguous uint8 slot")
+    dev = ids.device
+    _require(counts.device == dev and classes.device == dev and slot.device == dev, "panoptic_pack: all tensors on one device")
+    oh, ow = int(ids.shape[0]), int(ids.shape[1])
+    n = int(slot.numel())
+    _require(n >= panoptic_slot_bytes_needed(K, (oh, ow)),
+             f"panoptic_pack: {panoptic_slot_bytes_needed(K, (oh, ow))} bytes needed for K={K} and {oh} x {ow}, the slot has {n}")
+    ws = torch.empty((max(int(_lib.lib.ape_panoptic_pack_workspace_bytes(K, int(num_classes))), 1),), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev), _timed(("panoptic_pack", K, oh * ow)):
+        rc = _lib.lib.ape_panoptic_pack(ids.data_ptr(), counts.data_ptr(), classes.data_ptr(), K, int(num_classes), int(num_things),
+                                        1 if stuff_first else 0, float(overlap_threshold), oh, ow, ws.data_ptr(), slot.data_ptr(), n,
+                                        _lib.current_stream_ptr())
+        _lib.check(rc, "ape_panoptic_pack")
+
+
 _RESAMPLE_TABLES = {}
 
 

@@ -73,7 +73,10 @@ def unpack_packed(packed: torch.Tensor) -> List[dict]:
     bytes used, output height, width, labels present, 0), its rows in one of the forms above (R = 52: the 13 fp32 columns), then
     its semantic slot; the dicts gain `sem_seg_rle` as `model(inputs)` returns it with `sem_seg_format = "rle"` (none when the
     dataset's entity turned the branch off).  A slot that holds the map as uint16 is encoded here (`ops.label_map_rle`); a slot
-    that holds nothing raises ValueError."""
+    that holds nothing raises ValueError.
+    With panoptic maps, header word 7 is the size of a panoptic slot at the end of each image's row (the semantic slot may then
+    be empty, kind 0); the dicts gain `panoptic_seg` = (int32 [H, W] map, segments_info) as `model(inputs)` returns it (none when
+    the dataset's entity turned the branch off)."""
     if packed.dtype == torch.uint8 and packed.dim() == 2:
         return _unpack_packed_semantic(packed)
     if packed.dtype == torch.uint8:
@@ -149,6 +152,21 @@ def _unpack_packed_masks(packed: torch.Tensor, device=None) -> List[dict]:
 
 SEM_PACK_HEAD = 32  # = ops.SEM_PACK_HEAD
 SEM_SLOT_NONE, SEM_SLOT_CODES, SEM_SLOT_MAP, SEM_SLOT_OVER = 0, 1, 2, 3  # = ops.SEM_SLOT_*
+PAN_PACK_HEAD, PAN_ROW = 32, 12  # = ops.PAN_PACK_HEAD, ops.PAN_ROW
+
+
+def _panoptic_from_slot(slot):
+    """A panoptic slot (numpy uint8) -> (panoptic_seg int32 [H, W] host tensor, segments_info) as `model(inputs)` returns them,
+    or None when the dataset's entity turned the branch off (flag 0)."""
+    import numpy as np
+
+    on, S, H, W, K = (int(v) for v in slot[:20].view(np.int32))
+    if not on:
+        return None
+    rows = slot[PAN_PACK_HEAD:PAN_PACK_HEAD + PAN_ROW * S].view(np.int32).reshape(S, 3).tolist()
+    start = PAN_PACK_HEAD + PAN_ROW * K
+    seg = torch.from_numpy(slot[start:start + 2 * H * W].view(np.uint16).astype(np.int32).reshape(H, W))
+    return seg, [{"id": i, "isthing": bool(t), "category_id": c} for i, t, c in rows]
 
 
 def _unpack_packed_semantic(packed: torch.Tensor) -> List[dict]:
@@ -159,13 +177,13 @@ def _unpack_packed_semantic(packed: torch.Tensor) -> List[dict]:
     dev = packed.device if packed.is_cuda else torch.device("cuda")
     out = []
     for i in range(raw.shape[0]):
-        topk, R, kind, n, oh, ow, P, _ = raw[i, :SEM_PACK_HEAD].view(np.int32).tolist()
+        topk, R, kind, n, oh, ow, P, pan = raw[i, :SEM_PACK_HEAD].view(np.int32).tolist()
         det = host[i, SEM_PACK_HEAD:SEM_PACK_HEAD + topk * R].reshape(1, topk, R)
         if R == 4 * 13:
             res = _unpack_rows(det[0].contiguous().view(torch.float32))[0]
         else:
             res = _unpack_packed_masks(det, dev)[0]
-        slot = raw[i, SEM_PACK_HEAD + topk * R:]
+        slot = raw[i, SEM_PACK_HEAD + topk * R:raw.shape[1] - pan]
         if kind == SEM_SLOT_CODES:
             from . import ops
 
@@ -178,6 +196,10 @@ def _unpack_packed_semantic(packed: torch.Tensor) -> List[dict]:
         elif kind != SEM_SLOT_NONE:
             raise ValueError(f"unpack_packed: the semantic label map of image {i} ({oh} x {ow}) needs {n} bytes and did not fit its "
                              f"slot of {slot.size} bytes; raise model.sem_seg_slot_bytes")
+        if pan > 0:
+            panoptic = _panoptic_from_slot(raw[i, raw.shape[1] - pan:])
+            if panoptic is not None:
+                res["panoptic_seg"] = panoptic
         out.append(res)
     return out
 

@@ -534,6 +534,24 @@ int ape_label_rle_pack(const int64_t *label, int H, int W, int num_labels, int s
 int ape_panoptic_winners(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h, int w,
                          int Hp, int Wp, int img_h, int img_w, int out_h, int out_w, float prob, int logit_dtype, void *stream);
 
+/*
+ * One image's panoptic slot from what ape_panoptic_winners wrote (ids [out_h, out_w], counts [3, K]) and classes [K] int32, with
+ * no host read-back.  Replaces the segment bookkeeping and painting of deformable_detr_segm_vl.py:958-995: for k in order, query k
+ * takes part iff mask_area, original_area and inter_area are > 0 and !((double)mask_area / original_area < overlap_threshold)
+ * (and 0 <= classes[k] < num_classes); isthing = classes[k] < num_things; a stuff class that already has a segment maps to it,
+ * otherwise the next id (1, 2, ...) is assigned; category_id = classes[k] - num_things + 1 for stuff when stuff_first, else
+ * classes[k].  Queries whose score was -inf have all-zero counts and take no part.  The slot (slot_bytes, a multiple of 4, at
+ * least 32 + 12 K + 2 out_h out_w; 4-byte aligned) is written completely:
+ *   int32 [8]          1, segments S, out_h, out_w, K, bytes used (32 + 12 K + 2 out_h out_w), 0, 0
+ *   int32 [K][3]       (id, isthing, category_id) of segments 1..S in id order; rows >= S zero
+ *   uint16 [out_h, out_w]  segment id of each pixel (0 = none), row-major; then zeros to the slot's end
+ * workspace (256-byte aligned): ape_panoptic_pack_workspace_bytes(K, num_classes); ids 8-byte aligned.  Two kernels, no allocation,
+ * no synchronisation: capturable in a CUDA graph.  Deterministic.
+ */
+int64_t ape_panoptic_pack_workspace_bytes(int K, int num_classes);
+int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things, int stuff_first,
+                      double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot, int slot_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
