@@ -174,6 +174,10 @@ def _declare(lib):
     lib.ape_panoptic_pack_workspace_bytes.argtypes = [_i, _i]
     lib.ape_panoptic_pack.restype = _i
     lib.ape_panoptic_pack.argtypes = [_vp] * 3 + [_i] * 4 + [ctypes.c_double, _i, _i, _vp, _vp, _i, _vp]
+    lib.ape_pad_geometry.restype = _i
+    lib.ape_pad_geometry.argtypes = [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i] + [ctypes.c_float] * 3 + [_i, _vp, _vp, _i] + [_vp] * 6
+    lib.ape_zero_masked_rows.restype = _i
+    lib.ape_zero_masked_rows.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _vp]
 
 
 
@@ -246,6 +250,8 @@ EXPORTS = (
     "ape_panoptic_winners",
     "ape_panoptic_pack_workspace_bytes",
     "ape_panoptic_pack",
+    "ape_pad_geometry",
+    "ape_zero_masked_rows",
 )
 
 

@@ -144,7 +144,12 @@ class MultiScaleDeformableAttention(nn.Module):
             output = ops.ms_deform_attn_pair_fused_forward(value2, spatial_shapes, level_start_index, host_shapes,
                                                            qo[..., :n_off], qo[..., n_off:], ref32, self.num_points)
         else:
-            if key_padding_mask is not None:
+            if key_padding_mask is not None and engine and value.stride(2) == 1 and \
+                    value.stride(0) == value.shape[1] * value.stride(1):
+                # the projection's output is ours: zero the padded rows in place, and write nothing when there are none (inside
+                # a CUDA graph the mask is passed whatever the image size)
+                value = ops.zero_masked_rows_(value, key_padding_mask)
+            elif key_padding_mask is not None:
                 value = value.masked_fill(key_padding_mask[..., None], float(0))
             value = value.view(bs, num_value, self.num_heads, -1).contiguous()
             output = ops.ms_deform_attn_fused_forward(value, spatial_shapes, level_start_index, qo[..., :n_off], qo[..., n_off:],

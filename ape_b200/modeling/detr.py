@@ -15,6 +15,7 @@ import copy
 import math
 from typing import Dict, List
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -34,6 +35,11 @@ class PositionEmbeddingSine(nn.Module):
         self.num_pos_feats, self.temperature, self.normalize = num_pos_feats, temperature, normalize
         self.scale, self.eps, self.offset = scale, eps, offset
 
+    def dim_t(self, device):
+        """The frequency table [num_pos_feats] fp32; ops.pad_geometry takes it from here, so its rounding is torch's."""
+        dim_t = torch.arange(self.num_pos_feats, dtype=torch.float32, device=device)
+        return self.temperature ** (2 * torch.div(dim_t, 2, rounding_mode="floor") / self.num_pos_feats)
+
     def forward(self, mask):
         not_mask = ~mask
         y = not_mask.cumsum(1, dtype=torch.float32)
@@ -41,8 +47,7 @@ class PositionEmbeddingSine(nn.Module):
         if self.normalize:
             y = (y + self.offset) / (y[:, -1:, :] + self.eps) * self.scale
             x = (x + self.offset) / (x[:, :, -1:] + self.eps) * self.scale
-        dim_t = torch.arange(self.num_pos_feats, dtype=torch.float32, device=mask.device)
-        dim_t = self.temperature ** (2 * torch.div(dim_t, 2, rounding_mode="floor") / self.num_pos_feats)
+        dim_t = self.dim_t(mask.device)
         px = x[:, :, :, None] / dim_t
         py = y[:, :, :, None] / dim_t
         B, H, W = mask.shape
@@ -332,7 +337,7 @@ class DeformableDETRSegmVL(nn.Module):
         # (tools/train_net.py:641-642).  float32 = strict-parity mode on fp32 library kernels.
         self.engine_dtype = torch.float32
         self.profile_stages = False   # record CUDA-event stage times of the last forward in self.stage_ms
-        self.use_cuda_graphs = False  # capture the static stages once per input geometry (16-bit engine mode)
+        self.use_cuda_graphs = False  # capture the static stages once per padded shape and prompt configuration (16-bit engine mode)
         import collections
 
         self._geo_cache, self._graph_cache = {}, collections.OrderedDict()
@@ -508,7 +513,10 @@ class DeformableDETRSegmVL(nn.Module):
         images, img_masks, image_sizes = self.preprocess_image(batched_inputs)
         mark("preprocess")
         low = self.engine_dtype != torch.float32
-        geo = self._geometry(images.shape, image_sizes, img_masks)
+        # CUDA: the padded shape's geometry here; the per-size part (ops.pad_geometry, from `sizes` on the device) below, or
+        # at the start of the captured graph, which therefore serves every image size inside the padded shape
+        sizes = self._sizes_tensor(image_sizes) if images.is_cuda else None
+        geo = self._padded_geometry(images.shape) if images.is_cuda else self._geometry(images.shape, image_sizes, img_masks)
         mask_prompt_flatten = self._mask_prompt(batched_inputs, images.shape, geo) if "mask_prompt" in batched_inputs[0] else None
         graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion) and mask_prompt_flatten is None
         need_masks = self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)
@@ -531,26 +539,32 @@ class DeformableDETRSegmVL(nn.Module):
                 if do_postprocess in (True, "packed") and (not need_masks or packed_masks or packed_sem or packed_pan) and \
                         self.static_inference_cap > 0 and self.test_topk_per_image >= 0 and self.num_queries <= 1024:
                     ent = self.eval_dataset_entity
-                    sel = (tuple(image_sizes), bool(getattr(self, "_static_overflowed", False)), float(self.test_score_thresh),
+                    sel = (bool(getattr(self, "_static_overflowed", False)), float(self.test_score_thresh),
                            float(self.test_nms_thresh), int(self.test_topk_per_image), int(self.static_inference_cap),
                            self.eval_dataset_id, bool(self.instance_on and not (ent and "thing" not in ent)))
                     const = (geo, prompt, sel)
                     if packed_masks or packed_sem or packed_pan:
-                        sel += ((self._output_sizes(batched_inputs, image_sizes), int(self.mask_slot_bytes) if packed_masks else None,
-                                 packed_sem, packed_pan),)
+                        # the packed mask / semantic / panoptic stages size their grids and workspaces from host ints (ape_mask_pack's
+                        # output sizes and row width, the label-map GEMM and ape_panoptic_winners at the output resolution), so
+                        # their graphs keep the image and output sizes in the key: one graph per combination of sizes
+                        sel += ((tuple(image_sizes), self._output_sizes(batched_inputs, image_sizes),
+                                 int(self.mask_slot_bytes) if packed_masks else None, packed_sem, packed_pan),)
                         const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
+                # the image sizes are a graph input like the image: the key holds the padded shape, not the sizes
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
-                    ("forward", prompt, tuple(images.shape), tuple(image_sizes), tuple(features_l.shape), need_masks, sel),
-                    self._stage_all, (images, fusion, features_l), const)
+                    ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel),
+                    self._stage_all, (images, fusion, features_l, sizes), const)
                 self.transformer.last_topk_proposals = topk
                 mark("encode")
                 mark("select")
             else:
                 if graphs:
-                    memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._graphed(
-                        ("encode", tuple(images.shape), tuple(image_sizes), need_masks), self._stage_encode, (images, fusion), (geo,))
+                    memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features, geo = self._graphed(
+                        ("encode", tuple(images.shape), need_masks), self._stage_encode_sized, (images, fusion, sizes), (geo,))
                 else:
+                    if images.is_cuda:
+                        geo = self._geometry(images.shape, image_sizes, sizes=sizes)
                     memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = \
                         self._stage_encode(images, fusion, geo, mask_prompt_flatten)
                 mark("encode")
@@ -561,7 +575,7 @@ class DeformableDETRSegmVL(nn.Module):
                 if graphs:
                     # memory / output_memory / enc_coord are the encode graph's static outputs: constants of this graph
                     box_cls, box_pred, inter_states, init_reference, inter_references, mask_logits = self._graphed(
-                        ("decode", memory.data_ptr(), tuple(image_sizes), tuple(features_l.shape), need_masks), self._stage_decode,
+                        ("decode", memory.data_ptr(), tuple(features_l.shape), need_masks), self._stage_decode,
                         (topk, features_l), (memory, output_memory, enc_coord, geo, mask_features))
                 else:
                     box_cls, box_pred, inter_states, init_reference, inter_references, mask_logits = self._stage_decode(
@@ -622,23 +636,63 @@ class DeformableDETRSegmVL(nn.Module):
         return out
 
     # -- stages (static shapes, no host synchronisation: CUDA-graph capturable) -----------------------------
-    def _geometry(self, batch_shape, image_sizes, img_masks):
-        """Padding masks, sine position embeddings (:375-392) and the transformer's geometric constants for
-        one (batch shape, image sizes) combination; cached — they do not depend on pixel values."""
-        key = (tuple(batch_shape), tuple(image_sizes))
-        geo = self._geo_cache.get(key)
-        if geo is None:
-            levels = self.neck.in_features if self.neck is not None else self.backbone._out_features  # (:375-378)
-            strides = [self.backbone._out_feature_strides[f] for f in levels]
-            H, W = batch_shape[-2], batch_shape[-1]
-            shapes = [(-(-H // s), -(-W // s)) for s in strides]
+    def _level_shapes(self, batch_shape):
+        levels = self.neck.in_features if self.neck is not None else self.backbone._out_features  # (:375-378)
+        strides = [self.backbone._out_feature_strides[f] for f in levels]
+        H, W = batch_shape[-2], batch_shape[-1]
+        return [(-(-H // s), -(-W // s)) for s in strides]
+
+    def _geometry(self, batch_shape, image_sizes, img_masks=None, sizes=None):
+        """Padding masks, sine position embeddings (:375-392) and the transformer's geometric constants for one batch.  CUDA:
+        the padded shape's part (`_padded_geometry`) and the per-size part from ops.pad_geometry over `sizes` (int32 [B, 2] on
+        the device; uploaded from image_sizes when None).  Elsewhere: the torch restatement over the pixel masks img_masks."""
+        shapes = self._level_shapes(batch_shape)
+        if self.device.type != "cuda":
             masks = [F.interpolate(img_masks[None], size=sh).to(torch.bool).squeeze(0) for sh in shapes]
             pos = [self.position_embedding(m).to(torch.float32) for m in masks]
-            geo = self.transformer.geometry(shapes, masks, pos)
+            return self.transformer.geometry(shapes, masks, pos)
+        if sizes is None:
+            sizes = self._sizes_tensor(image_sizes)
+        return self._size_geometry(self._padded_geometry(batch_shape), sizes, self._has_padding(batch_shape, shapes, image_sizes))
+
+    def _padded_geometry(self, batch_shape):
+        """The geometry that depends only on the padded shape (level shapes, start indices, level ids, the sine table),
+        cached per padded shape: few keys whatever the image sizes."""
+        H, W = int(batch_shape[-2]), int(batch_shape[-1])
+        key = (H, W, str(self.device))
+        geo = self._geo_cache.get(key)
+        if geo is None:
+            geo = self.transformer.padded_geometry(self._level_shapes(batch_shape), self.device)
+            geo.update(padded_hw=(H, W), dim_t=self.position_embedding.dim_t(self.device))
             if len(self._geo_cache) > 16:
                 self._geo_cache.clear()
             self._geo_cache[key] = geo
         return geo
+
+    def _size_geometry(self, padded, sizes, has_padding):
+        return self.transformer.size_geometry(padded, sizes, padded["padded_hw"], padded["dim_t"], self.position_embedding,
+                                              self.engine_dtype, has_padding)
+
+    def _sizes_tensor(self, image_sizes):
+        """The image sizes as int32 [B, 2] (h, w) on the device, cached per sizes (read-only): a repeated size costs no upload, a
+        new one is copied from pinned memory without a host synchronisation."""
+        key = (tuple((int(h), int(w)) for h, w in image_sizes), str(self.device))
+        cache = self.__dict__.setdefault("_sizes_dev", {})
+        sizes = cache.get(key)
+        if sizes is None:
+            if len(cache) > 64:
+                cache.clear()
+            sizes = cache[key] = torch.tensor(key[0], dtype=torch.int32, pin_memory=True).to(self.device, non_blocking=True)
+        return sizes
+
+    @staticmethod
+    def _has_padding(batch_shape, shapes, image_sizes):
+        """bool(mask_flatten.any()) of the torch geometry, from the host sizes: a level has padding when the nearest source
+        pixel of its last row or column (F.interpolate: min(floor(i * (float)in / out), in - 1) in fp32) lies outside the image."""
+        def src(n_in, n_out):
+            return min(int(np.floor(np.float32(n_out - 1) * (np.float32(n_in) / np.float32(n_out)))), n_in - 1)
+        H, W = int(batch_shape[-2]), int(batch_shape[-1])
+        return any(src(H, hl) >= h or src(W, wl) >= w for hl, wl in shapes for h, w in image_sizes)
 
     def _mask_prompt(self, batched_inputs, batch_shape, geo):
         """:394-412: region prompts.  Per-image masks padded like the image (ImageList.from_tensors), an all-zero batch means
@@ -683,19 +737,29 @@ class DeformableDETRSegmVL(nn.Module):
             return features_l
         return 0.0 * features_l + 1.0 * fusion_out.float()  # (:448)
 
-    def _stage_all(self, images, fusion, features_l, geo, prompt, sel=None, size_columns=None):
+    def _stage_encode_sized(self, images, fusion, sizes, padded):
+        """_stage_encode after the per-size geometry, for the encode graph of the profiling split; the geometry is returned too,
+        because selection and the decode graph read it."""
+        geo = self._size_geometry(padded, sizes, True)
+        return self._stage_encode(images, fusion, geo) + (geo,)
+
+    def _stage_all(self, images, fusion, features_l, sizes, padded, prompt, sel=None, size_columns=None):
+        # inside a graph the padding mask is always passed: an all-false mask gives the values of None (masked_fill with no
+        # true entry changes nothing), so one graph serves padded and unpadded sizes alike
+        geo = self._size_geometry(padded, sizes, True)
         memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._stage_encode(images, fusion, geo)
         topk = self.transformer.stage_select(enc_cls, enc_coord, geo)
         features_l = self._mix_text(prompt, features_l, fusion_out)
         box_cls, box_pred, inter_states, init_reference, inter_references, mask_logits = self._stage_decode(
             topk, features_l, memory, output_memory, enc_coord, geo, mask_features)
         pack = None
-        if sel is not None:  # (image sizes, class-wise path?, thresholds ..., instance branch on?) — see forward()
-            det_cls = self._detector_box_cls(box_cls) if sel[7] else box_cls
-            pack = self._select_device(det_cls, box_pred, sel[0], sel[1])
-            if size_columns is not None:  # sel[8] = (output sizes, mask slot bytes or None, semantic / panoptic configuration or None)
-                pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sel[0], tuple(images.shape[-2:]),
-                                       sel[1], *sel[8])
+        if sel is not None:  # (class-wise path?, thresholds ..., instance branch on?) — see forward()
+            det_cls = self._detector_box_cls(box_cls) if sel[6] else box_cls
+            pack = self._select_device(det_cls, box_pred, sizes, sel[0])
+            if size_columns is not None:  # sel[7] = (image sizes, output sizes, mask slot bytes or None, semantic / panoptic configuration)
+                image_sizes, out_sizes, mask_slot, sem, pan = sel[7]
+                pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, tuple(images.shape[-2:]),
+                                       sel[0], out_sizes, mask_slot, sem, pan)
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                 init_reference, inter_references, mask_logits, pack)
 
@@ -741,8 +805,8 @@ class DeformableDETRSegmVL(nn.Module):
         if entry is not None:
             self._graph_cache.move_to_end(key)
         if entry is None:
-            # bounded cache: every distinct (h, w) inside the square pad is its own graph (masks / valid ratios are baked in),
-            # each with a private memory pool; evict the least recently used together with its geometry
+            # bounded cache, each graph with a private memory pool: the image sizes are an input, but prompts, batch shapes,
+            # selection settings and the packed stages' output sizes still make keys; evict the least recently used
             while len(self._graph_cache) >= self.graph_cache_size:
                 self._graph_cache.popitem(last=False)
             static_in = [None if t is None else t.clone() for t in tensor_args]  # None: no fusion input (DeformableDETRSegm)
@@ -920,9 +984,12 @@ class DeformableDETRSegmVL(nn.Module):
         if topk < 0 or box_cls.shape[1] > 1024:
             return None
         classwise = bool(getattr(self, "_static_overflowed", False))
+        sizes = None
         for attempt in range(2):
+            if not (attempt == 0 and first_pack is not None) and sizes is None:
+                sizes = self._sizes_tensor(image_sizes)
             dev_pack = first_pack if (attempt == 0 and first_pack is not None) else \
-                self._select_device(box_cls, box_pred, image_sizes, classwise)
+                self._select_device(box_cls, box_pred, sizes, classwise)
             host = dev_pack.to("cpu")  # the one synchronising copy
             over = any(int(host[b, 0, 7].item()) > cap for b in range(len(image_sizes)))
             if over == classwise:
@@ -938,19 +1005,23 @@ class DeformableDETRSegmVL(nn.Module):
                                      pred_classes=p[:, 5].to(torch.int64), query_index=p[:, 6].to(torch.int64)))
         return results
 
-    def _select_device(self, box_cls, box_pred, image_sizes, classwise):
+    def _select_device(self, box_cls, box_pred, sizes, classwise):
         """Device half of `_inference_static`: [B, topk, 9] fp32 = (x1, y1, x2, y2, score, class, query index, number of
         candidates, number kept) per detection slot; static shapes, no host synchronisation (CUDA-graph / NCCL friendly)."""
         cap, topk = int(self.static_inference_cap), int(self.test_topk_per_image)
+        # sizes: int32 [B, 2] (h, w) on the device (a graph input), so the fp32 scaling and clamp below read them from device memory
+        hw = sizes.to(device=box_cls.device, dtype=torch.float32)
+        zero = hw.new_zeros(())
         packs = []
-        for b, (h, w) in enumerate(image_sizes):
+        for b in range(box_cls.shape[0]):
+            h, w = hw[b, 0], hw[b, 1]
             scores = box_cls[b].float().sigmoid().contiguous()                              # [Q, N] (bg column dropped again, :772)
             xyxy = box_cxcywh_to_xyxy(box_pred[b].float())
-            boxes = torch.stack((xyxy[:, 0] * float(w), xyxy[:, 1] * float(h), xyxy[:, 2] * float(w), xyxy[:, 3] * float(h)), dim=-1)
+            boxes = torch.stack((xyxy[:, 0] * w, xyxy[:, 1] * h, xyxy[:, 2] * w, xyxy[:, 3] * h), dim=-1)
             valid = torch.isfinite(boxes).all(dim=1) & torch.isfinite(scores).all(dim=1)     # fast_rcnn.py:120-123
             qmap = valid.cumsum(0) - 1                                                       # row index after the filter
-            boxes = torch.stack((boxes[:, 0].clamp(min=0, max=w), boxes[:, 1].clamp(min=0, max=h),
-                                 boxes[:, 2].clamp(min=0, max=w), boxes[:, 3].clamp(min=0, max=h)), dim=-1).contiguous()
+            boxes = torch.stack((boxes[:, 0].clamp(min=zero, max=w), boxes[:, 1].clamp(min=zero, max=h),
+                                 boxes[:, 2].clamp(min=zero, max=w), boxes[:, 3].clamp(min=zero, max=h)), dim=-1).contiguous()
             mask = (scores > self.test_score_thresh) & valid[:, None]
             n = mask.sum().to(torch.int32).reshape(1)
             Q, N = scores.shape
@@ -1019,10 +1090,10 @@ class DeformableDETRSegmVL(nn.Module):
         if pack is None:  # no graph for this call (fp32 mode, phrase prompts ...): the same selection, eagerly
             ent = self.eval_dataset_entity
             det_cls = self._detector_box_cls(box_cls) if (self.instance_on and not (ent and "thing" not in ent)) else box_cls
-            pack = self._select_device(det_cls, box_pred, image_sizes, bool(getattr(self, "_static_overflowed", False)))
+            pack = self._select_device(det_cls, box_pred, self._sizes_tensor(image_sizes), bool(getattr(self, "_static_overflowed", False)))
         cols = self._size_columns(batched_inputs, image_sizes, pack.device)
         if masks or sem is not None or pan is not None:
-            return self._pack_rows(pack, cols, box_cls, box_pred, mask_pred, tuple(image_sizes), padded_hw,
+            return self._pack_rows(pack, cols, box_cls, box_pred, mask_pred, self._sizes_tensor(image_sizes), tuple(image_sizes), padded_hw,
                                    bool(getattr(self, "_static_overflowed", False)), self._output_sizes(batched_inputs, image_sizes),
                                    int(self.mask_slot_bytes) if masks else None, sem, pan)
         return torch.cat([pack, cols[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
@@ -1103,8 +1174,8 @@ class DeformableDETRSegmVL(nn.Module):
                 raise ValueError(f"ape_b200: the panoptic map of image {i} ({oh} x {ow}, {K} queries) needs {need} bytes; "
                                  f"model.panoptic_slot_bytes is {slot}")
 
-    def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes, mask_slot,
-                   sem, pan=None):
+    def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes,
+                   mask_slot, sem, pan=None):
         """Selection rows [B, topk, 9] + size columns -> what forward_packed returns: fp32 [B, topk, 13] rows, or uint8
         [B, topk, 60 + mask_slot] with the kept masks' run-length codes (mask_slot not None); with a semantic configuration
         (`_packed_semantic_config`) or a panoptic one (`_packed_panoptic_config`) each image's header, those rows as bytes, its
@@ -1124,10 +1195,10 @@ class DeformableDETRSegmVL(nn.Module):
         info = torch.zeros((B, 3), dtype=torch.int32, device=rows.device)  # kind, bytes used, labels present
         if sem is not None:
             self._pack_semantic(sem, out[:, ops.SEM_PACK_HEAD + det.shape[1]:ops.SEM_PACK_HEAD + det.shape[1] + sem_bytes], info, pack,
-                                box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes)
+                                box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes)
         if pan is not None:
-            self._pack_panoptic(pan, out[:, out.shape[1] - pan_bytes:], pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw,
-                                classwise, out_sizes)
+            self._pack_panoptic(pan, out[:, out.shape[1] - pan_bytes:], pack, box_cls, box_pred, mask_logits, sizes, image_sizes,
+                                padded_hw, classwise, out_sizes)
         hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
         hdr[:, 0], hdr[:, 1] = topk, R
         hdr[:, 2:4] = info[:, 0:2]
@@ -1137,7 +1208,8 @@ class DeformableDETRSegmVL(nn.Module):
         out[:, :ops.SEM_PACK_HEAD] = hdr.view(torch.uint8)
         return out
 
-    def _pack_semantic(self, sem, slots, info, pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes):
+    def _pack_semantic(self, sem, slots, info, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise,
+                       out_sizes):
         """The semantic slots [B, slot] of `_pack_rows` and their (kind, bytes used, labels present) in info [B, 3]."""
         slot, on, post_nms, class0, things, stuff, entity = sem
         B = slots.shape[0]
@@ -1147,7 +1219,7 @@ class DeformableDETRSegmVL(nn.Module):
                     self._detector_box_cls(box_cls) is box_cls and sem_cls.shape == box_cls.shape:
                 keep = pack  # _semantic reuses the instance branch's kept queries in this case
             elif post_nms:
-                keep = self._select_device(sem_cls, box_pred, list(image_sizes), classwise)
+                keep = self._select_device(sem_cls, box_pred, sizes, classwise)
             else:
                 keep = None
             labels = [self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw, image_sizes[b],
@@ -1156,7 +1228,7 @@ class DeformableDETRSegmVL(nn.Module):
         else:
             slots.zero_()
 
-    def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, image_sizes, padded_hw, classwise, out_sizes):
+    def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes):
         """The panoptic slots [B, slot] of `_pack_rows`: `_panoptic`'s merge with K = topk queries whatever the kept count (every
         query without panoptic_post_nms), no host synchronisation.  The rows of the selection at or past the kept count and the
         queries under object_mask_threshold get the score -inf, so they take no part (ops.panoptic_winners)."""
@@ -1171,7 +1243,7 @@ class DeformableDETRSegmVL(nn.Module):
         if post_nms and self.instance_on and not (ent and "thing" not in ent) and self._detector_box_cls(box_cls) is box_cls:
             keep = pack  # _panoptic reuses the instance branch's kept queries in this case
         elif post_nms:
-            keep = self._select_device(box_cls, box_pred, list(image_sizes), classwise)
+            keep = self._select_device(box_cls, box_pred, sizes, classwise)
         else:
             keep = None
         B, Q = box_cls.shape[0], box_cls.shape[1]

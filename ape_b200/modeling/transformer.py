@@ -462,6 +462,26 @@ class DeformableDetrTransformerVL(nn.Module):
                     output_proposals=out, proposal_invalid=mask_flatten.unsqueeze(-1) | ~valid,
                     level_ids=torch.cat(level_ids), has_padding=bool(mask_flatten.any()))
 
+    @staticmethod
+    def padded_geometry(shapes, device):
+        """The part of `geometry` that depends only on the padded shape: level shapes, their start indices and the level of
+        every token.  One per padded shape, whatever the image sizes inside it."""
+        spatial_shapes = torch.as_tensor(shapes, dtype=torch.long, device=device)
+        level_start_index = torch.cat((spatial_shapes.new_zeros((1,)), spatial_shapes.prod(1).cumsum(0)[:-1]))
+        level_ids = torch.cat([torch.full((h * w,), lvl, dtype=torch.long, device=device) for lvl, (h, w) in enumerate(shapes)])
+        return dict(shapes=list(shapes), spatial_shapes=spatial_shapes, level_start_index=level_start_index, level_ids=level_ids)
+
+    def size_geometry(self, padded, sizes, padded_hw, dim_t, position_embedding, engine_dtype, has_padding):
+        """`geometry` for the image sizes int32 [B, 2] (h, w) held on the device, over `padded_geometry`'s part.  One launch
+        (ops.pad_geometry) writes the padding masks, the position + level embedding in the engine dtype (`pos_lvl`, what
+        stage_encode adds), the valid ratios, reference points and anchors from the same fp32 operations as `geometry` and
+        PositionEmbeddingSine; it reads the sizes from device memory, so a captured graph replays it for any sizes."""
+        pe = position_embedding
+        g = ops.pad_geometry(sizes, padded_hw, padded["shapes"], dim_t, self.level_embeds, engine_dtype, offset=pe.offset,
+                             eps=pe.eps, scale=pe.scale, normalize=pe.normalize)
+        del g["pos_flatten"]
+        return dict(padded, **g, has_padding=has_padding)
+
     def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l):
         """The encoder call of stage_encode -> (memory, language features after the fusion layers)."""
         return self.encoder(
@@ -478,14 +498,16 @@ class DeformableDetrTransformerVL(nn.Module):
         if feat_flatten is None:
             feat_flatten = torch.cat([f.flatten(2).transpose(1, 2) for f in multi_level_feats], 1)
         engine_dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else torch.float32
-        ck = (self.level_embeds._version, self.level_embeds.data_ptr())
-        cache = geo.setdefault("_pos_lvl", {})  # position + level embedding: constant per geometry and weights, one entry per dtype
-        if engine_dtype not in cache or cache[engine_dtype][0] != ck:
-            with torch.no_grad():
-                lvl_embed = torch.cat([self.level_embeds[i].view(1, 1, -1).expand(1, h * w, -1)
-                                       for i, (h, w) in enumerate(geo["shapes"])], 1)
-                cache[engine_dtype] = (ck, (geo["pos_flatten"] + lvl_embed.float()).to(engine_dtype).contiguous())
-        pos_flatten = cache[engine_dtype][1]
+        pos_flatten = geo.get("pos_lvl")  # size_geometry: already summed in the engine dtype
+        if pos_flatten is None:
+            ck = (self.level_embeds._version, self.level_embeds.data_ptr())
+            cache = geo.setdefault("_pos_lvl", {})  # position + level embedding: constant per geometry and weights, one entry per dtype
+            if engine_dtype not in cache or cache[engine_dtype][0] != ck:
+                with torch.no_grad():
+                    lvl_embed = torch.cat([self.level_embeds[i].view(1, 1, -1).expand(1, h * w, -1)
+                                           for i, (h, w) in enumerate(geo["shapes"])], 1)
+                    cache[engine_dtype] = (ck, (geo["pos_flatten"] + lvl_embed.float()).to(engine_dtype).contiguous())
+            pos_flatten = cache[engine_dtype][1]
         memory, query_l = self._encode(feat_flatten, pos_flatten, geo, query_l, attention_mask_l)
         # gen_encoder_output_proposals (:354-369): zero the memory of invalid anchors, project, normalise
         output_proposals = geo["output_proposals"]

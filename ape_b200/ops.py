@@ -147,8 +147,9 @@ def msda_pair_values(value, num_heads, token_mask=None):
     H = int(num_heads)
     out = torch.empty((B, S, H, 2, C // H), dtype=value.dtype, device=value.device)
     mptr = None
-    if token_mask is not None:
-        token_mask = token_mask.to(torch.uint8).contiguous()
+    if token_mask is not None:  # a bool mask is read as its bytes (no conversion launch)
+        token_mask = token_mask.contiguous()
+        token_mask = token_mask.view(torch.uint8) if token_mask.dtype == torch.bool else token_mask.to(torch.uint8)
         _require(token_mask.numel() == B * S, "msda_pair_values: token_mask must be [B,S]")
         mptr = token_mask.data_ptr()
     with torch.cuda.device(value.device), _timed(("msda_pair_values", B, S, C)):
@@ -1216,3 +1217,60 @@ def _register():
 
 
 _LIBRARY = _register()
+
+
+def pad_geometry(sizes, padded_hw, shapes, dim_t, level_embeds, engine_dtype, offset=0.0, eps=1e-6, scale=6.283185307179586,
+                 normalize=True, want_pos=False):
+    """The per-image-size geometry of a padded batch in one launch (ape_pad_geometry), what
+    DeformableDetrTransformerVL.geometry returns for the padding masks F.interpolate'd from the image sizes, plus
+    PositionEmbeddingSine's embedding: sizes int32 [B, 2] (h, w) on the device; padded_hw and the level shapes [L, 2] host ints;
+    dim_t fp32 [E/2] (PositionEmbeddingSine.dim_t); level_embeds [L, E].  Returns a dict of mask_flatten bool [B, S],
+    pos_lvl engine_dtype [B, S, E] (pos + level embedding), pos_flatten fp32 [B, S, E] (only with want_pos, else None),
+    valid_ratios fp32 [B, L, 2], reference_points fp32 [B, S, L, 2], output_proposals fp32 [B, S, 4] and proposal_invalid
+    bool [B, S, 1].  The outputs are allocated here, so inside a capture they belong to the graph's pool."""
+    _require(sizes.is_cuda and sizes.dtype == torch.int32 and sizes.dim() == 2 and sizes.shape[1] == 2 and sizes.is_contiguous(),
+             "pad_geometry: sizes must be a contiguous CUDA int32 [B, 2] tensor")
+    dev = sizes.device
+    B = int(sizes.shape[0])
+    L = len(shapes)
+    E = int(level_embeds.shape[-1]) if level_embeds.dim() == 2 else -1
+    _require(level_embeds.dim() == 2 and int(level_embeds.shape[0]) >= L, "pad_geometry: level_embeds must be [L, E]")
+    _require(dim_t.dim() == 1 and 2 * int(dim_t.numel()) == E, f"pad_geometry: dim_t must have E/2 = {E // 2} entries")
+    hw = (ctypes.c_int * max(2 * L, 1))(*[int(v) for sh in shapes for v in sh])
+    S = sum(int(h) * int(w) for h, w in shapes)
+    dt = dim_t.to(device=dev, dtype=torch.float32).contiguous()
+    lv = level_embeds.detach()[:L].to(device=dev, dtype=torch.float32).contiguous()
+    out = dict(mask_flatten=torch.empty((B, S), dtype=torch.bool, device=dev),
+               pos_lvl=torch.empty((B, S, E), dtype=engine_dtype, device=dev),
+               pos_flatten=torch.empty((B, S, E), dtype=torch.float32, device=dev) if want_pos else None,
+               valid_ratios=torch.empty((B, L, 2), dtype=torch.float32, device=dev),
+               reference_points=torch.empty((B, S, L, 2), dtype=torch.float32, device=dev),
+               output_proposals=torch.empty((B, S, 4), dtype=torch.float32, device=dev),
+               proposal_invalid=torch.empty((B, S, 1), dtype=torch.bool, device=dev))
+    code = _lib.dtype_code(engine_dtype) if engine_dtype in (torch.float32, torch.float16, torch.bfloat16) else -1
+    pf = out["pos_flatten"]
+    with torch.cuda.device(dev), _timed(("pad_geometry", B, S, E)):
+        rc = _lib.lib.ape_pad_geometry(sizes.data_ptr(), B, int(padded_hw[0]), int(padded_hw[1]), hw, L, dt.data_ptr(), lv.data_ptr(),
+                                       E, float(offset), float(eps), float(scale), 1 if normalize else 0,
+                                       out["mask_flatten"].data_ptr(), out["pos_lvl"].data_ptr(), code,
+                                       pf.data_ptr() if pf is not None else None, out["valid_ratios"].data_ptr(),
+                                       out["reference_points"].data_ptr(), out["output_proposals"].data_ptr(),
+                                       out["proposal_invalid"].data_ptr(), _lib.current_stream_ptr())
+        _lib.check(rc, "ape_pad_geometry")
+    return out
+
+
+def zero_masked_rows_(x, mask):
+    """In place: the rows of x [B, S, C] (CUDA, unit inner stride, uniform row pitch) whose mask [B, S] entry is true become +0.0,
+    as `x.masked_fill(mask[..., None], 0)` would give them (ape_zero_masked_rows); the other rows are not written, so an all-false
+    mask costs its read alone.  Returns x."""
+    _require(x.is_cuda and x.dim() == 3 and x.stride(2) == 1 and x.stride(0) == x.shape[1] * x.stride(1),
+             "zero_masked_rows_: CUDA [B,S,C] with uniform row pitch")
+    _require(tuple(mask.shape) == tuple(x.shape[:2]) and mask.device == x.device, "zero_masked_rows_: mask must be [B,S] on x's device")
+    m = mask.contiguous()
+    m = m.view(torch.uint8) if m.dtype == torch.bool else m.to(torch.uint8)
+    with torch.cuda.device(x.device), _timed(("zero_masked_rows", x.shape[0], x.shape[1], x.shape[2])):
+        rc = _lib.lib.ape_zero_masked_rows(x.data_ptr(), x.stride(1), m.data_ptr(), x.shape[0] * x.shape[1], x.shape[2],
+                                           _lib.dtype_code(x.dtype), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_zero_masked_rows")
+    return x

@@ -552,6 +552,44 @@ int64_t ape_panoptic_pack_workspace_bytes(int K, int num_classes);
 int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things, int stuff_first,
                       double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot, int slot_bytes, void *stream);
 
+/*
+ * Per-image-size geometry of the deformable transformer for a padded batch (DeformableDetrTransformerVL.geometry and the sine
+ * position embedding, deformable_transformer_vl.py:435-477 and the anchor part of :321-353), built on the device from the image
+ * sizes so that one CUDA graph serves every size inside the padded shape.
+ *   sizes         int32 [B, 2] (h, w) in device memory, clamped to [1, Hp] x [1, Wp] (values only, never addresses)
+ *   level_hw      HOST int [L, 2], 1 <= L <= 8, each level inside Hp x Wp; S = sum h_l w_l tokens, levels flattened in order
+ *   dim_t         fp32 [E / 2]: PositionEmbeddingSine's temperature ** (2 * (k // 2) / (E / 2)), computed by the caller; its
+ *                 entries come in equal pairs (dim_t[2m] == dim_t[2m + 1]) and the kernel reads the first of each
+ *   level_embeds  fp32 [L, E]
+ * Level l's padding mask is F.interpolate(mode="nearest") of the pixel mask: row i is valid iff
+ * min(floor(i * ((float)Hp / h_l)), Hp - 1) < h (columns likewise).  Outputs (written completely):
+ *   mask_flatten      bool [B, S]             padded tokens
+ *   pos_lvl           pos_dtype [B, S, E]     (pos + level_embeds[l]) rounded to pos_dtype (fp32 / fp16 / bf16)
+ *   pos_flatten       fp32 [B, S, E] or NULL  pos: channels [0, E/2) from the row sums y, [E/2, E) from the column sums x, each
+ *                                             as (sin, cos) of ((c + offset) / (last + eps) * scale) / dim_t[k] (c alone when
+ *                                             normalize is 0), precise sinf / cosf
+ *   valid_ratios      fp32 [B, L, 2]          (valid columns * (1 / w_l), valid rows * (1 / h_l)): torch divides a tensor by a
+ *                                             scalar as a product with the scalar's fp32 reciprocal
+ *   reference_points  fp32 [B, S, L, 2]       ((j + 0.5) / (ratio_w * w_l), (i + 0.5) / (ratio_h * h_l)) * the ratios of every level
+ *   output_proposals  fp32 [B, S, 4]          log(p / (1 - p)) of ((j + 0.5) / valid_w, (i + 0.5) / valid_h, 0.05 * 2^l, 0.05 * 2^l),
+ *                                             inf where padded or any p outside (0.01, 0.99)
+ *   proposal_invalid  bool [B, S, 1]          padded or outside (0.01, 0.99)
+ * pos_flatten and reference_points 8-byte, output_proposals 16-byte aligned.  One kernel, no allocation, no synchronisation:
+ * capturable in a CUDA graph.  Deterministic; every fp32 operation is the torch code's, in its order.
+ */
+int ape_pad_geometry(const int *sizes, int B, int Hp, int Wp, const int *level_hw, int L, const float *dim_t, const float *level_embeds,
+                     int E, float offset, float eps, float scale, int normalize, uint8_t *mask_flatten, void *pos_lvl, int pos_dtype,
+                     float *pos_flatten, float *valid_ratios, float *reference_points, float *output_proposals,
+                     uint8_t *proposal_invalid, void *stream);
+
+/*
+ * In place: x[r, 0:cols] = +0.0 for every row r < rows with mask[r] != 0 (row pitch ld elements; dtype fp32 / fp16 / bf16).  Rows
+ * whose mask is 0 are not written, so an all-false mask costs its read alone.  Replaces `value.masked_fill(key_padding_mask[..., None],
+ * 0)` of MultiScaleDeformableAttention.forward (ape/layers/multi_scale_deform_attn.py:322-323) on the engine path.  One kernel, no
+ * allocation, no synchronisation: capturable in a CUDA graph.
+ */
+int ape_zero_masked_rows(void *x, int64_t ld, const uint8_t *mask, int64_t rows, int cols, int dtype, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
