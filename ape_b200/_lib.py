@@ -178,6 +178,22 @@ def _declare(lib):
     lib.ape_pad_geometry.argtypes = [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i] + [ctypes.c_float] * 3 + [_i, _vp, _vp, _i] + [_vp] * 6
     lib.ape_zero_masked_rows.restype = _i
     lib.ape_zero_masked_rows.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _vp]
+    lib.ape_mask_pack_dev.restype = _i
+    lib.ape_mask_pack_dev.argtypes = [_vp, _vp, _vp, _i, _vp, _vp] + [_i] * 10 + [_vp]
+    lib.ape_semseg_keys_init_dev.restype = _i
+    lib.ape_semseg_keys_init_dev.argtypes = [_vp, _vp, _i, ctypes.c_float, _i, _i64, _i, _vp, _vp]
+    lib.ape_semseg_resample_dev.restype = _i
+    lib.ape_semseg_resample_dev.argtypes = [_vp, _vp, _vp, _i64] + [_i] * 5 + [_vp, _i, _i64, _i, _i, _i, _vp]
+    lib.ape_gemm_tn_argmax_dev.restype = _i
+    lib.ape_gemm_tn_argmax_dev.argtypes = [_vp, _i64, _vp, _i64, _vp, _i, _vp, _i, _i, _i, _i, _vp]
+    lib.ape_semseg_keys_decode_dev.restype = _i
+    lib.ape_semseg_keys_decode_dev.argtypes = [_vp, _vp, _i, _vp, _vp, _vp]
+    lib.ape_label_rle_pack_dev.restype = _i
+    lib.ape_label_rle_pack_dev.argtypes = [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]
+    lib.ape_panoptic_winners_dev.restype = _i
+    lib.ape_panoptic_winners_dev.argtypes = [_vp] * 5 + [_i] * 5 + [_vp, _i, ctypes.c_float, _i, _vp]
+    lib.ape_panoptic_pack_dev.restype = _i
+    lib.ape_panoptic_pack_dev.argtypes = [_vp] * 3 + [_i] * 4 + [ctypes.c_double, _vp, _i, _vp, _vp, _i, _vp]
 
 
 
@@ -252,6 +268,14 @@ EXPORTS = (
     "ape_panoptic_pack",
     "ape_pad_geometry",
     "ape_zero_masked_rows",
+    "ape_mask_pack_dev",
+    "ape_semseg_keys_init_dev",
+    "ape_semseg_resample_dev",
+    "ape_gemm_tn_argmax_dev",
+    "ape_semseg_keys_decode_dev",
+    "ape_label_rle_pack_dev",
+    "ape_panoptic_winners_dev",
+    "ape_panoptic_pack_dev",
 )
 
 

@@ -107,6 +107,21 @@ __device__ __forceinline__ void stg_stream_v4(uint4 *p, uint4 v) {
                : "memory");
 }
 
+// ---- sizes held on the device (the *_dev entry points of the packed result stages) ------------
+// One image's row (image h, w, output h, w) of an int32 [B, 4] device tensor.  The image is clamped to [1, Hp] x [1, Wp] (the
+// pad), the output to [1, cap] x [1, cap] (the buffers' capacity): a bad size changes values, never addresses.
+struct DevSizes {
+  int ih, iw, oh, ow;
+};
+__device__ __forceinline__ DevSizes dev_sizes(const int *row, int Hp, int Wp, int cap) {
+  DevSizes s;
+  s.ih = min(max(row[0], 1), Hp);
+  s.iw = min(max(row[1], 1), Wp);
+  s.oh = min(max(row[2], 1), cap);
+  s.ow = min(max(row[3], 1), cap);
+  return s;
+}
+
 // ---- class-argmax keys (semantic label maps: gemm_tc.cu EpiArgmax, semseg.cu) ---------------------
 // (order-preserving bits of the fp32 value) << 32 | (0xFFFFFFFF - column): the unsigned maximum of such keys is the largest
 // value and, among equal values, the lowest column, i.e. torch.argmax.  -0 is folded into +0 (argmax compares them equal).

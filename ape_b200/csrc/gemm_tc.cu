@@ -251,8 +251,21 @@ struct EpiArgmax {
   static constexpr bool out32 = true, ln = false, rope = false, stats = false;
   static constexpr int act = ACT_NONE, res = RES_NONE;
 };
+// The same epilogue for a map whose size is on the device (ape_gemm_tn_argmax_dev): M is the capacity, and `residual`, which no
+// argmax epilogue reads, points at the number of rows in use (device int32), so GemmParams and the other kernels stay as they were
+struct EpiArgmaxDev : EpiArgmax {};
 template <class E>
-constexpr bool kArgmax = std::is_same<E, EpiArgmax>::value;
+constexpr bool kArgmax = std::is_same<E, EpiArgmax>::value || std::is_same<E, EpiArgmaxDev>::value;
+template <class E>
+constexpr bool kDevRows = std::is_same<E, EpiArgmaxDev>::value;
+
+// row blocks that hold rows of A: all of them, or (kDevRows) those below the device count at p.residual.  Read after pdl_wait(): a kernel before this
+// one writes the count.
+template <class E>
+__device__ __forceinline__ int live_m_blocks(const GemmParams &p) {
+  if constexpr (kDevRows<E>) return (min(max(*static_cast<const int *>(p.residual), 0), p.M) + BM - 1) / BM;
+  return p.m_blocks;
+}
 
 template <int BN>
 __device__ __forceinline__ void argmax_epilogue(const GemmParams &p, const float *acc, int m_blk, int n_blk, int wg, int lane) {
@@ -298,8 +311,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   // work items: (m group of CL row blocks, n block); CTA `rank` of the cluster takes row block CL*m_group + rank
   const int rank = CL > 1 ? (int)tc::cluster_ctarank() : 0;
-  const int m_groups = (p.m_blocks + CL - 1) / CL;
-  const int num_tiles = m_groups * p.n_blocks;
+  int m_groups = (p.m_blocks + CL - 1) / CL;
+  int num_tiles = m_groups * p.n_blocks;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
   // t-th tile of this CTA: tiles first, first + stride, ... of the (row group, column block) grid, walked in bands of
   // p.band row groups; inside a band the row group changes fastest.  The tiles resident at one time then cover a few row
@@ -329,6 +342,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (CL > 1) tc::cluster_sync_all();  // peer barriers are initialised before any multicast / remote arrive can reach them
   pdl_wait();  // set-up done: operands / residual of the previous kernel may be read, C may be written from here on
   if (threadIdx.x == 0) trace_stamp(p, 1);
+  if constexpr (kDevRows<E>) {
+    m_groups = (live_m_blocks<E>(p) + CL - 1) / CL;
+    num_tiles = m_groups * p.n_blocks;
+  }
 
   if (warp >= kConsumerWarps) {
     // ===================== TMA producer (one thread of the producer warpgroup) =====================
@@ -1042,14 +1059,16 @@ extern "C" int ape_conv3x3_nhwc(const void *x, const void *w, void *y, const flo
 
 // keys[m] = max over n of argmax_key((A W^T)[m, n], n + col_base): the class argmax of every pixel row, merged into keys that
 // the caller initialised (ape_semseg_keys_init).  Single-CTA BN = 128 kernel; K is the padded number of kept queries.
-extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, int N, int K,
-                                  int col_base, int in_dtype, void *stream) {
+// E = EpiArgmaxDev (ape_gemm_tn_argmax_dev): the same over the first *m_dev rows, M being the capacity.
+template <class E>
+static int gemm_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, const int *m_dev, int N, int K,
+                       int col_base, int in_dtype, void *stream) {
   if (in_dtype != APE_DTYPE_F16 && in_dtype != APE_DTYPE_BF16)
     return fail(APE_ERR_INVALID_ARG, "gemm_argmax: operands must be fp16 or bf16 (got dtype %d)", in_dtype);
   if (M < 0 || N <= 0 || K <= 0 || col_base < 0 || (long long)col_base + N > 0x7fffffffLL)
     return fail(APE_ERR_INVALID_ARG, "gemm_argmax: bad sizes M=%d N=%d K=%d col_base=%d", M, N, K, col_base);
   if (M == 0) return APE_OK;
-  if (!A || !W || !keys) return fail(APE_ERR_NULL_PTR, "gemm_argmax: null pointer argument");
+  if (!A || !W || !keys || (kDevRows<E> && !m_dev)) return fail(APE_ERR_NULL_PTR, "gemm_argmax: null pointer argument");
   if ((lda * 2) % 16 || (ldw * 2) % 16 || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15))
     return fail(APE_ERR_INVALID_ARG, "gemm_argmax: A/W base and row pitch must be 16-byte aligned (TMA)");
   if (lda < K || ldw < K) return fail(APE_ERR_INVALID_ARG, "gemm_argmax: row pitch smaller than K");
@@ -1064,13 +1083,28 @@ extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int
   p.k_blocks = (K + BK - 1) / BK;
   p.trace = g_gemm_trace;
   p.argmax_col_base = col_base;
+  p.residual = m_dev;  // EpiArgmaxDev's row count (nullptr otherwise, as before)
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (use_pingpong(p.m_blocks * ((N + bn - 1) / bn))) {
-    if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiArgmax, true>(ma, mb, p, st);
-    return launch_gemm<bn, 6, 1, __half, EpiArgmax, true>(ma, mb, p, st);
+  // the device row count is read by the cooperative kernel's tile walk only, so EpiArgmaxDev always takes that kernel; both
+  // kernels give every key the same MMA sequence and the keys merge by atomicMax, so the keys are the same either way
+  if constexpr (!kDevRows<E>) {
+    if (use_pingpong(p.m_blocks * ((N + bn - 1) / bn))) {
+      if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, E, true>(ma, mb, p, st);
+      return launch_gemm<bn, 6, 1, __half, E, true>(ma, mb, p, st);
+    }
   }
-  if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiArgmax>(ma, mb, p, st);
-  return launch_gemm<bn, 6, 1, __half, EpiArgmax>(ma, mb, p, st);
+  if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, E>(ma, mb, p, st);
+  return launch_gemm<bn, 6, 1, __half, E>(ma, mb, p, st);
+}
+
+extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, int N, int K,
+                                  int col_base, int in_dtype, void *stream) {
+  return gemm_argmax<EpiArgmax>(A, lda, W, ldw, keys, M, nullptr, N, K, col_base, in_dtype, stream);
+}
+
+extern "C" int ape_gemm_tn_argmax_dev(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, const int *m_rows,
+                                      int N, int K, int col_base, int in_dtype, void *stream) {
+  return gemm_argmax<EpiArgmaxDev>(A, lda, W, ldw, keys, M, m_rows, N, K, col_base, in_dtype, stream);
 }
 
 extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,

@@ -33,12 +33,22 @@ constexpr unsigned FULL = 0xffffffffu;
 enum { I_KIND, I_BYTES, I_P, I_M, I_BAD, I_CODES, I_CHARS, I_WORDS = 8 };
 constexpr int KIND_CODES = 1, KIND_MAP = 2, KIND_NONE_FITS = 3;
 
+// ape_label_rle_pack_dev: the map's H x W is the output size of the device size row dims (clamped to [1, cap]); the host's H and W
+// are then the capacity, which sizes the grids and the workspace
+__device__ __forceinline__ void dev_map_size(const int *dims, int cap, int &H, int &W) {
+  if (!dims) return;
+  const DevSizes d = dev_sizes(dims, 1, 1, cap);
+  H = d.oh;
+  W = d.ow;
+}
+
 // boundaries per column and the labels present (a run starts at every first occurrence of a label in column-major order).
 // Labels outside [0, nlab) are flagged in info[I_BAD] and left out of the bitmap.
 __global__ void __launch_bounds__(256) lrle_columns_kernel(const long long *__restrict__ L, int H, int W, int nlab,
                                                            uint32_t *__restrict__ present, int *__restrict__ colb,
-                                                           int *__restrict__ info) {
+                                                           int *__restrict__ info, const int *__restrict__ dims, int cap) {
   pdl_prologue();
+  dev_map_size(dims, cap, H, W);
   const int lane = threadIdx.x & 31;
   const int x = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (x >= W) return;
@@ -69,8 +79,11 @@ __global__ void __launch_bounds__(256) lrle_columns_kernel(const long long *__re
 // of at least 12 P + (2 m + 1 + P) bytes fits `cap`.  sizes (optional) <- P, m, labels out of range.
 __global__ void __launch_bounds__(256) lrle_compact_kernel(const uint32_t *__restrict__ present, const int *__restrict__ colb, int W,
                                                            int p_cap, long long cap, int *__restrict__ index_of,
-                                                           int *__restrict__ label_of, int *__restrict__ info, int *__restrict__ sizes) {
+                                                           int *__restrict__ label_of, int *__restrict__ info, int *__restrict__ sizes,
+                                                           const int *__restrict__ dims, int size_cap) {
   pdl_prologue();
+  int H = 0;
+  dev_map_size(dims, size_cap, H, W);
   __shared__ int s_warp[8];
   constexpr int PER = LRLE_WORDS / 256;
   uint32_t w[PER];
@@ -111,9 +124,11 @@ __global__ void __launch_bounds__(256) lrle_compact_kernel(const uint32_t *__res
 
 // events per (present label, column): the label that starts and, after t = 0, the label that ends at every boundary
 __global__ void __launch_bounds__(256) lrle_count_kernel(const long long *__restrict__ L, int H, int W, const int *__restrict__ index_of,
-                                                         int *__restrict__ cnt, const int *__restrict__ info) {
+                                                         int *__restrict__ cnt, const int *__restrict__ info,
+                                                         const int *__restrict__ dims, int cap) {
   pdl_prologue();
   if (!info[I_CODES]) return;
+  dev_map_size(dims, cap, H, W);
   const int lane = threadIdx.x & 31;
   const int x = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (x >= W) return;
@@ -196,9 +211,11 @@ __global__ void __launch_bounds__(256) lrle_scan_apply_kernel(int *__restrict__ 
 // number of such changes at lower lanes.  A label that ends at lane i is the label of lane i - 1: its mask comes from there.
 __global__ void __launch_bounds__(256) lrle_positions_kernel(const long long *__restrict__ L, int H, int W,
                                                              const int *__restrict__ index_of, int *__restrict__ off,
-                                                             int *__restrict__ pos, const int *__restrict__ info) {
+                                                             int *__restrict__ pos, const int *__restrict__ info,
+                                                             const int *__restrict__ dims, int cap) {
   pdl_prologue();
   if (!info[I_CODES]) return;
+  dev_map_size(dims, cap, H, W);
   const int lane = threadIdx.x & 31;
   const int x = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (x >= W) return;
@@ -255,9 +272,15 @@ __device__ __forceinline__ long long lrle_value(int g, const int *__restrict__ o
 template <bool LEN>
 __global__ void __launch_bounds__(256) lrle_chars_kernel(const int *__restrict__ off, int W, const int *__restrict__ pos, long long HW,
                                                          int *__restrict__ clen, long long ncap, const int *__restrict__ label_of,
-                                                         const int *__restrict__ info, uint8_t *__restrict__ body) {
+                                                         const int *__restrict__ info, uint8_t *__restrict__ body,
+                                                         const int *__restrict__ dims, int cap) {
   pdl_prologue();
   if (LEN ? !info[I_CODES] : info[I_KIND] != KIND_CODES) return;
+  if (dims) {
+    int H = 0;
+    dev_map_size(dims, cap, H, W);
+    HW = (long long)H * W;
+  }
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= ncap) return;
   const int P = info[I_P];
@@ -283,8 +306,14 @@ __global__ void __launch_bounds__(256) lrle_chars_kernel(const int *__restrict__
 
 // kind, bytes and P of the result; a codes body that turned out longer than cap falls back to the map (2 H W bytes) if that
 // fits, else nothing fits: bytes is then the smaller of the two forms (a lower bound for codes that were not built)
-__global__ void lrle_finalize_kernel(int *__restrict__ info, long long HW, long long cap, int map_ok, int *__restrict__ out_info) {
+__global__ void lrle_finalize_kernel(int *__restrict__ info, long long HW, long long cap, int map_ok, int *__restrict__ out_info,
+                                     const int *__restrict__ dims, int size_cap) {
   pdl_prologue();
+  if (dims) {
+    int H = 0, W = 0;
+    dev_map_size(dims, size_cap, H, W);
+    HW = (long long)H * W;
+  }
   const long long P = info[I_P], codes_min = 12 * P + 2LL * info[I_M] + 1 + P;
   const long long codes = info[I_CODES] ? 12 * P + info[I_CHARS] : codes_min;
   int kind, bytes;
@@ -307,9 +336,14 @@ __global__ void lrle_finalize_kernel(int *__restrict__ info, long long HW, long 
 
 // the map as uint16, row-major, when the slot holds it
 __global__ void __launch_bounds__(256) lrle_map_kernel(const long long *__restrict__ L, long long HW, const int *__restrict__ info,
-                                                       uint16_t *__restrict__ out) {
+                                                       uint16_t *__restrict__ out, const int *__restrict__ dims, int cap) {
   pdl_prologue();
   if (info[I_KIND] != KIND_MAP) return;
+  if (dims) {
+    int H = 0, W = 0;
+    dev_map_size(dims, cap, H, W);
+    HW = (long long)H * W;
+  }
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < HW) out[i] = (uint16_t)__ldg(L + i);
 }
@@ -360,44 +394,45 @@ int lrle_scan(int *data, long long n, int *sums, int *total, const int *run, cud
 }
 
 // the first two passes (bitmap, boundaries, compaction); the state block says whether the rest runs
-int lrle_front(const long long *L, int H, int W, int nlab, int p_cap, long long cap, const LrleWs &ws, int *sizes, cudaStream_t st) {
+int lrle_front(const long long *L, int H, int W, int nlab, int p_cap, long long cap, const LrleWs &ws, int *sizes, cudaStream_t st,
+               const int *dims = nullptr) {
   cudaError_t e = cudaMemsetAsync(ws.present, 0, 4LL * LRLE_WORDS, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(ws.info, 0, 4LL * I_WORDS, st);
   if (e != cudaSuccess) return fail((int)e, "label_rle: %s", cudaGetErrorString(e));
   int rc;
-  APE_LAUNCH(lrle_columns_kernel, (W + 7) / 8, 256, 0, st, L, H, W, nlab, ws.present, ws.colb, ws.info);
+  APE_LAUNCH(lrle_columns_kernel, (W + 7) / 8, 256, 0, st, L, H, W, nlab, ws.present, ws.colb, ws.info, dims, W);
   if ((rc = check_launch("lrle_columns_kernel"))) return rc;
   APE_LAUNCH(lrle_compact_kernel, 1, 256, 0, st, (const uint32_t *)ws.present, (const int *)ws.colb, W, p_cap, cap, ws.index_of,
-             ws.label_of, ws.info, sizes);
+             ws.label_of, ws.info, sizes, dims, W);
   return check_launch("lrle_compact_kernel");
 }
 
 // everything after lrle_front: the codes body at `body` if it fits cap, else (map != NULL) the map as uint16 if that fits
 int lrle_rest(const long long *L, int H, int W, int p_cap, long long cap, const LrleWs &ws, uint8_t *body, uint16_t *map, int *out_info,
-              cudaStream_t st) {
+              cudaStream_t st, const int *dims = nullptr) {
   const long long HW = (long long)H * W;
   const int *run = ws.info + I_CODES;
   cudaError_t e = cudaMemsetAsync(ws.off, 0, 4LL * p_cap * W, st);
   if (e != cudaSuccess) return fail((int)e, "label_rle: %s", cudaGetErrorString(e));
   int rc;
   const int col_blocks = (W + 7) / 8;
-  APE_LAUNCH(lrle_count_kernel, col_blocks, 256, 0, st, L, H, W, (const int *)ws.index_of, ws.off, (const int *)ws.info);
+  APE_LAUNCH(lrle_count_kernel, col_blocks, 256, 0, st, L, H, W, (const int *)ws.index_of, ws.off, (const int *)ws.info, dims, W);
   if ((rc = check_launch("lrle_count_kernel"))) return rc;
   if ((rc = lrle_scan(ws.off, (long long)p_cap * W, ws.sums, nullptr, run, st))) return rc;
-  APE_LAUNCH(lrle_positions_kernel, col_blocks, 256, 0, st, L, H, W, (const int *)ws.index_of, ws.off, ws.pos, (const int *)ws.info);
+  APE_LAUNCH(lrle_positions_kernel, col_blocks, 256, 0, st, L, H, W, (const int *)ws.index_of, ws.off, ws.pos, (const int *)ws.info, dims, W);
   if ((rc = check_launch("lrle_positions_kernel"))) return rc;
   const long long blocks = (ws.ncap + 255) / 256;
   APE_LAUNCH((lrle_chars_kernel<true>), blocks, 256, 0, st, (const int *)ws.off, W, (const int *)ws.pos, HW, ws.clen, ws.ncap,
-             (const int *)ws.label_of, (const int *)ws.info, body);
+             (const int *)ws.label_of, (const int *)ws.info, body, dims, W);
   if ((rc = check_launch("lrle_chars_kernel"))) return rc;
   if ((rc = lrle_scan(ws.clen, ws.ncap, ws.sums, ws.info + I_CHARS, run, st))) return rc;
-  APE_LAUNCH(lrle_finalize_kernel, 1, 1, 0, st, ws.info, HW, cap, map ? 1 : 0, out_info);
+  APE_LAUNCH(lrle_finalize_kernel, 1, 1, 0, st, ws.info, HW, cap, map ? 1 : 0, out_info, dims, W);
   if ((rc = check_launch("lrle_finalize_kernel"))) return rc;
   APE_LAUNCH((lrle_chars_kernel<false>), blocks, 256, 0, st, (const int *)ws.off, W, (const int *)ws.pos, HW, ws.clen, ws.ncap,
-             (const int *)ws.label_of, (const int *)ws.info, body);
+             (const int *)ws.label_of, (const int *)ws.info, body, dims, W);
   if ((rc = check_launch("lrle_chars_kernel"))) return rc;
   if (map) {
-    APE_LAUNCH(lrle_map_kernel, (HW + 255) / 256, 256, 0, st, L, HW, (const int *)ws.info, map);
+    APE_LAUNCH(lrle_map_kernel, (HW + 255) / 256, 256, 0, st, L, HW, (const int *)ws.info, map, dims, W);
     if ((rc = check_launch("lrle_map_kernel"))) return rc;
   }
   return APE_OK;
@@ -478,4 +513,25 @@ extern "C" int ape_label_rle_pack(const int64_t *label, int H, int W, int num_la
   int rc = lrle_front((const long long *)label, H, W, num_labels, p_cap, slot, ws, nullptr, st);
   if (rc) return rc;
   return lrle_rest((const long long *)label, H, W, p_cap, slot, ws, out, reinterpret_cast<uint16_t *>(out), out_info, st);
+}
+
+extern "C" int ape_label_rle_pack_dev(const int64_t *label, const int *sizes, int cap, int num_labels, int slot, void *workspace,
+                                      uint8_t *out, int *out_info, void *stream) {
+  if (!label || !sizes || !workspace || !out || !out_info) return fail(APE_ERR_NULL_PTR, "label_rle_pack_dev: null pointer");
+  if (!lrle_geometry_ok(cap, cap))
+    return fail(APE_ERR_INVALID_ARG, "label_rle_pack_dev: capacity %d (at most 2^27 pixels in a capacity x capacity map)", cap);
+  if (num_labels <= 0 || num_labels > LRLE_LABELS)
+    return fail(APE_ERR_INVALID_ARG, "label_rle_pack_dev: num_labels %d outside [1, 65536]", num_labels);
+  if (slot < 16 || slot % 4 != 0) return fail(APE_ERR_INVALID_ARG, "label_rle_pack_dev: slot of %d bytes (a multiple of 4, >= 16)", slot);
+  if ((reinterpret_cast<uintptr_t>(workspace) & 255) || (reinterpret_cast<uintptr_t>(out) & 3))
+    return fail(APE_ERR_INVALID_ARG, "label_rle_pack_dev: workspace must be 256-byte and out 4-byte aligned");
+  int p_cap;
+  const int ev_cap = lrle_pack_caps(num_labels, slot, &p_cap);
+  const LrleWs ws = lrle_ws(workspace, cap, p_cap, ev_cap);
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaMemsetAsync(out, 0, slot, st);
+  if (e != cudaSuccess) return fail((int)e, "label_rle_pack_dev: %s", cudaGetErrorString(e));
+  int rc = lrle_front((const long long *)label, cap, cap, num_labels, p_cap, slot, ws, nullptr, st, sizes);
+  if (rc) return rc;
+  return lrle_rest((const long long *)label, cap, cap, p_cap, slot, ws, out, reinterpret_cast<uint16_t *>(out), out_info, st, sizes);
 }

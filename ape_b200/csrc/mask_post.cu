@@ -162,14 +162,21 @@ __global__ void __launch_bounds__(256) mask_paste_kernel(const uint8_t *__restri
 //   pass 2  the positions j = x * H + y of the boundaries, written in order at the column's offset.
 // Run lengths are the differences of consecutive positions (plus the leading and the trailing run).
 // SKIP: mask n does nothing unless live[n] (its counts and positions are then left unwritten).
+// dims (ape_mask_pack_dev): the output size is dev_sizes(dims) inside the img_h x img_w capacity; columns past it return.
 template <bool WRITE, bool SKIP>
 __global__ void __launch_bounds__(256) mask_rle_kernel(const uint8_t *__restrict__ masks, const float *__restrict__ boxes, int S,
                                                        int img_h, int img_w, float threshold, int *__restrict__ col_count,
                                                        const long long *__restrict__ col_offset, int *__restrict__ positions,
-                                                       const int *__restrict__ live) {
+                                                       const int *__restrict__ live, const int *__restrict__ dims) {
   pdl_prologue();
   if (SKIP && !__ldg(live + blockIdx.y)) return;
   const int n = blockIdx.y, x = blockIdx.x;
+  if (dims) {
+    const DevSizes d = dev_sizes(dims, 1, 1, min(img_h, img_w));
+    img_h = d.oh;
+    img_w = d.ow;
+    if (x >= img_w) return;
+  }
   const float4 b = __ldg(reinterpret_cast<const float4 *>(boxes) + n);
   const uint8_t *m = masks + (size_t)n * S * S;
   long long out0 = 0;
@@ -257,10 +264,12 @@ __global__ void __launch_bounds__(256) mask_pack_prep_kernel(const float *__rest
 // One CTA per slot: exclusive scan of the slot's column counts -> col_offset (the slot's positions start at n * slot), the
 // number of boundaries, and chars[n] = whether they fit: m boundaries make m + 1 counts of at least one character each, so a slot
 // with m >= slot boundaries goes straight to bits and the positions workspace stays at slot int32 per slot.
+// dims: the output width is dev_sizes(dims) within the capacity W.
 __global__ void __launch_bounds__(256) mask_pack_scan_kernel(const int *__restrict__ col_count, const int *__restrict__ live, int W,
                                                              int slot, long long *__restrict__ col_offset, int *__restrict__ total,
-                                                             int *__restrict__ chars) {
+                                                             int *__restrict__ chars, const int *__restrict__ dims) {
   pdl_prologue();
+  if (dims) W = dev_sizes(dims, 1, 1, W).ow;
   const int n = blockIdx.x;
   if (!__ldg(live + n)) {
     if (threadIdx.x == 0) chars[n] = 0;
@@ -288,8 +297,14 @@ __global__ void __launch_bounds__(256) mask_pack_scan_kernel(const int *__restri
 __global__ void __launch_bounds__(256) mask_pack_encode_kernel(const float *__restrict__ rows, const int *__restrict__ live,
                                                                const int *__restrict__ chars, const int *__restrict__ total,
                                                                const int *__restrict__ positions, const uint8_t *__restrict__ masks,
-                                                               int S, int H, int W, int slot, uint8_t *__restrict__ out) {
+                                                               int S, int H, int W, int slot, uint8_t *__restrict__ out,
+                                                               const int *__restrict__ dims) {
   pdl_prologue();
+  if (dims) {  // the output size from the device, within the H x W capacity
+    const DevSizes d = dev_sizes(dims, 1, 1, min(H, W));
+    H = d.oh;
+    W = d.ow;
+  }
   const int n = blockIdx.x, tid = threadIdx.x;
   uint8_t *dst = out + (size_t)n * (PACK_HEAD + slot);
   uint8_t *body = dst + PACK_HEAD;
@@ -409,11 +424,11 @@ extern "C" int ape_mask_paste_rle(const uint8_t *masks, const float *boxes, int 
   if (positions == nullptr) {
     if (!col_count) return fail(APE_ERR_NULL_PTR, "mask_paste_rle: null col_count");
     APE_LAUNCH((mask_rle_kernel<false, false>), dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, col_count,
-               (const long long *)nullptr, (int *)nullptr, (const int *)nullptr);
+               (const long long *)nullptr, (int *)nullptr, (const int *)nullptr, (const int *)nullptr);
   } else {
     if (!col_offset) return fail(APE_ERR_NULL_PTR, "mask_paste_rle: null col_offset");
     APE_LAUNCH((mask_rle_kernel<true, false>), dim3(img_w, N), 256, 0, st, masks, boxes, S, img_h, img_w, threshold, (int *)nullptr,
-               (const long long *)col_offset, positions, (const int *)nullptr);
+               (const long long *)col_offset, positions, (const int *)nullptr, (const int *)nullptr);
   }
   return check_launch("mask_rle_kernel");
 }
@@ -459,10 +474,46 @@ extern "C" int64_t ape_mask_pack_workspace_bytes(int topk, int Hp, int Wp, int m
   return pack_ws(nullptr, topk, Hp, Wp, max_w, S, slot).bytes;
 }
 
-extern "C" int ape_mask_pack(const void *logits, const float *rows, const int *out_hw, void *workspace, uint8_t *out, int B, int topk,
-                             int Q, int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream) {
-  if (B == 0 || topk == 0) return APE_OK;
-  if (!logits || !rows || !out_hw || !workspace || !out) return fail(APE_ERR_NULL_PTR, "mask_pack: null pointer");
+namespace {
+// the 7 launches of one image; dims == nullptr: H x W is the output size, else the capacity and dims the image's device sizes
+int mask_pack_image(const void *lg, const float *r, const int *dims, int H, int W, const PackWs &ws, uint8_t *out, int topk, int h,
+                    int w, int Hp, int Wp, int S, int slot, int dtype, cudaStream_t st) {
+  const int words = (Wp + 31) / 32;
+  const float sh = (float)h / (float)Hp, sw = (float)w / (float)Wp;  // as ape_mask_crop
+  int rc;
+  APE_LAUNCH(mask_pack_prep_kernel, (topk + 255) / 256, 256, 0, st, r, topk, ws.index, ws.crop_box, ws.paste_box, ws.live);
+  if ((rc = check_launch("mask_pack_prep_kernel"))) return rc;
+  const dim3 g1((words + 7) / 8, Hp, topk);
+  if (dtype == APE_DTYPE_F32)
+    APE_LAUNCH((mask_binarize_kernel<float, true>), g1, 256, 0, st, (const float *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
+               Wp, sh, sw, (const int *)ws.live);
+  else if (dtype == APE_DTYPE_F16)
+    APE_LAUNCH((mask_binarize_kernel<__half, true>), g1, 256, 0, st, (const __half *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
+               Wp, sh, sw, (const int *)ws.live);
+  else
+    APE_LAUNCH((mask_binarize_kernel<__nv_bfloat16, true>), g1, 256, 0, st, (const __nv_bfloat16 *)lg, (const long long *)ws.index,
+               ws.bits, h, w, Hp, Wp, sh, sw, (const int *)ws.live);
+  if ((rc = check_launch("mask_binarize_kernel"))) return rc;
+  APE_LAUNCH((mask_roialign_kernel<true>), dim3((S * S + 255) / 256, topk), 256, 0, st, (const uint32_t *)ws.bits,
+             (const float *)ws.crop_box, ws.masks, Hp, Wp, S, (const int *)ws.live);
+  if ((rc = check_launch("mask_roialign_kernel"))) return rc;
+  APE_LAUNCH((mask_rle_kernel<false, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
+             0.5f, ws.col_count, (const long long *)nullptr, (int *)nullptr, (const int *)ws.live, dims);
+  if ((rc = check_launch("mask_rle_kernel"))) return rc;
+  APE_LAUNCH(mask_pack_scan_kernel, topk, 256, 0, st, (const int *)ws.col_count, (const int *)ws.live, W, slot, ws.col_offset,
+             ws.total, ws.chars, dims);
+  if ((rc = check_launch("mask_pack_scan_kernel"))) return rc;
+  APE_LAUNCH((mask_rle_kernel<true, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
+             0.5f, (int *)nullptr, (const long long *)ws.col_offset, ws.positions, (const int *)ws.chars, dims);
+  if ((rc = check_launch("mask_rle_kernel"))) return rc;
+  APE_LAUNCH(mask_pack_encode_kernel, topk, 256, 0, st, r, (const int *)ws.live, (const int *)ws.chars, (const int *)ws.total,
+             (const int *)ws.positions, (const uint8_t *)ws.masks, S, H, W, slot, out, dims);
+  return check_launch("mask_pack_encode_kernel");
+}
+
+int mask_pack_check(const void *logits, const float *rows, const void *workspace, uint8_t *out, int B, int topk, int Q, int h, int w,
+                    int Hp, int Wp, int S, int slot, int dtype) {
+  if (!logits || !rows || !workspace || !out) return fail(APE_ERR_NULL_PTR, "mask_pack: null pointer");
   if (B < 0 || topk < 0 || topk > 65535 || Q <= 0 || h <= 0 || w <= 0 || Hp <= 0 || Wp <= 0 || Hp > 65535 || S <= 0 || S > 1024)
     return fail(APE_ERR_INVALID_ARG, "mask_pack: bad geometry B=%d topk=%d Q=%d %dx%d -> %dx%d, S=%d", B, topk, Q, h, w, Hp, Wp, S);
   if (slot % 4 != 0 || slot < (S * S + 7) / 8)
@@ -471,6 +522,16 @@ extern "C" int ape_mask_pack(const void *logits, const float *rows, const int *o
     return fail(APE_ERR_INVALID_ARG, "mask_pack: rows and out must be 4-byte aligned");
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(APE_ERR_INVALID_ARG, "mask_pack: workspace must be 256-byte aligned");
   if (dtype != APE_DTYPE_F32 && dtype != APE_DTYPE_F16 && dtype != APE_DTYPE_BF16) return fail(APE_ERR_INVALID_ARG, "mask_pack: dtype %d", dtype);
+  return APE_OK;
+}
+}  // namespace
+
+extern "C" int ape_mask_pack(const void *logits, const float *rows, const int *out_hw, void *workspace, uint8_t *out, int B, int topk,
+                             int Q, int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream) {
+  if (B == 0 || topk == 0) return APE_OK;
+  if (!out_hw) return fail(APE_ERR_NULL_PTR, "mask_pack: null pointer");
+  int rc = mask_pack_check(logits, rows, workspace, out, B, topk, Q, h, w, Hp, Wp, S, slot, dtype);
+  if (rc) return rc;
   int max_w = 0;
   for (int b = 0; b < B; ++b) {
     const int oh = out_hw[2 * b], ow = out_hw[2 * b + 1];
@@ -479,43 +540,31 @@ extern "C" int ape_mask_pack(const void *logits, const float *rows, const int *o
     max_w = max(max_w, ow);
   }
   const PackWs ws = pack_ws(workspace, topk, Hp, Wp, max_w, S, slot);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int words = (Wp + 31) / 32;
-  const float sh = (float)h / (float)Hp, sw = (float)w / (float)Wp;  // as ape_mask_crop
   const size_t esize = dtype == APE_DTYPE_F32 ? 4 : 2;
-  int rc;
   for (int b = 0; b < B; ++b) {
-    const int H = out_hw[2 * b], W = out_hw[2 * b + 1];
-    const float *r = rows + (size_t)b * topk * PACK_COLS;
     const void *lg = reinterpret_cast<const char *>(logits) + (size_t)b * Q * h * w * esize;
-    APE_LAUNCH(mask_pack_prep_kernel, (topk + 255) / 256, 256, 0, st, r, topk, ws.index, ws.crop_box, ws.paste_box, ws.live);
-    if ((rc = check_launch("mask_pack_prep_kernel"))) return rc;
-    const dim3 g1((words + 7) / 8, Hp, topk);
-    if (dtype == APE_DTYPE_F32)
-      APE_LAUNCH((mask_binarize_kernel<float, true>), g1, 256, 0, st, (const float *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
-                 Wp, sh, sw, (const int *)ws.live);
-    else if (dtype == APE_DTYPE_F16)
-      APE_LAUNCH((mask_binarize_kernel<__half, true>), g1, 256, 0, st, (const __half *)lg, (const long long *)ws.index, ws.bits, h, w, Hp,
-                 Wp, sh, sw, (const int *)ws.live);
-    else
-      APE_LAUNCH((mask_binarize_kernel<__nv_bfloat16, true>), g1, 256, 0, st, (const __nv_bfloat16 *)lg, (const long long *)ws.index,
-                 ws.bits, h, w, Hp, Wp, sh, sw, (const int *)ws.live);
-    if ((rc = check_launch("mask_binarize_kernel"))) return rc;
-    APE_LAUNCH((mask_roialign_kernel<true>), dim3((S * S + 255) / 256, topk), 256, 0, st, (const uint32_t *)ws.bits,
-               (const float *)ws.crop_box, ws.masks, Hp, Wp, S, (const int *)ws.live);
-    if ((rc = check_launch("mask_roialign_kernel"))) return rc;
-    APE_LAUNCH((mask_rle_kernel<false, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
-               0.5f, ws.col_count, (const long long *)nullptr, (int *)nullptr, (const int *)ws.live);
-    if ((rc = check_launch("mask_rle_kernel"))) return rc;
-    APE_LAUNCH(mask_pack_scan_kernel, topk, 256, 0, st, (const int *)ws.col_count, (const int *)ws.live, W, slot, ws.col_offset,
-               ws.total, ws.chars);
-    if ((rc = check_launch("mask_pack_scan_kernel"))) return rc;
-    APE_LAUNCH((mask_rle_kernel<true, true>), dim3(W, topk), 256, 0, st, (const uint8_t *)ws.masks, (const float *)ws.paste_box, S, H, W,
-               0.5f, (int *)nullptr, (const long long *)ws.col_offset, ws.positions, (const int *)ws.chars);
-    if ((rc = check_launch("mask_rle_kernel"))) return rc;
-    APE_LAUNCH(mask_pack_encode_kernel, topk, 256, 0, st, r, (const int *)ws.live, (const int *)ws.chars, (const int *)ws.total,
-               (const int *)ws.positions, (const uint8_t *)ws.masks, S, H, W, slot, out + (size_t)b * topk * (PACK_HEAD + slot));
-    if ((rc = check_launch("mask_pack_encode_kernel"))) return rc;
+    rc = mask_pack_image(lg, rows + (size_t)b * topk * PACK_COLS, nullptr, out_hw[2 * b], out_hw[2 * b + 1], ws,
+                         out + (size_t)b * topk * (PACK_HEAD + slot), topk, h, w, Hp, Wp, S, slot, dtype, (cudaStream_t)stream);
+    if (rc) return rc;
+  }
+  return APE_OK;
+}
+
+extern "C" int ape_mask_pack_dev(const void *logits, const float *rows, const int *sizes, int cap, void *workspace, uint8_t *out, int B,
+                                 int topk, int Q, int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream) {
+  if (B == 0 || topk == 0) return APE_OK;
+  if (!sizes) return fail(APE_ERR_NULL_PTR, "mask_pack_dev: null pointer");
+  if (cap <= 0 || (long long)cap * cap > 0x7fffffffLL) return fail(APE_ERR_INVALID_ARG, "mask_pack_dev: capacity %d", cap);
+  if (reinterpret_cast<uintptr_t>(sizes) & 15) return fail(APE_ERR_INVALID_ARG, "mask_pack_dev: sizes must be 16-byte aligned");
+  int rc = mask_pack_check(logits, rows, workspace, out, B, topk, Q, h, w, Hp, Wp, S, slot, dtype);
+  if (rc) return rc;
+  const PackWs ws = pack_ws(workspace, topk, Hp, Wp, cap, S, slot);
+  const size_t esize = dtype == APE_DTYPE_F32 ? 4 : 2;
+  for (int b = 0; b < B; ++b) {
+    const void *lg = reinterpret_cast<const char *>(logits) + (size_t)b * Q * h * w * esize;
+    rc = mask_pack_image(lg, rows + (size_t)b * topk * PACK_COLS, sizes + 4 * b, cap, cap, ws, out + (size_t)b * topk * (PACK_HEAD + slot),
+                         topk, h, w, Hp, Wp, S, slot, dtype, (cudaStream_t)stream);
+    if (rc) return rc;
   }
   return APE_OK;
 }

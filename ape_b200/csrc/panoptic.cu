@@ -42,10 +42,22 @@ __global__ void __launch_bounds__(kThreads) panoptic_winners_kernel(const TL *__
                                                                     const float *__restrict__ scores, int *__restrict__ ids,
                                                                     int *__restrict__ counts, int K, int h, int w, float s1h,
                                                                     float s1w, int img_h, int img_w, float s2h, float s2w, int out_h,
-                                                                    int out_w, float prob, int tiles_x, int tiles) {
+                                                                    int out_w, float prob, int tiles_x, int tiles,
+                                                                    const int *__restrict__ dims, int Hp, int Wp) {
   extern __shared__ int hist[];
   for (int i = threadIdx.x; i < 3 * K; i += kThreads) hist[i] = 0;
   pdl_prologue();
+  if (dims) {  // ape_panoptic_winners_dev: sizes from the device, the output within the out_h x out_w capacity
+    const DevSizes d = dev_sizes(dims, Hp, Wp, min(out_h, out_w));
+    img_h = d.ih;
+    img_w = d.iw;
+    out_h = d.oh;
+    out_w = d.ow;
+    s2h = __fdiv_rn((float)img_h, (float)out_h);  // the host's IEEE divisions
+    s2w = __fdiv_rn((float)img_w, (float)out_w);
+    tiles_x = (out_w + kTileW - 1) / kTileW;
+    tiles = tiles_x * ((out_h + kTileH - 1) / kTileH);
+  }
   __syncthreads();
   const int lane = threadIdx.x & 31;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
@@ -92,10 +104,10 @@ __global__ void __launch_bounds__(kThreads) panoptic_winners_kernel(const TL *__
 template <typename TL>
 void launch_winners(int grid, size_t smem, cudaStream_t st, const void *logits, const int64_t *index, const float *scores, int *ids,
                     int *counts, int K, int h, int w, float s1h, float s1w, int img_h, int img_w, float s2h, float s2w, int out_h,
-                    int out_w, float prob, int tiles_x, int tiles) {
+                    int out_w, float prob, int tiles_x, int tiles, const int *dims, int Hp, int Wp) {
   auto kernel = panoptic_winners_kernel<TL>;
   APE_LAUNCH(kernel, grid, kThreads, smem, st, (const TL *)logits, (const long long *)index, scores, ids, counts, K, h, w, s1h, s1w,
-             img_h, img_w, s2h, s2w, out_h, out_w, prob, tiles_x, tiles);
+             img_h, img_w, s2h, s2w, out_h, out_w, prob, tiles_x, tiles, dims, Hp, Wp);
 }
 
 // ---- the panoptic slot ----------------------------------------------------------------------------------------------------
@@ -111,10 +123,16 @@ __global__ void __launch_bounds__(kSegThreads) panoptic_segments_kernel(const in
                                                                         int K, int num_classes, int num_things, int stuff_first,
                                                                         double overlap, int out_h, int out_w, int map_bytes,
                                                                         int *__restrict__ first, int *__restrict__ lut,
-                                                                        int *__restrict__ slot) {
+                                                                        int *__restrict__ slot, const int *__restrict__ dims) {
   __shared__ int s_id[APE_PANOPTIC_MAX_K];  // segment id of every query that opens one
   __shared__ int s_warp[kSegThreads / 32];
   pdl_prologue();
+  if (dims) {  // ape_panoptic_pack_dev: the output size from the device, within the out_h x out_w capacity
+    const DevSizes d = dev_sizes(dims, 1, 1, min(out_h, out_w));
+    out_h = d.oh;
+    out_w = d.ow;
+    map_bytes = 2 * out_h * out_w;
+  }
   for (int c = threadIdx.x; c < num_classes; c += kSegThreads) first[c] = INT_MAX;
   __syncthreads();
   const int k0 = threadIdx.x * kSegPer;
@@ -208,9 +226,15 @@ __device__ __forceinline__ uint32_t paint_pair(const int *__restrict__ ids, cons
 
 // map words w = [0, words) of the slot from its map on (word w = pixels 2w, 2w+1): 16-byte stores from the first 16-byte
 // boundary, single words before it (head < 4) and after the last whole vector
+// dims: HW from the device size row, within the capacity cap x cap
 __global__ void __launch_bounds__(256) panoptic_paint_kernel(const int *__restrict__ ids, const int *__restrict__ lut, long long HW,
-                                                             uint32_t *__restrict__ map, long long words, int head) {
+                                                             uint32_t *__restrict__ map, long long words, int head,
+                                                             const int *__restrict__ dims, int cap) {
   pdl_prologue();
+  if (dims) {
+    const DevSizes d = dev_sizes(dims, 1, 1, cap);
+    HW = (long long)d.oh * d.ow;
+  }
   const long long vecs = (words - head) / 4, tail = head + 4 * vecs;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < vecs; i += (long long)gridDim.x * blockDim.x) {
     const long long w = head + 4 * i;
@@ -232,9 +256,11 @@ __global__ void __launch_bounds__(256) panoptic_paint_kernel(const int *__restri
 
 using namespace ape;
 
-extern "C" int ape_panoptic_winners(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h,
-                                    int w, int Hp, int Wp, int img_h, int img_w, int out_h, int out_w, float prob, int logit_dtype,
-                                    void *stream) {
+namespace {
+// dims == nullptr: the host sizes; else the device size row, out_h x out_w being the capacity (grid and checks)
+int panoptic_winners_run(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h, int w,
+                         int Hp, int Wp, int img_h, int img_w, int out_h, int out_w, float prob, int logit_dtype, const int *dims,
+                         void *stream) {
   if (logit_dtype != APE_DTYPE_F32 && logit_dtype != APE_DTYPE_F16 && logit_dtype != APE_DTYPE_BF16)
     return fail(APE_ERR_INVALID_ARG, "panoptic_winners: logit dtype %d", logit_dtype);
   if (K < 0 || K > APE_PANOPTIC_MAX_K)
@@ -262,12 +288,29 @@ extern "C" int ape_panoptic_winners(const void *logits, const int64_t *index, co
   const size_t smem = (size_t)3 * K * sizeof(int);
 #define APE_PANOPTIC(TL) \
   launch_winners<TL>(grid, smem, st, logits, index, scores, ids, counts, K, h, w, s1h, s1w, img_h, img_w, s2h, s2w, out_h, out_w, prob, \
-                     tiles_x, tiles)
+                     tiles_x, tiles, dims, Hp, Wp)
   if (logit_dtype == APE_DTYPE_F32) APE_PANOPTIC(float);
   else if (logit_dtype == APE_DTYPE_F16) APE_PANOPTIC(__half);
   else APE_PANOPTIC(__nv_bfloat16);
 #undef APE_PANOPTIC
   return check_launch("panoptic_winners_kernel");
+}
+}  // namespace
+
+extern "C" int ape_panoptic_winners(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h,
+                                    int w, int Hp, int Wp, int img_h, int img_w, int out_h, int out_w, float prob, int logit_dtype,
+                                    void *stream) {
+  return panoptic_winners_run(logits, index, scores, ids, counts, K, h, w, Hp, Wp, img_h, img_w, out_h, out_w, prob, logit_dtype,
+                              nullptr, stream);
+}
+
+extern "C" int ape_panoptic_winners_dev(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K,
+                                        int h, int w, int Hp, int Wp, const int *sizes, int cap, float prob, int logit_dtype,
+                                        void *stream) {
+  if (!sizes) return fail(APE_ERR_NULL_PTR, "panoptic_winners_dev: null sizes");
+  if (cap <= 0) return fail(APE_ERR_INVALID_ARG, "panoptic_winners_dev: capacity %d", cap);
+  // the host-side image size only has to pass the checks: the kernel reads the real one
+  return panoptic_winners_run(logits, index, scores, ids, counts, K, h, w, Hp, Wp, 1, 1, cap, cap, prob, logit_dtype, sizes, stream);
 }
 
 namespace {
@@ -280,14 +323,15 @@ extern "C" int64_t ape_panoptic_pack_workspace_bytes(int K, int num_classes) {
   return pan_align(4LL * std::max(num_classes, 1)) + pan_align(4LL * std::max(K, 1));
 }
 
-extern "C" int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things,
-                                 int stuff_first, double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot,
-                                 int slot_bytes, void *stream) {
+namespace {
+int panoptic_pack_run(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things, int stuff_first,
+                      double overlap_threshold, int out_h, int out_w, long long need, void *workspace, uint8_t *slot, int slot_bytes,
+                      const int *dims, int cap, void *stream) {
   if (K < 0 || K > APE_PANOPTIC_MAX_K)
     return fail(APE_ERR_INVALID_ARG, "panoptic_pack: K=%d outside [0, %d]", K, APE_PANOPTIC_MAX_K);
   if (num_classes < 0 || num_things < 0) return fail(APE_ERR_INVALID_ARG, "panoptic_pack: num_classes %d, num_things %d", num_classes, num_things);
   if (out_h <= 0 || out_w <= 0) return fail(APE_ERR_INVALID_ARG, "panoptic_pack: bad output size %dx%d", out_h, out_w);
-  const long long HW = (long long)out_h * out_w, need = 4LL * kSlotHead + 12LL * K + 2 * HW;
+  const long long HW = (long long)out_h * out_w;
   if (slot_bytes < 0 || slot_bytes % 4 != 0 || need > slot_bytes)
     return fail(APE_ERR_INVALID_ARG, "panoptic_pack: slot of %d bytes (a multiple of 4 of at least %lld for K=%d and %dx%d)", slot_bytes,
                 need, K, out_h, out_w);
@@ -298,7 +342,7 @@ extern "C" int ape_panoptic_pack(const int *ids, const int *counts, const int *c
   int *first = reinterpret_cast<int *>(workspace);
   int *lut = reinterpret_cast<int *>(reinterpret_cast<char *>(workspace) + pan_align(4LL * std::max(num_classes, 1)));
   APE_LAUNCH(panoptic_segments_kernel, 1, kSegThreads, 0, st, counts, classes, K, num_classes, num_things, stuff_first ? 1 : 0,
-             overlap_threshold, out_h, out_w, (int)(2 * HW), first, lut, reinterpret_cast<int *>(slot));
+             overlap_threshold, out_h, out_w, (int)std::min(2 * HW, 0x7fffffffLL), first, lut, reinterpret_cast<int *>(slot), dims);
   int rc = check_launch("panoptic_segments_kernel");
   if (rc != APE_OK) return rc;
   uint8_t *map = slot + 4LL * kSlotHead + 12LL * K;
@@ -309,6 +353,25 @@ extern "C" int ape_panoptic_pack(const int *ids, const int *counts, const int *c
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long blocks = ((words - head) / 4 + 255) / 256;
   const int grid = (int)std::max(1LL, std::min(blocks, 8LL * std::max(sms, 1)));
-  APE_LAUNCH(panoptic_paint_kernel, grid, 256, 0, st, ids, (const int *)lut, HW, reinterpret_cast<uint32_t *>(map), words, head);
+  APE_LAUNCH(panoptic_paint_kernel, grid, 256, 0, st, ids, (const int *)lut, HW, reinterpret_cast<uint32_t *>(map), words, head, dims, cap);
   return check_launch("panoptic_paint_kernel");
+}
+}  // namespace
+
+extern "C" int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things,
+                                 int stuff_first, double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot,
+                                 int slot_bytes, void *stream) {
+  const long long need = 4LL * kSlotHead + 12LL * K + 2LL * out_h * out_w;
+  return panoptic_pack_run(ids, counts, classes, K, num_classes, num_things, stuff_first, overlap_threshold, out_h, out_w, need, workspace,
+                           slot, slot_bytes, nullptr, 0, stream);
+}
+
+extern "C" int ape_panoptic_pack_dev(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things,
+                                     int stuff_first, double overlap_threshold, const int *sizes, int cap, void *workspace, uint8_t *slot,
+                                     int slot_bytes, void *stream) {
+  if (!sizes) return fail(APE_ERR_NULL_PTR, "panoptic_pack_dev: null sizes");
+  if (cap <= 0 || (long long)cap * cap > 0x3fffffffLL) return fail(APE_ERR_INVALID_ARG, "panoptic_pack_dev: capacity %d", cap);
+  // the slot must hold the header and the table; a map larger than the rest of the slot is cut at the slot's end
+  return panoptic_pack_run(ids, counts, classes, K, num_classes, num_things, stuff_first, overlap_threshold, cap, cap,
+                           4LL * kSlotHead + 12LL * K, workspace, slot, slot_bytes, sizes, cap, stream);
 }

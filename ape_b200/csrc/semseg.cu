@@ -29,16 +29,11 @@ __device__ __forceinline__ float up_sigmoid(const TL *plane, int w, const Lerp &
   return 1.f / (1.f + expf(-up_value(plane, w, ry, rx)));
 }
 
-// A[(y - row0) * out_w + x, k] for output rows [row0, row0 + rows), k < Kp; thread = one pixel x 8 queries (one 16-byte store)
+// the 8 queries of blockIdx.y at output pixel (y, x) -> one 16-byte store into `row`, the pixel's row of A
 template <typename TL, typename TO>
-__global__ void __launch_bounds__(256) semseg_resample_kernel(const TL *__restrict__ logits, const long long *__restrict__ index,
-                                                              TO *__restrict__ A, long long lda, int K, int h, int w, float s1h,
-                                                              float s1w, int img_h, int img_w, float s2h, float s2w, int out_w,
-                                                              int row0, int rows) {
-  pdl_prologue();
-  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= (long long)rows * out_w) return;
-  const int y = row0 + (int)(pix / out_w), x = (int)(pix % out_w);
+__device__ __forceinline__ void resample_px(const TL *__restrict__ logits, const long long *__restrict__ index, TO *__restrict__ row,
+                                            int K, int h, int w, float s1h, float s1w, int img_h, int img_w, float s2h, float s2w, int y,
+                                            int x) {
   const int k0 = blockIdx.y * 8;
   const Lerp ry = lerp_at(s2h, y, img_h), rx = lerp_at(s2w, x, img_w);  // resize2 over the crop of the padded map
   const Lerp ay0 = lerp_at(s1h, ry.i0, h), ay1 = lerp_at(s1h, ry.i1, h);  // resize1 at the two padded rows it reads
@@ -54,7 +49,37 @@ __global__ void __launch_bounds__(256) semseg_resample_kernel(const TL *__restri
       v[i] = ry.l0 * (rx.l0 * m00 + rx.l1 * m01) + ry.l1 * (rx.l0 * m10 + rx.l1 * m11);
     }
   }
-  *reinterpret_cast<uint4 *>(A + (size_t)pix * lda + k0) = Elem<TO>::pack(v);
+  *reinterpret_cast<uint4 *>(row + k0) = Elem<TO>::pack(v);
+}
+
+// A[(y - row0) * out_w + x, k] for output rows [row0, row0 + rows), k < Kp; thread = one pixel x 8 queries (one 16-byte store)
+template <typename TL, typename TO>
+__global__ void __launch_bounds__(256) semseg_resample_kernel(const TL *__restrict__ logits, const long long *__restrict__ index,
+                                                              TO *__restrict__ A, long long lda, int K, int h, int w, float s1h,
+                                                              float s1w, int img_h, int img_w, float s2h, float s2w, int out_w,
+                                                              int row0, int rows) {
+  pdl_prologue();
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= (long long)rows * out_w) return;
+  resample_px(logits, index, A + (size_t)pix * lda, K, h, w, s1h, s1w, img_h, img_w, s2h, s2w, row0 + (int)(pix / out_w),
+              (int)(pix % out_w));
+}
+
+// The same for a map whose sizes are on the device (ape_semseg_resample_dev): A row i is pixel p0 + i of the row-major
+// out_h x out_w map.  Pixels past the map's end return, so the work follows the real size, not the capacity.
+template <typename TL, typename TO>
+__global__ void __launch_bounds__(256) semseg_resample_dev_kernel(const TL *__restrict__ logits, const long long *__restrict__ index,
+                                                                  TO *__restrict__ A, long long lda, int K, int h, int w, float s1h,
+                                                                  float s1w, int Hp, int Wp, const int *__restrict__ dims, int cap,
+                                                                  long long p0, int n) {
+  pdl_prologue();
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= n) return;
+  const DevSizes d = dev_sizes(dims, Hp, Wp, cap);
+  const long long g = p0 + pix;
+  if (g >= (long long)d.oh * d.ow) return;
+  const float s2h = __fdiv_rn((float)d.ih, (float)d.oh), s2w = __fdiv_rn((float)d.iw, (float)d.ow);  // the host's IEEE divisions
+  resample_px(logits, index, A + (size_t)pix * lda, K, h, w, s1h, s1w, d.ih, d.iw, s2h, s2w, (int)(g / d.ow), (int)(g % d.ow));
 }
 
 __global__ void __launch_bounds__(256) semseg_keys_init_kernel(unsigned long long *__restrict__ keys, long long n,
@@ -63,9 +88,28 @@ __global__ void __launch_bounds__(256) semseg_keys_init_kernel(unsigned long lon
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) keys[i] = key;
 }
 
-__global__ void __launch_bounds__(256) semseg_keys_decode_kernel(const unsigned long long *__restrict__ keys, long long n,
-                                                                 long long *__restrict__ label, float *__restrict__ score) {
+// ape_semseg_keys_init_dev: the keys of the map's out_h x out_w pixels, and the number of those pixels in each band of `band`
+// (the rows the argmax GEMM of that band reads, ape_gemm_tn_argmax_dev)
+__global__ void __launch_bounds__(256) semseg_keys_init_dev_kernel(unsigned long long *__restrict__ keys, const int *__restrict__ dims,
+                                                                   int cap, unsigned long long key, long long band, int nbands,
+                                                                   int *__restrict__ band_rows) {
   pdl_prologue();
+  const DevSizes d = dev_sizes(dims, 1, 1, cap);
+  const long long n = (long long)d.oh * d.ow;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) keys[i] = key;
+  if (blockIdx.x == 0)
+    for (int t = threadIdx.x; t < nbands; t += blockDim.x) band_rows[t] = (int)max(0LL, min(band, n - t * band));
+}
+
+// dims (ape_semseg_keys_decode_dev): n is the map's out_h x out_w from the device, within the capacity n
+__global__ void __launch_bounds__(256) semseg_keys_decode_kernel(const unsigned long long *__restrict__ keys, long long n,
+                                                                 long long *__restrict__ label, float *__restrict__ score,
+                                                                 const int *__restrict__ dims, int cap) {
+  pdl_prologue();
+  if (dims) {
+    const DevSizes d = dev_sizes(dims, 1, 1, cap);
+    n = min(n, (long long)d.oh * d.ow);
+  }
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const unsigned long long k = keys[i];
     label[i] = (long long)(0xFFFFFFFFu - (uint32_t)k);
@@ -144,6 +188,67 @@ extern "C" int ape_semseg_keys_decode(const uint64_t *keys, int64_t n, int64_t *
   if ((reinterpret_cast<uintptr_t>(keys) | reinterpret_cast<uintptr_t>(label)) & 7 || reinterpret_cast<uintptr_t>(score) & 3)
     return fail(APE_ERR_INVALID_ARG, "semseg_keys_decode: misaligned buffers");
   APE_LAUNCH(semseg_keys_decode_kernel, grid_1d(n), 256, 0, (cudaStream_t)stream, (const unsigned long long *)keys, (long long)n,
-             (long long *)label, score);
+             (long long *)label, score, (const int *)nullptr, 0);
+  return check_launch("semseg_keys_decode_kernel");
+}
+
+// ---- device-held sizes ------------------------------------------------------------------------------------------------------
+extern "C" int ape_semseg_resample_dev(const void *logits, const int64_t *index, void *A, int64_t lda, int K, int h, int w, int Hp,
+                                       int Wp, const int *sizes, int cap, int64_t p0, int n, int logit_dtype, int a_dtype, void *stream) {
+  if (logit_dtype != APE_DTYPE_F32 && logit_dtype != APE_DTYPE_F16 && logit_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: logit dtype %d", logit_dtype);
+  if (a_dtype != APE_DTYPE_F16 && a_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: the operand must be fp16 or bf16 (got dtype %d)", a_dtype);
+  if (K <= 0 || h <= 0 || w <= 0 || Hp <= 0 || Wp <= 0 || cap <= 0 || (long long)cap * cap > (1LL << 30) || p0 < 0 || n <= 0 ||
+      p0 + n > (long long)cap * cap)
+    return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: bad geometry K=%d logits %dx%d, padded %dx%d, capacity %d, pixels %lld+%d",
+                K, h, w, Hp, Wp, cap, (long long)p0, n);
+  const int Kp = (K + 7) / 8 * 8;
+  if (Kp / 8 > 65535) return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: K=%d too large", K);
+  if (lda < Kp || lda % 8) return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: row pitch %lld must be >= %d and a multiple of 8", (long long)lda, Kp);
+  if (!logits || !index || !A || !sizes) return fail(APE_ERR_NULL_PTR, "semseg_resample_dev: null pointer");
+  if (reinterpret_cast<uintptr_t>(A) & 15) return fail(APE_ERR_INVALID_ARG, "semseg_resample_dev: A must be 16-byte aligned");
+  const float s1h = (float)h / (float)Hp, s1w = (float)w / (float)Wp;  // area_pixel_compute_scale
+  const dim3 grid((unsigned)((n + 255) / 256), (unsigned)(Kp / 8));
+  cudaStream_t st = (cudaStream_t)stream;
+#define APE_SEMSEG_RESAMPLE_DEV(TL, TO)                                                                                          \
+  APE_LAUNCH((semseg_resample_dev_kernel<TL, TO>), grid, 256, 0, st, (const TL *)logits, (const long long *)index, (TO *)A,     \
+             (long long)lda, K, h, w, s1h, s1w, Hp, Wp, sizes, cap, (long long)p0, n)
+  if (a_dtype == APE_DTYPE_F16) {
+    if (logit_dtype == APE_DTYPE_F32) APE_SEMSEG_RESAMPLE_DEV(float, __half);
+    else if (logit_dtype == APE_DTYPE_F16) APE_SEMSEG_RESAMPLE_DEV(__half, __half);
+    else APE_SEMSEG_RESAMPLE_DEV(__nv_bfloat16, __half);
+  } else {
+    if (logit_dtype == APE_DTYPE_F32) APE_SEMSEG_RESAMPLE_DEV(float, __nv_bfloat16);
+    else if (logit_dtype == APE_DTYPE_F16) APE_SEMSEG_RESAMPLE_DEV(__half, __nv_bfloat16);
+    else APE_SEMSEG_RESAMPLE_DEV(__nv_bfloat16, __nv_bfloat16);
+  }
+#undef APE_SEMSEG_RESAMPLE_DEV
+  return check_launch("semseg_resample_dev_kernel");
+}
+
+extern "C" int ape_semseg_keys_init_dev(uint64_t *keys, const int *sizes, int cap, float value, int column, int64_t band, int nbands,
+                                        int *band_rows, void *stream) {
+  if (cap <= 0 || (long long)cap * cap > (1LL << 30) || column < 0 || band <= 0 || nbands <= 0 || band * nbands < (long long)cap * cap)
+    return fail(APE_ERR_INVALID_ARG, "semseg_keys_init_dev: bad capacity %d, column %d, %d bands of %lld", cap, column, nbands,
+                (long long)band);
+  if (!keys || !sizes || !band_rows) return fail(APE_ERR_NULL_PTR, "semseg_keys_init_dev: null pointer");
+  if (reinterpret_cast<uintptr_t>(keys) & 7) return fail(APE_ERR_INVALID_ARG, "semseg_keys_init_dev: keys must be 8-byte aligned");
+  const float v = value + 0.f;
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  APE_LAUNCH(semseg_keys_init_dev_kernel, grid_1d((long long)cap * cap), 256, 0, (cudaStream_t)stream, (unsigned long long *)keys,
+             sizes, cap, argmax_key_bits(u, (uint32_t)column), (long long)band, nbands, band_rows);
+  return check_launch("semseg_keys_init_dev_kernel");
+}
+
+extern "C" int ape_semseg_keys_decode_dev(const uint64_t *keys, const int *sizes, int cap, int64_t *label, float *score, void *stream) {
+  if (cap <= 0 || (long long)cap * cap > (1LL << 30)) return fail(APE_ERR_INVALID_ARG, "semseg_keys_decode_dev: capacity %d", cap);
+  if (!keys || !sizes || !label || !score) return fail(APE_ERR_NULL_PTR, "semseg_keys_decode_dev: null pointer");
+  if ((reinterpret_cast<uintptr_t>(keys) | reinterpret_cast<uintptr_t>(label)) & 7 || reinterpret_cast<uintptr_t>(score) & 3)
+    return fail(APE_ERR_INVALID_ARG, "semseg_keys_decode_dev: misaligned buffers");
+  const long long n = (long long)cap * cap;
+  APE_LAUNCH(semseg_keys_decode_kernel, grid_1d(n), 256, 0, (cudaStream_t)stream, (const unsigned long long *)keys, n,
+             (long long *)label, score, sizes, cap);
   return check_launch("semseg_keys_decode_kernel");
 }

@@ -306,6 +306,10 @@ class DeformableDETRSegmVL(nn.Module):
         # the panoptic slot per image of `forward_packed`: a 32-byte header, 12 bytes per query of the merge and the map as uint16
         # (ops.panoptic_pack); the default holds any output up to 1024 x 1024 with up to 1024 queries.  A multiple of 4
         self.panoptic_slot_bytes = (1 << 21) + (1 << 14)
+        # None, or an int C: `forward_packed` calls whose image and output sizes all fit C x C run the packed mask / semantic /
+        # panoptic stages on sizes held on the device (ops.*_dev), so `use_cuda_graphs` captures one graph per padded shape and
+        # configuration for them instead of one per combination of sizes.  Larger outputs take the per-size path
+        self.packed_output_capacity = None
         self.semantic_post_nms = semantic_post_nms
         self.panoptic_post_nms = panoptic_post_nms
         self.panoptic_configs = panoptic_configs if panoptic_configs is not None else {
@@ -527,7 +531,7 @@ class DeformableDETRSegmVL(nn.Module):
                 # thresholding touches the host
                 # the final selection (threshold, class-aware NMS, top-k: static shapes) rides in the same graph when boxes are
                 # all that is asked for; its configuration is part of the graph key
-                sel, const = None, (geo, prompt)
+                sel, const, dims = None, (geo, prompt), None
                 # forward_packed with instance masks: the mask stage (csrc/mask_post.cu, ape_mask_pack) follows the selection in
                 # the graph; the output sizes and the slot size join the key
                 # with semantic_on the semantic stage (ape_label_rle_pack) follows too, and its configuration joins the key; so
@@ -544,17 +548,25 @@ class DeformableDETRSegmVL(nn.Module):
                            self.eval_dataset_id, bool(self.instance_on and not (ent and "thing" not in ent)))
                     const = (geo, prompt, sel)
                     if packed_masks or packed_sem or packed_pan:
-                        # the packed mask / semantic / panoptic stages size their grids and workspaces from host ints (ape_mask_pack's
-                        # output sizes and row width, the label-map GEMM and ape_panoptic_winners at the output resolution), so
-                        # their graphs keep the image and output sizes in the key: one graph per combination of sizes
-                        sel += ((tuple(image_sizes), self._output_sizes(batched_inputs, image_sizes),
-                                 int(self.mask_slot_bytes) if packed_masks else None, packed_sem, packed_pan),)
-                        const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
+                        mask_slot = int(self.mask_slot_bytes) if packed_masks else None
+                        cap = self._packed_capacity(batched_inputs, image_sizes)
+                        if cap is None:
+                            # the packed mask / semantic / panoptic stages size their grids and workspaces from host ints (ape_mask_pack's
+                            # output sizes and row width, the label-map GEMM and ape_panoptic_winners at the output resolution), so
+                            # their graphs keep the image and output sizes in the key: one graph per combination of sizes
+                            sel += ((tuple(image_sizes), self._output_sizes(batched_inputs, image_sizes), mask_slot, packed_sem,
+                                     packed_pan),)
+                            const = (geo, prompt, sel, self._size_columns(batched_inputs, image_sizes))
+                        else:
+                            # capacity mode: the stages read the sizes from `dims`, a graph input like `sizes`; the key holds C
+                            sel += ((None, None, mask_slot, packed_sem, packed_pan, cap),)
+                            const = (geo, prompt, sel)
+                            dims = self._dims_tensor(batched_inputs, image_sizes)
                 # the image sizes are a graph input like the image: the key holds the padded shape, not the sizes
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
                     ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel),
-                    self._stage_all, (images, fusion, features_l, sizes), const)
+                    self._stage_all, (images, fusion, features_l, sizes, dims), const)
                 self.transformer.last_topk_proposals = topk
                 mark("encode")
                 mark("select")
@@ -743,7 +755,7 @@ class DeformableDETRSegmVL(nn.Module):
         geo = self._size_geometry(padded, sizes, True)
         return self._stage_encode(images, fusion, geo) + (geo,)
 
-    def _stage_all(self, images, fusion, features_l, sizes, padded, prompt, sel=None, size_columns=None):
+    def _stage_all(self, images, fusion, features_l, sizes, dims, padded, prompt, sel=None, size_columns=None):
         # inside a graph the padding mask is always passed: an all-false mask gives the values of None (masked_fill with no
         # true entry changes nothing), so one graph serves padded and unpadded sizes alike
         geo = self._size_geometry(padded, sizes, True)
@@ -756,10 +768,13 @@ class DeformableDETRSegmVL(nn.Module):
         if sel is not None:  # (class-wise path?, thresholds ..., instance branch on?) — see forward()
             det_cls = self._detector_box_cls(box_cls) if sel[6] else box_cls
             pack = self._select_device(det_cls, box_pred, sizes, sel[0])
-            if size_columns is not None:  # sel[7] = (image sizes, output sizes, mask slot bytes or None, semantic / panoptic configuration)
-                image_sizes, out_sizes, mask_slot, sem, pan = sel[7]
+            if len(sel) > 7:  # sel[7] = (image sizes, output sizes, mask slot bytes or None, semantic / panoptic configuration[, C])
+                image_sizes, out_sizes, mask_slot, sem, pan = sel[7][:5]
+                cap = sel[7][5] if len(sel[7]) > 5 else None
+                if cap is not None:  # capacity mode: the size columns come from the device sizes (exact in fp32)
+                    size_columns = dims.to(torch.float32)
                 pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, tuple(images.shape[-2:]),
-                                       sel[0], out_sizes, mask_slot, sem, pan)
+                                       sel[0], out_sizes, mask_slot, sem, pan, dims=dims, cap=cap)
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                 init_reference, inter_references, mask_logits, pack)
 
@@ -1093,9 +1108,12 @@ class DeformableDETRSegmVL(nn.Module):
             pack = self._select_device(det_cls, box_pred, self._sizes_tensor(image_sizes), bool(getattr(self, "_static_overflowed", False)))
         cols = self._size_columns(batched_inputs, image_sizes, pack.device)
         if masks or sem is not None or pan is not None:
+            # capacity mode runs the kernels the graph runs, so the two agree by construction
+            cap = self._packed_capacity(batched_inputs, image_sizes)
+            dims = self._dims_tensor(batched_inputs, image_sizes) if cap is not None else None
             return self._pack_rows(pack, cols, box_cls, box_pred, mask_pred, self._sizes_tensor(image_sizes), tuple(image_sizes), padded_hw,
                                    bool(getattr(self, "_static_overflowed", False)), self._output_sizes(batched_inputs, image_sizes),
-                                   int(self.mask_slot_bytes) if masks else None, sem, pan)
+                                   int(self.mask_slot_bytes) if masks else None, sem, pan, dims=dims, cap=cap)
         return torch.cat([pack, cols[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
 
     @staticmethod
@@ -1114,6 +1132,29 @@ class DeformableDETRSegmVL(nn.Module):
                 cache.clear()
             extra = cache[(rows, str(device))] = torch.tensor(rows, dtype=torch.float32).to(device)
         return extra
+
+    def _packed_capacity(self, batched_inputs, image_sizes):
+        """model.packed_output_capacity when it is set and every image and output size of the call fits C x C, else None.
+        ValueError for a capacity that is not an int in [1, ops.PACKED_CAPACITY_MAX]."""
+        cap = self.packed_output_capacity
+        if cap is None:
+            return None
+        cap = ops.check_capacity(cap)
+        sizes = list(image_sizes) + list(self._output_sizes(batched_inputs, image_sizes))
+        return cap if all(h <= cap and w <= cap for h, w in sizes) else None
+
+    def _dims_tensor(self, batched_inputs, image_sizes):
+        """(image h, w, output h, w) as int32 [B, 4] on the device, cached per sizes like _sizes_tensor: capacity mode's graph input."""
+        rows = tuple((int(h), int(w), int(oh), int(ow))
+                     for (h, w), (oh, ow) in zip(image_sizes, self._output_sizes(batched_inputs, image_sizes)))
+        key = (rows, str(self.device))
+        cache = self.__dict__.setdefault("_dims_dev", {})
+        dims = cache.get(key)
+        if dims is None:
+            if len(cache) > 64:
+                cache.clear()
+            dims = cache[key] = torch.tensor(rows, dtype=torch.int32, pin_memory=True).to(self.device, non_blocking=True)
+        return dims
 
     def _packed_semantic_config(self):
         """Everything the packed semantic stage reads from the model, as a graph-key tuple: (slot bytes, branch on for the
@@ -1175,14 +1216,18 @@ class DeformableDETRSegmVL(nn.Module):
                                  f"model.panoptic_slot_bytes is {slot}")
 
     def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes,
-                   mask_slot, sem, pan=None):
+                   mask_slot, sem, pan=None, dims=None, cap=None):
         """Selection rows [B, topk, 9] + size columns -> what forward_packed returns: fp32 [B, topk, 13] rows, or uint8
         [B, topk, 60 + mask_slot] with the kept masks' run-length codes (mask_slot not None); with a semantic configuration
         (`_packed_semantic_config`) or a panoptic one (`_packed_panoptic_config`) each image's header, those rows as bytes, its
-        semantic slot (empty without one) and its panoptic slot (none without one).  No host synchronisation."""
+        semantic slot (empty without one) and its panoptic slot (none without one).  No host synchronisation.  With a capacity cap,
+        the stages read the sizes from dims (int32 [B, 4] on the device) and image_sizes / out_sizes are not used."""
         rows = torch.cat([pack, size_columns[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
         if mask_slot is not None:
-            rows = ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, mask_slot)
+            if cap is not None:
+                rows = ops.mask_pack_dev(mask_logits.contiguous(), rows, dims, padded_hw, mask_slot, cap)
+            else:
+                rows = ops.mask_pack(mask_logits.contiguous(), rows, out_sizes, padded_hw, mask_slot)
         if sem is None and pan is None:
             return rows
         B, topk = rows.shape[0], rows.shape[1]
@@ -1195,10 +1240,10 @@ class DeformableDETRSegmVL(nn.Module):
         info = torch.zeros((B, 3), dtype=torch.int32, device=rows.device)  # kind, bytes used, labels present
         if sem is not None:
             self._pack_semantic(sem, out[:, ops.SEM_PACK_HEAD + det.shape[1]:ops.SEM_PACK_HEAD + det.shape[1] + sem_bytes], info, pack,
-                                box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes)
+                                box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes, dims, cap)
         if pan is not None:
             self._pack_panoptic(pan, out[:, out.shape[1] - pan_bytes:], pack, box_cls, box_pred, mask_logits, sizes, image_sizes,
-                                padded_hw, classwise, out_sizes)
+                                padded_hw, classwise, out_sizes, dims, cap)
         hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
         hdr[:, 0], hdr[:, 1] = topk, R
         hdr[:, 2:4] = info[:, 0:2]
@@ -1209,7 +1254,7 @@ class DeformableDETRSegmVL(nn.Module):
         return out
 
     def _pack_semantic(self, sem, slots, info, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise,
-                       out_sizes):
+                       out_sizes, dims=None, cap=None):
         """The semantic slots [B, slot] of `_pack_rows` and their (kind, bytes used, labels present) in info [B, 3]."""
         slot, on, post_nms, class0, things, stuff, entity = sem
         B = slots.shape[0]
@@ -1222,13 +1267,19 @@ class DeformableDETRSegmVL(nn.Module):
                 keep = self._select_device(sem_cls, box_pred, sizes, classwise)
             else:
                 keep = None
+            if cap is not None:
+                labels = torch.stack([self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw,
+                                                                  None, None, class0, dims[b], cap) for b in range(B)])
+                ops.semseg_pack_dev(labels, dims, cap, sem_cls.shape[-1], slots, info)
+                return
             labels = [self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw, image_sizes[b],
                                                   out_sizes[b], class0) for b in range(B)]
             ops.semseg_pack(labels, sem_cls.shape[-1], slots, info)
         else:
             slots.zero_()
 
-    def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes):
+    def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes,
+                       dims=None, cap=None):
         """The panoptic slots [B, slot] of `_pack_rows`: `_panoptic`'s merge with K = topk queries whatever the kept count (every
         query without panoptic_post_nms), no host synchronisation.  The rows of the selection at or past the kept count and the
         queries under object_mask_threshold get the score -inf, so they take no part (ops.panoptic_winners)."""
@@ -1257,15 +1308,21 @@ class DeformableDETRSegmVL(nn.Module):
             scores, labels, kept = _query_scores(box_cls[b, qi].float(), cfg)
             if live is not None:
                 kept = kept & live
-            ids, counts = ops.panoptic_winners(mask_logits[b].contiguous(), qi, torch.where(kept, scores, float("-inf")), padded_hw,
-                                               image_sizes[b], out_sizes[b], prob)
+            scores = torch.where(kept, scores, float("-inf"))
+            if cap is not None:
+                ids, counts = ops.panoptic_winners_dev(mask_logits[b].contiguous(), qi, scores, padded_hw, dims[b], cap, prob)
+                ops.panoptic_pack_dev(ids, counts, labels.to(torch.int32), box_cls.shape[-1], len(things), stuff_first, overlap_threshold,
+                                      dims[b], cap, slots[b])
+                continue
+            ids, counts = ops.panoptic_winners(mask_logits[b].contiguous(), qi, scores, padded_hw, image_sizes[b], out_sizes[b], prob)
             ops.panoptic_pack(ids, counts, labels.to(torch.int32), box_cls.shape[-1], len(things), stuff_first, overlap_threshold,
                               slots[b])
 
-    def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0):
+    def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0, dims=None, cap=None):
         """`_semantic`'s label map of one image with K = topk queries whatever the kept count (no host synchronisation): the
         rows of `keep` ([topk, 9] selection rows, None = every query) at or past the kept count get zero class weights, so the
-        class GEMM adds exact zeros for them."""
+        class GEMM adds exact zeros for them.  With a capacity cap the sizes are dims ([4] on the device) and the map is
+        ops.semseg_label_dev's [cap * cap] buffer."""
         Q = sem_cls.shape[0]
         if keep is None:
             qi, live = torch.arange(Q, device=sem_cls.device), None
@@ -1275,6 +1332,8 @@ class DeformableDETRSegmVL(nn.Module):
         cls = F.softmax(sem_cls[qi].float().sigmoid() / 0.06, dim=-1)
         if live is not None:
             cls = torch.where(live[:, None], cls, cls.new_zeros(()))
+        if cap is not None:
+            return ops.semseg_label_dev(mask_logits.contiguous(), qi, cls.to(self.engine_dtype), padded_hw, dims, cap, class0)
         label, _ = ops.semseg_label(mask_logits.contiguous(), qi, cls.to(self.engine_dtype), padded_hw, size, out_hw, class0)
         return label
 

@@ -1117,6 +1117,169 @@ def panoptic_pack(ids, counts, classes, num_classes, num_things, stuff_first, ov
         _lib.check(rc, "ape_panoptic_pack")
 
 
+# ---- the packed result stages with the sizes held on the device (one CUDA graph for every size up to a capacity) ------------
+# sizes: int32 [B, 4] (image h, w, output h, w) CUDA tensors, or one [4] row; cap: the capacity C.  Maps of out_h x out_w are
+# row-major with pitch out_w at the start of C * C buffers.  The device clamps every size (image to the pad, output to [1, C]).
+PACKED_CAPACITY_MAX = 11585  # C * C <= 2^27, the label codes' bound (ape_label_rle_pack_dev)
+
+
+def check_capacity(cap):
+    """cap as an int in [1, PACKED_CAPACITY_MAX]; ValueError otherwise."""
+    if isinstance(cap, bool) or not isinstance(cap, int) or not 1 <= cap <= PACKED_CAPACITY_MAX:
+        raise ValueError(f"ape_b200: a packed output capacity must be an int in [1, {PACKED_CAPACITY_MAX}] (got {cap!r})")
+    return cap
+
+
+def _size_rows(sizes, dev, B):
+    _require(sizes.is_cuda and sizes.dtype == torch.int32 and sizes.is_contiguous() and sizes.device == dev
+             and tuple(sizes.shape) in ((B, 4),) + (((4,),) if B == 1 else ()),
+             f"device sizes must be a contiguous int32 [{B}, 4] tensor on {dev}")
+
+
+def mask_pack_dev(mask_logits, rows, sizes, padded_hw, slot, cap, mask_size=128):
+    """mask_pack with the output sizes read from sizes int32 [B, 4] on the device (ape_mask_pack_dev): the same bytes for every
+    output size up to cap x cap, with launches sized from cap."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 4 and mask_logits.is_contiguous(), "mask_pack_dev: contiguous CUDA logits [B,Q,h,w]")
+    B, Q, h, w = (int(v) for v in mask_logits.shape)
+    _require(rows.dtype == torch.float32 and rows.is_contiguous() and rows.dim() == 3 and rows.shape[0] == B and rows.shape[2] == 13
+             and rows.device == mask_logits.device, "mask_pack_dev: rows must be contiguous fp32 [B,topk,13] on the logits' device")
+    _size_rows(sizes, mask_logits.device, B)
+    cap = check_capacity(cap)
+    topk, slot, S = int(rows.shape[1]), int(slot), int(mask_size)
+    out = torch.empty((B, topk, MASK_PACK_HEAD + slot), dtype=torch.uint8, device=mask_logits.device)
+    if B == 0 or topk == 0:
+        return out
+    Hp, Wp = int(padded_hw[0]), int(padded_hw[1])
+    ws = torch.empty((max(int(_lib.lib.ape_mask_pack_workspace_bytes(topk, Hp, Wp, cap, S, slot)), 1),), dtype=torch.uint8,
+                     device=mask_logits.device)
+    with torch.cuda.device(mask_logits.device), _timed(("mask_pack_dev", B, topk, Hp, Wp, slot)):
+        rc = _lib.lib.ape_mask_pack_dev(mask_logits.data_ptr(), rows.data_ptr(), sizes.data_ptr(), cap, ws.data_ptr(), out.data_ptr(), B,
+                                        topk, Q, h, w, Hp, Wp, S, slot, _lib.dtype_code(mask_logits.dtype), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_mask_pack_dev")
+    return out
+
+
+def semseg_label_dev(mask_logits, query_index, cls, padded_hw, sizes, cap, class0_const=None, band_bytes=None):
+    """semseg_label with the image and output sizes read from sizes int32 [4] on the device: label int64 [cap * cap] whose first
+    out_h * out_w entries are semseg_label's map, row-major (the rest is not written).  Bands of pixels of the capacity are
+    resampled and contracted as there; the argmax GEMM of a band walks only the row tiles that hold pixels of the map."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 3 and mask_logits.is_contiguous(), "semseg_label_dev: contiguous CUDA logits [Q,h,w]")
+    _require(cls.dim() == 2 and cls.dtype in (torch.float16, torch.bfloat16), "semseg_label_dev: cls must be fp16 / bf16 [K, N]")
+    dev = mask_logits.device
+    _size_rows(sizes, dev, 1)
+    cap = check_capacity(cap)
+    K, N = int(cls.shape[0]), int(cls.shape[1])
+    _require(int(query_index.numel()) == K and N >= 1, "semseg_label_dev: query_index [K] and cls [K, N >= 1] disagree")
+    Hp, Wp = int(padded_hw[0]), int(padded_hw[1])
+    P = cap * cap
+    col_base = 0 if class0_const is None else 1
+    init = (float("-inf"), 0) if class0_const is None else (float(class0_const), 0)
+    if K == 0 and N > col_base and (class0_const is None or float(class0_const) < 0.0):
+        init = (0.0, col_base)  # as semseg_label
+    Kp = (K + 7) // 8 * 8
+    budget = SEMSEG_BAND_BYTES if band_bytes is None else int(band_bytes)
+    band = max(1, min(P, budget // (max(Kp, 8) * 2)))
+    nbands = -(-P // band)
+    keys = torch.empty((P,), dtype=torch.int64, device=dev)
+    label = torch.empty((P,), dtype=torch.int64, device=dev)
+    score = torch.empty((P,), dtype=torch.float32, device=dev)
+    band_rows = torch.empty((nbands,), dtype=torch.int32, device=dev)
+    stream = _lib.current_stream_ptr()
+    with torch.cuda.device(dev), _timed(("semseg_label_dev", K, N, P)):
+        _lib.check(_lib.lib.ape_semseg_keys_init_dev(keys.data_ptr(), sizes.data_ptr(), cap, init[0], init[1], band, nbands,
+                                                     band_rows.data_ptr(), stream), "ape_semseg_keys_init_dev")
+        if K > 0:
+            dt = cls.dtype
+            w = torch.zeros((N - col_base, Kp), dtype=dt, device=dev)
+            w[:, :K] = cls[:, col_base:].t()
+            index = query_index.to(device=dev, dtype=torch.int64).contiguous()
+            ws = torch.empty((band, Kp), dtype=dt, device=dev)
+            for t in range(nbands):
+                p0 = t * band
+                n = min(band, P - p0)
+                rc = _lib.lib.ape_semseg_resample_dev(mask_logits.data_ptr(), index.data_ptr(), ws.data_ptr(), Kp, K, mask_logits.shape[1],
+                                                      mask_logits.shape[2], Hp, Wp, sizes.data_ptr(), cap, p0, n,
+                                                      _lib.dtype_code(mask_logits.dtype), _lib.dtype_code(dt), stream)
+                _lib.check(rc, "ape_semseg_resample_dev")
+                if N > col_base:
+                    rc = _lib.lib.ape_gemm_tn_argmax_dev(ws.data_ptr(), Kp, w.data_ptr(), Kp, keys[p0:].data_ptr(), n,
+                                                         band_rows[t:].data_ptr(), N - col_base, Kp, col_base, _lib.dtype_code(dt), stream)
+                    _lib.check(rc, "ape_gemm_tn_argmax_dev")
+        _lib.check(_lib.lib.ape_semseg_keys_decode_dev(keys.data_ptr(), sizes.data_ptr(), cap, label.data_ptr(), score.data_ptr(), stream),
+                   "ape_semseg_keys_decode_dev")
+    return label
+
+
+def semseg_pack_dev(labels, sizes, cap, num_labels, slots, info):
+    """semseg_pack of device-sized maps (ape_label_rle_pack_dev): labels int64 [B, cap * cap] (semseg_label_dev's layout), sizes
+    int32 [B, 4]; slots and info as semseg_pack."""
+    B = int(labels.shape[0])
+    _require(slots.dim() == 2 and slots.shape[0] == B and slots.dtype == torch.uint8 and slots.stride(1) == 1,
+             "semseg_pack_dev: slots must be uint8 [B, slot] with contiguous rows")
+    _require(info.dtype == torch.int32 and info.is_contiguous() and tuple(info.shape) == (B, 3), "semseg_pack_dev: info int32 [B, 3]")
+    cap = check_capacity(cap)
+    dev = slots.device
+    _require(labels.is_cuda and labels.dtype == torch.int64 and labels.is_contiguous() and tuple(labels.shape) == (B, cap * cap)
+             and labels.device == dev, "semseg_pack_dev: labels must be contiguous CUDA int64 [B, cap * cap] on the slots' device")
+    _size_rows(sizes, dev, B)
+    if B == 0:
+        return
+    slot = int(slots.shape[1])
+    ws = torch.empty((max(int(_lib.lib.ape_label_rle_pack_workspace_bytes(cap, int(num_labels), slot)), 1),), dtype=torch.uint8, device=dev)
+    stream = _lib.current_stream_ptr()
+    with torch.cuda.device(dev), _timed(("semseg_pack_dev", B, slot)):
+        for b in range(B):
+            rc = _lib.lib.ape_label_rle_pack_dev(labels[b].data_ptr(), sizes[b].data_ptr(), cap, int(num_labels), slot, ws.data_ptr(),
+                                                 slots[b].data_ptr(), info[b].data_ptr(), stream)
+            _lib.check(rc, "ape_label_rle_pack_dev")
+
+
+def panoptic_winners_dev(mask_logits, query_index, scores, padded_hw, sizes, cap, prob):
+    """panoptic_winners with the image and output sizes read from sizes int32 [4] on the device: (ids int32 [cap * cap], whose
+    first out_h * out_w entries are panoptic_winners' ids row-major, counts int32 [3, K])."""
+    _require(mask_logits.is_cuda and mask_logits.dim() == 3 and mask_logits.is_contiguous(),
+             "panoptic_winners_dev: contiguous CUDA logits [Q,h,w]")
+    dev = mask_logits.device
+    _size_rows(sizes, dev, 1)
+    cap = check_capacity(cap)
+    K = int(query_index.numel())
+    _require(query_index.dim() == 1 and scores.dim() == 1 and int(scores.numel()) == K,
+             "panoptic_winners_dev: query_index [K] and scores [K] disagree")
+    index = query_index.to(device=dev, dtype=torch.int64).contiguous()
+    sc = scores.to(device=dev, dtype=torch.float32).contiguous()
+    ids = torch.empty((cap * cap,), dtype=torch.int32, device=dev)
+    counts = torch.empty((3, K), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev), _timed(("panoptic_winners_dev", K, cap * cap)):
+        rc = _lib.lib.ape_panoptic_winners_dev(mask_logits.data_ptr(), index.data_ptr(), sc.data_ptr(), ids.data_ptr(), counts.data_ptr(),
+                                               K, mask_logits.shape[1], mask_logits.shape[2], int(padded_hw[0]), int(padded_hw[1]),
+                                               sizes.data_ptr(), cap, float(prob), _lib.dtype_code(mask_logits.dtype),
+                                               _lib.current_stream_ptr())
+        _lib.check(rc, "ape_panoptic_winners_dev")
+    return ids, counts
+
+
+def panoptic_pack_dev(ids, counts, classes, num_classes, num_things, stuff_first, overlap_threshold, sizes, cap, slot):
+    """panoptic_pack of panoptic_winners_dev's (ids, counts) with the output size read from sizes int32 [4] on the device.  The
+    slot must hold the header and the K table rows; the caller checks that the map fits (a longer one is cut at the slot's end)."""
+    cap = check_capacity(cap)
+    _require(ids.is_cuda and ids.dtype == torch.int32 and ids.is_contiguous() and tuple(ids.shape) == (cap * cap,),
+             "panoptic_pack_dev: ids must be CUDA int32 [cap * cap]")
+    K = int(counts.shape[1]) if counts.dim() == 2 else -1
+    _require(counts.dtype == torch.int32 and counts.is_contiguous() and tuple(counts.shape) == (3, K), "panoptic_pack_dev: int32 counts [3, K]")
+    _require(classes.dtype == torch.int32 and classes.is_contiguous() and tuple(classes.shape) == (K,), "panoptic_pack_dev: int32 classes [K]")
+    _require(slot.dtype == torch.uint8 and slot.dim() == 1 and slot.is_contiguous(), "panoptic_pack_dev: contiguous uint8 slot")
+    dev = ids.device
+    _require(counts.device == dev and classes.device == dev and slot.device == dev, "panoptic_pack_dev: all tensors on one device")
+    _size_rows(sizes, dev, 1)
+    n = int(slot.numel())
+    ws = torch.empty((max(int(_lib.lib.ape_panoptic_pack_workspace_bytes(K, int(num_classes))), 1),), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev), _timed(("panoptic_pack_dev", K, cap * cap)):
+        rc = _lib.lib.ape_panoptic_pack_dev(ids.data_ptr(), counts.data_ptr(), classes.data_ptr(), K, int(num_classes), int(num_things),
+                                            1 if stuff_first else 0, float(overlap_threshold), sizes.data_ptr(), cap, ws.data_ptr(),
+                                            slot.data_ptr(), n, _lib.current_stream_ptr())
+        _lib.check(rc, "ape_panoptic_pack_dev")
+
+
 _RESAMPLE_TABLES = {}
 
 

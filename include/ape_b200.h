@@ -553,6 +553,47 @@ int ape_panoptic_pack(const int *ids, const int *counts, const int *classes, int
                       double overlap_threshold, int out_h, int out_w, void *workspace, uint8_t *slot, int slot_bytes, void *stream);
 
 /*
+ * Device-size forms of the packed result stages: the same results as the entry points above, but each image's sizes are read
+ * from device memory, so one CUDA graph serves every image and output size up to a capacity.  sizes is one image's row (or, for
+ * ape_mask_pack_dev, B rows, 16-byte aligned) of an int32 [B, 4] device tensor: image h, w, output h, w.  The image is clamped
+ * to [1, Hp] x [1, Wp] and the output to [1, cap] x [1, cap]: a bad size changes values, never addresses.  Grids and workspaces
+ * are sized from cap on the host; each CTA reads the real sizes and returns past them, so the work follows the real pixels.
+ * Scale factors (img_h / out_h ...) are computed on the device with the host's IEEE fp32 divisions.  Maps of out_h x out_w live
+ * row-major with pitch out_w at the start of cap * cap buffers (label, keys, ids, score).
+ *   ape_mask_pack_dev           ape_mask_pack with the output sizes from sizes [B, 4] (the rows' columns hold the same values);
+ *                               workspace: ape_mask_pack_workspace_bytes(topk, Hp, Wp, cap, S, slot).  cap^2 < 2^31.
+ *   ape_semseg_keys_init_dev    keys [out_h * out_w] <- the key of (value, column); band_rows [nbands] <- the pixels of the map
+ *                               in each band [t * band, (t + 1) * band): min(band, max(0, out_h * out_w - t * band)).  nbands *
+ *                               band >= cap^2, cap^2 <= 2^30.
+ *   ape_semseg_resample_dev     A [n, lda] for pixels [p0, p0 + n) of the row-major map (rows past the map are not written).
+ *   ape_gemm_tn_argmax_dev      ape_gemm_tn_argmax over the first *m_rows rows of A [M, K] (m_rows: device int32, clamped to
+ *                               [0, M]); tiles past them are not walked.  A separate instantiation: the other GEMM kernels are
+ *                               unchanged.
+ *   ape_semseg_keys_decode_dev  label, score [out_h * out_w] from keys.
+ *   ape_label_rle_pack_dev      ape_label_rle_pack of the out_h x out_w map at label; workspace:
+ *                               ape_label_rle_pack_workspace_bytes(cap, num_labels, slot).  cap^2 <= 2^27.
+ *   ape_panoptic_winners_dev    ids [out_h * out_w] (a cap * cap buffer), counts [3, K].
+ *   ape_panoptic_pack_dev       the slot of ape_panoptic_pack from ids [out_h * out_w]; slot_bytes >= 32 + 12 K (the caller checks
+ *                               that the map fits: a longer one is cut at the slot's end).
+ */
+int ape_mask_pack_dev(const void *logits, const float *rows, const int *sizes, int cap, void *workspace, uint8_t *out, int B, int topk,
+                      int Q, int h, int w, int Hp, int Wp, int S, int slot, int dtype, void *stream);
+int ape_semseg_keys_init_dev(uint64_t *keys, const int *sizes, int cap, float value, int column, int64_t band, int nbands, int *band_rows,
+                             void *stream);
+int ape_semseg_resample_dev(const void *logits, const int64_t *index, void *A, int64_t lda, int K, int h, int w, int Hp, int Wp,
+                            const int *sizes, int cap, int64_t p0, int n, int logit_dtype, int a_dtype, void *stream);
+int ape_gemm_tn_argmax_dev(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, const int *m_rows, int N, int K,
+                           int col_base, int in_dtype, void *stream);
+int ape_semseg_keys_decode_dev(const uint64_t *keys, const int *sizes, int cap, int64_t *label, float *score, void *stream);
+int ape_label_rle_pack_dev(const int64_t *label, const int *sizes, int cap, int num_labels, int slot, void *workspace, uint8_t *out,
+                           int *out_info, void *stream);
+int ape_panoptic_winners_dev(const void *logits, const int64_t *index, const float *scores, int *ids, int *counts, int K, int h, int w,
+                             int Hp, int Wp, const int *sizes, int cap, float prob, int logit_dtype, void *stream);
+int ape_panoptic_pack_dev(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things, int stuff_first,
+                          double overlap_threshold, const int *sizes, int cap, void *workspace, uint8_t *slot, int slot_bytes,
+                          void *stream);
+
+/*
  * Per-image-size geometry of the deformable transformer for a padded batch (DeformableDetrTransformerVL.geometry and the sine
  * position embedding, deformable_transformer_vl.py:435-477 and the anchor part of :321-353), built on the device from the image
  * sizes so that one CUDA graph serves every size inside the padded shape.
