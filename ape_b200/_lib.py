@@ -114,6 +114,12 @@ def _declare(lib):
     lib.ape_vlf_pool_workspace_bytes.argtypes = [_i, _i, _i, _i]
     lib.ape_vlf_pool.restype = _i
     lib.ape_vlf_pool.argtypes = [_vp, _vp, _vp, _vp, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(_i)] + [_i] * 6 + [_vp]
+    lib.ape_vlf_fold_vision.restype = _i
+    lib.ape_vlf_fold_vision.argtypes = [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64] + [_i] * 6 + [_vp]
+    lib.ape_vlf_fold_pool_workspace_bytes.restype = _i64
+    lib.ape_vlf_fold_pool_workspace_bytes.argtypes = [_i, _i, _i, _i]
+    lib.ape_vlf_fold_pool.restype = _i
+    lib.ape_vlf_fold_pool.argtypes = [_vp, _i64, _vp, _vp, _vp, _i64] + [_i] * 6 + [_vp]
     lib.ape_nms_workspace_bytes.restype = _i64
     lib.ape_nms_workspace_bytes.argtypes = [_i]
     lib.ape_nms_sorted.restype = _i
@@ -236,6 +242,9 @@ EXPORTS = (
     "ape_groupnorm_nhwc",
     "ape_vlf_pool_workspace_bytes",
     "ape_vlf_pool",
+    "ape_vlf_fold_vision",
+    "ape_vlf_fold_pool_workspace_bytes",
+    "ape_vlf_fold_pool",
     "ape_nms_workspace_bytes",
     "ape_nms_sorted",
     "ape_nms_sorted_dev",

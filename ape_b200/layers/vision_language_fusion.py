@@ -136,11 +136,13 @@ class BiAttentionBlock(nn.Module):
         if v.is_cuda and v.dtype in (torch.float16, torch.bfloat16) and l.shape[1] > 1 and attention_mask_l is None and \
                 not (a.use_attention_mask_v and attention_mask_v is not None) and a.head_dim in (64, 256) and \
                 v.shape[-1] % 8 == 0 and l.shape[-1] % 8 == 0:
-            from .. import ops  # engine: LayerNorm kernel, wgmma GEMMs, two flash-attention passes (forward_engine)
+            from .. import ops  # engine: LayerNorm kernel, then the folded fusion (256-channel vision tokens) or forward_engine
 
             vn = ops.layernorm_module(self.layer_norm_v, v.contiguous())
             with torch.autocast("cuda", enabled=False):
                 ln = self.layer_norm_l(l.float())
+            if self.folds(vn.shape[-1], ln.shape[-1], ln.shape[1]):
+                return self.folded(vn, ln)
             dv, dl = a.forward_engine(vn, ln)
             return vn + self.gamma_v.to(vn.dtype) * dv, ln + self.gamma_l.float() * dl
         v = self.layer_norm_v(v)
@@ -150,6 +152,51 @@ class BiAttentionBlock(nn.Module):
         else:
             dv, dl = self.attn(v, l, attention_mask_v=attention_mask_v, attention_mask_l=attention_mask_l)
         return v + self.gamma_v * dv, l + self.gamma_l * dl
+
+    # The folded path removes three S x v_dim x embed_dim projections but evaluates each head's vision-side softmax in two
+    # passes over the keys once they exceed one block, so its cost grows faster with N than forward_engine's.  On an H100 SXM
+    # (700 W) it is faster up to at least N = 1203 (one fusion layer at 1024^2: 6.1 ms against 7.1 ms) and slower at N = 5000
+    # (bench.py --workload ape_l_d_1536_phrase); forward_engine takes the longer prompts.
+    fold_max_tokens = 1536
+
+    def folds(self, v_dim, l_dim, n_tokens, masked_v=True):
+        """True when a 16-bit CUDA call with n_tokens > 1 unmasked language tokens takes the folded path (`folded`): the
+        engine gate of `forward` with 256-channel vision tokens and at most fold_max_tokens tokens.  masked_v: a vision
+        padding mask is passed (as inside a CUDA graph)."""
+        a = self.attn
+        return a.head_dim in (64, 256) and v_dim == 256 and l_dim % 8 == 0 and n_tokens <= self.fold_max_tokens and \
+            not (a.use_attention_mask_v and masked_v)
+
+    def folded(self, vn, ln):
+        """BiMultiHeadAttention.forward (fuse_helper.py:67-166) for N >= 1 unmasked language tokens, with the language side
+        folded into the 256-dimensional vision space (fold_maps): per layer ONE GEMM maps the LayerNormed tokens to the
+        per-head keys qa, biases qc and values U, and
+          vision side:   out_s = vn_s + gamma_v (sum_h sum_n softmax_n(vn_s . qa[h,n] + qc[h,n]) U[h,n] + b_out_v)
+          language side: pooled[h,n] = sum_s softmax_s(vn_s . qa[h,n]) vn_s  (qc is constant in s and cancels),
+                         delta_l = E pooled + e0.
+        Nothing of width embed_dim is formed over the S vision tokens: no v_proj / values_v_proj / out_v_proj GEMMs.  The
+        +-5e4 clamps and the global-max shift are treated as softmax-invariant translations, as in forward_engine.
+        vn [B,S,256] 16-bit (layer-normed), ln [B,N,l_dim] fp32.  Returns (query [B,S,256] in vn's dtype, l [B,N,l_dim] fp32)."""
+        from .. import ops
+
+        a = self.attn
+        nh, dt = a.num_heads, vn.dtype
+        B, N, L = ln.shape
+        C = vn.shape[-1]
+        Gm, gm0, E, e0 = self._folded_multi_maps(dt)
+        with torch.autocast("cuda", enabled=False):
+            y = ops.linear_tc(ln.to(dt).reshape(B * N, L), Gm, gm0, out_dtype=torch.float32).view(B, N, -1)  # [qa | U | qc]
+            qa = torch.empty((B, nh, N, C), dtype=dt, device=vn.device)
+            qa.copy_(y[..., : nh * C].view(B, N, nh, C).transpose(1, 2))
+            u = torch.empty_like(qa)
+            u.copy_(y[..., nh * C: 2 * nh * C].view(B, N, nh, C).transpose(1, 2))
+            qc = y[..., 2 * nh * C:].transpose(1, 2).contiguous()
+            vn = vn.contiguous()
+            _, bo = ops.packed(a.out_v_proj, dt)
+            out = ops.vlf_fold_vision(vn, qa, u, qc, self.gamma_v.detach().float().contiguous(), bo)
+            pooled = ops.vlf_fold_pool(vn, qa)
+            dl = ops.linear_tc(pooled, E, e0, out_dtype=torch.float32).view(B, N, L)
+        return out, ln + self.gamma_l.float() * dl
 
     def single_token(self, v, l):
         """BiMultiHeadAttention.forward (fuse_helper.py:67-166) for ONE language token — the "name" prompt
@@ -165,37 +212,66 @@ class BiAttentionBlock(nn.Module):
         dl = self.single_token_pool(v, qa, qc)
         return dv.to(v.dtype), dl.to(l.dtype)
 
-    def _folded_language_maps(self):
-        """The one-token case is affine in the language token on both sides, so the chains of small projections are
-        folded once per set of weights (fp64, stored fp32):
-          [qa | qc | delta_v] = ln_l @ G^T + g0     (l_proj -> per-head v_proj^T; l_proj -> v_proj bias; values_l_proj -> out_v_proj)
-          delta_l             = pooled @ E^T + e0   (values_v_proj per head -> out_l_proj)
-        One GEMV each per layer instead of ~25 small kernels; results differ from the op-by-op order by fp32 rounding."""
+    def _fold_params(self):
         a = self.attn
-        params = [a.l_proj.weight, a.l_proj.bias, a.v_proj.weight, a.v_proj.bias, a.values_l_proj.weight, a.values_l_proj.bias,
-                  a.out_v_proj.weight, a.out_v_proj.bias, a.values_v_proj.weight, a.values_v_proj.bias, a.out_l_proj.weight,
-                  a.out_l_proj.bias]
-        key = tuple((t._version, t.data_ptr()) for t in params)
+        return [a.l_proj.weight, a.l_proj.bias, a.v_proj.weight, a.v_proj.bias, a.values_l_proj.weight, a.values_l_proj.bias,
+                a.out_v_proj.weight, a.out_v_proj.bias, a.values_v_proj.weight, a.values_v_proj.bias, a.out_l_proj.weight,
+                a.out_l_proj.bias]
+
+    def fold_maps(self, dtype=torch.float64):
+        """The fusion is affine in each language token on both sides, so the chains of small projections fold (computed in
+        fp64, returned in `dtype`):
+          one token:  [qa | qc | delta_v] = ln_l @ G^T + g0     (l_proj -> per-head v_proj^T; l_proj -> v_proj bias;
+                                                                 values_l_proj -> out_v_proj summed over heads)
+          N tokens:   [qa | U | qc]       = ln_l @ Gm^T + gm0   (the same qa / qc; U[h] = out_v_proj restricted to head h
+                                                                 after values_l_proj: the per-head values in the vision space)
+          both:       delta_l             = pooled @ E^T + e0   (values_v_proj per head -> out_l_proj)
+        qa [nh, v_dim], qc [nh] per token: scores[s, h] = v_s . qa[h] + qc[h]; pooled [nh * v_dim] per token."""
+        a = self.attn
+        nh, hd = a.num_heads, a.head_dim
+        with torch.no_grad():
+            d = lambda t: t.detach().double()
+            wl, bl = d(a.l_proj.weight).view(nh, hd, -1), d(a.l_proj.bias).view(nh, hd)           # [nh,hd,L]
+            wq, bq = d(a.v_proj.weight).view(nh, hd, -1), d(a.v_proj.bias).view(nh, hd)           # [nh,hd,C]
+            A = torch.einsum("hdc,hdj->hcj", wq, wl) * a.scale                                    # [nh,C,L]
+            a0 = torch.einsum("hdc,hd->hc", wq, bl) * a.scale
+            Cm = torch.einsum("hd,hdj->hj", bq, wl) * a.scale                                     # [nh,L]
+            c0 = torch.einsum("hd,hd->h", bq, bl) * a.scale
+            wvl, bvl = d(a.values_l_proj.weight).view(nh, hd, -1), d(a.values_l_proj.bias).view(nh, hd)
+            wov = d(a.out_v_proj.weight).view(-1, nh, hd)                                         # [C,nh,hd]
+            U = torch.einsum("chd,hdj->hcj", wov, wvl)                                            # [nh,C,L]
+            u0 = torch.einsum("chd,hd->hc", wov, bvl)                                             # [nh,C]
+            D = d(a.out_v_proj.weight) @ d(a.values_l_proj.weight)                                # [C,L]
+            d0 = d(a.out_v_proj.weight) @ d(a.values_l_proj.bias) + d(a.out_v_proj.bias)
+            G = torch.cat([A.reshape(-1, A.shape[-1]), Cm, D], 0)
+            g0 = torch.cat([a0.reshape(-1), c0, d0], 0)
+            Gm = torch.cat([A.reshape(-1, A.shape[-1]), U.reshape(-1, U.shape[-1]), Cm], 0)
+            gm0 = torch.cat([a0.reshape(-1), u0.reshape(-1), c0], 0)
+            wvv, bvv = d(a.values_v_proj.weight).view(nh, hd, -1), d(a.values_v_proj.bias)        # [nh,hd,C]
+            wol = d(a.out_l_proj.weight).view(-1, nh, hd)                                         # [L,nh,hd]
+            E = torch.einsum("jhd,hdc->jhc", wol, wvv).reshape(wol.shape[0], -1)
+            e0 = d(a.out_l_proj.weight) @ bvv + d(a.out_l_proj.bias)
+        return tuple(t.to(dtype).contiguous() for t in (G, g0, E, e0, Gm, gm0))
+
+    def _folded_language_maps(self):
+        """fold_maps in fp32, cached per set of weights: (G, g0, E, e0, Gm, gm0).  One GEMV / GEMM each per layer instead of
+        ~25 small kernels; results differ from the op-by-op order by rounding."""
+        key = tuple((t._version, t.data_ptr()) for t in self._fold_params())
         if getattr(self, "_folded", (None,))[0] != key:
-            nh, hd = a.num_heads, a.head_dim
-            with torch.no_grad():
-                d = lambda t: t.detach().double()
-                wl, bl = d(a.l_proj.weight).view(nh, hd, -1), d(a.l_proj.bias).view(nh, hd)           # [nh,hd,L]
-                wq, bq = d(a.v_proj.weight).view(nh, hd, -1), d(a.v_proj.bias).view(nh, hd)           # [nh,hd,C]
-                A = torch.einsum("hdc,hdj->hcj", wq, wl) * a.scale                                    # [nh,C,L]
-                a0 = torch.einsum("hdc,hd->hc", wq, bl) * a.scale
-                Cm = torch.einsum("hd,hdj->hj", bq, wl) * a.scale                                     # [nh,L]
-                c0 = torch.einsum("hd,hd->h", bq, bl) * a.scale
-                D = d(a.out_v_proj.weight) @ d(a.values_l_proj.weight)                                # [C,L]
-                d0 = d(a.out_v_proj.weight) @ d(a.values_l_proj.bias) + d(a.out_v_proj.bias)
-                G = torch.cat([A.reshape(-1, A.shape[-1]), Cm, D], 0).float().contiguous()
-                g0 = torch.cat([a0.reshape(-1), c0, d0], 0).float().contiguous()
-                wvv, bvv = d(a.values_v_proj.weight).view(nh, hd, -1), d(a.values_v_proj.bias)        # [nh,hd,C]
-                wol = d(a.out_l_proj.weight).view(-1, nh, hd)                                         # [L,nh,hd]
-                E = torch.einsum("jhd,hdc->jhc", wol, wvv).reshape(wol.shape[0], -1).float().contiguous()
-                e0 = (d(a.out_l_proj.weight) @ bvv + d(a.out_l_proj.bias)).float().contiguous()
-            self._folded = (key, G, g0, E, e0)
+            self._folded = (key,) + self.fold_maps(torch.float32)
         return self._folded[1:]
+
+    def _folded_multi_maps(self, dtype):
+        """(Gm, gm0, E, e0) for the N-token GEMMs: weights in the engine dtype, biases fp32; one copy per dtype (ops.cached)."""
+        from .. import ops
+
+        key = tuple((t._version, t.data_ptr()) for t in self._fold_params())
+
+        def build():
+            _, _, E, e0, Gm, gm0 = self._folded_language_maps()
+            return Gm.to(dtype).contiguous(), gm0, E.to(dtype).contiguous(), e0
+
+        return ops.cached(self, "_ape_fold_multi", dtype, key, build)
 
     def single_token_language_side(self, l):
         """Everything of the one-token case that depends on the language token only: delta_v [B,1,v_dim] and the
@@ -204,7 +280,7 @@ class BiAttentionBlock(nn.Module):
         nh, hd = a.num_heads, a.head_dim
         if l.is_cuda and self.fold_language_side:
             with torch.autocast("cuda", enabled=False):
-                G, g0, _, _ = self._folded_language_maps()
+                G, g0 = self._folded_language_maps()[:2]
                 B = l.shape[0]
                 from .. import ops
 
@@ -249,7 +325,7 @@ class BiAttentionBlock(nn.Module):
             if shift is not None:
                 pooled = pooled - shift.reshape(B, 1, -1).float()
             if v.is_cuda and self.fold_language_side:
-                _, _, E, e0 = self._folded_language_maps()
+                E, e0 = self._folded_language_maps()[2:4]
                 from .. import ops
 
                 return ops.gemv_f32(pooled.reshape(B, 1, -1).contiguous(), E, e0)

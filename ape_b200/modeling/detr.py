@@ -11,6 +11,7 @@ ape/modeling/ape_deta/ape_deta.py:20-40 (`SomeThing`).  Same constructor keyword
 
 Scope (SURVEY.md §8): inference (boxes, instance masks, semantic and panoptic maps) for "name", "phrase" / "text" and
 "expression" prompts.  Training and mask prompts raise NotImplementedError (next rows of §8f) — loudly, never silently."""
+import collections
 import copy
 import math
 from typing import Dict, List
@@ -342,8 +343,6 @@ class DeformableDETRSegmVL(nn.Module):
         self.engine_dtype = torch.float32
         self.profile_stages = False   # record CUDA-event stage times of the last forward in self.stage_ms
         self.use_cuda_graphs = False  # capture the static stages once per padded shape and prompt configuration (16-bit engine mode)
-        import collections
-
         self._geo_cache, self._graph_cache = {}, collections.OrderedDict()
         self.graph_cache_size = 8  # captured graphs kept (LRU)
         # static-shape final selection (one host sync per batch) for up to this many (query, class) pairs above the
@@ -524,6 +523,9 @@ class DeformableDETRSegmVL(nn.Module):
         mask_prompt_flatten = self._mask_prompt(batched_inputs, images.shape, geo) if "mask_prompt" in batched_inputs[0] else None
         graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion) and mask_prompt_flatten is None
         need_masks = self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)
+        if graphs and fusion is not None and fusion.shape[1] > 1:
+            graphs = self._graph_seen((prompt, tuple(images.shape), tuple(features_l.shape), self.engine_dtype, need_masks,
+                                       do_postprocess, self.profile_stages))
         with torch.autocast("cuda", dtype=self.engine_dtype, enabled=low):
             if graphs and not self.profile_stages:
                 # encode -> select -> decode in ONE graph: the selection is written with static shapes and no host
@@ -735,11 +737,30 @@ class DeformableDETRSegmVL(nn.Module):
             mask_features = self.maskdino_mask_features(memory, features, geo)
         return memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features
 
-    @staticmethod
-    def _graph_prompt(prompt, fusion):
-        """Prompts whose step is captured in a CUDA graph: one fusion token ("name" prompts), so the encoder's launch sequence
-        does not depend on the text."""
-        return fusion is not None and fusion.shape[1] == 1
+    def _graph_prompt(self, prompt, fusion):
+        """Prompts whose step is captured in a CUDA graph, because the encoder's launch sequence does not depend on the text:
+        one fusion token ("name" prompts), or several (phrase, expression and fused-vocabulary prompts) when every fusion
+        layer takes the folded path (BiAttentionBlock.folds), whose launches depend on the token count alone; the graph key
+        holds that count through the shape of the text features."""
+        if fusion is None:
+            return False
+        if fusion.shape[1] == 1:
+            return True
+        enc = self.transformer.encoder
+        return all(vl is None or vl.b_attn.folds(enc.embed_dim, fusion.shape[-1], fusion.shape[1]) for vl in enc.vl_layers)
+
+    def _graph_seen(self, key):
+        """Multi-token prompts: True the second time `key` is seen.  A new token count costs two eager warm-ups and a capture,
+        which an interactive session whose text changes on every call would pay every time; so the first call of a key runs
+        eagerly, as an uncaptured prompt does, and the capture waits for a repeat.  Bounded (LRU) like the graph cache."""
+        seen = self.__dict__.setdefault("_graph_seen_keys", collections.OrderedDict())
+        if key in seen:
+            seen.move_to_end(key)
+            return True
+        seen[key] = None
+        while len(seen) > 64:
+            seen.popitem(last=False)
+        return False
 
     @staticmethod
     def _mix_text(prompt, features_l, fusion_out):

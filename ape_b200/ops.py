@@ -653,6 +653,50 @@ def vlf_pool(v, qa, qc, stable_softmax_2d=True):
     return part[..., :C] / part[..., C:]
 
 
+def _check_fold_operands(v, qa, name):
+    _require(v.is_cuda and v.dim() == 3 and v.shape[-1] == 256 and v.dtype in (torch.float16, torch.bfloat16) and
+             v.stride(2) == 1 and v.stride(0) == v.shape[1] * v.stride(1), f"{name}: v must be CUDA fp16/bf16 [B,S,256] with rows of one pitch")
+    B = v.shape[0]
+    _require(qa.is_cuda and qa.dtype == v.dtype and qa.dim() == 4 and qa.shape[0] == B and qa.shape[3] == 256 and qa.is_contiguous(),
+             f"{name}: qa must be contiguous [B,NH,N,256] in the dtype of v")
+    return B, v.shape[1], qa.shape[2], qa.shape[1]
+
+
+def vlf_fold_vision(v, qa, u, qc, gamma, bias, out=None):
+    """v + gamma * (sum_h sum_n softmax_n(v . qa[:,h,n] + qc[:,h,n]) u[:,h,n] + bias) over all S rows (ape_vlf_fold_vision).
+    v [B,S,256] fp16/bf16; qa / u [B,NH,N,256] contiguous, dtype of v; qc fp32 [B,NH,N]; gamma / bias fp32 [256].
+    Returns [B,S,256] in the dtype of v (`out` may be given, v itself included)."""
+    B, S, N, NH = _check_fold_operands(v, qa, "vlf_fold_vision")
+    _require(u.shape == qa.shape and u.dtype == v.dtype and u.is_contiguous(), "vlf_fold_vision: u must be like qa")
+    _require(qc.dtype == torch.float32 and qc.is_contiguous() and tuple(qc.shape) == (B, NH, N), "vlf_fold_vision: qc fp32 [B,NH,N]")
+    for t in (gamma, bias):
+        _require(t.dtype == torch.float32 and t.is_contiguous() and t.numel() == 256, "vlf_fold_vision: gamma / bias fp32 [256]")
+    if out is None:
+        out = torch.empty((B, S, 256), dtype=v.dtype, device=v.device)
+    _require(out.shape == v.shape and out.dtype == v.dtype and out.stride(2) == 1 and out.stride(0) == S * out.stride(1),
+             "vlf_fold_vision: bad `out`")
+    with torch.cuda.device(v.device), _timed(("vlf_fold_vision", B, S, N, NH)):
+        rc = _lib.lib.ape_vlf_fold_vision(v.data_ptr(), v.stride(1), qa.data_ptr(), u.data_ptr(), qc.data_ptr(), gamma.data_ptr(),
+                                          bias.data_ptr(), out.data_ptr(), out.stride(1), B, S, N, NH, 256, _lib.dtype_code(v.dtype),
+                                          _lib.current_stream_ptr())
+    _lib.check(rc, "ape_vlf_fold_vision")
+    return out
+
+
+def vlf_fold_pool(v, qa):
+    """sum_s softmax_s(v_s . qa[:,h,n]) v_s for every head h and token n (ape_vlf_fold_pool: S split across the SMs, the chunks
+    combined in a fixed order).  v [B,S,256] fp16/bf16, qa [B,NH,N,256] contiguous in the dtype of v.
+    Returns [B*N, NH*256] in the dtype of v (row b*N + n, head h at columns h*256)."""
+    B, S, N, NH = _check_fold_operands(v, qa, "vlf_fold_pool")
+    pooled = torch.empty((B * N, NH * 256), dtype=v.dtype, device=v.device)
+    ws = torch.empty((int(_lib.lib.ape_vlf_fold_pool_workspace_bytes(B, S, N, NH)) // 4,), dtype=torch.float32, device=v.device)
+    with torch.cuda.device(v.device), _timed(("vlf_fold_pool", B, S, N, NH)):
+        rc = _lib.lib.ape_vlf_fold_pool(v.data_ptr(), v.stride(1), qa.data_ptr(), ws.data_ptr(), pooled.data_ptr(), pooled.stride(0),
+                                        B, S, N, NH, 256, _lib.dtype_code(v.dtype), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_vlf_fold_pool")
+    return pooled
+
+
 def nms_sorted_mask(sorted_boxes, iou_threshold, n_valid=None):
     """Greedy NMS over boxes ALREADY sorted by descending score: uint8 keep mask [n] (static shape, no host
     synchronisation: usable inside CUDA-graph capture) and the int32 [1] number of survivors.

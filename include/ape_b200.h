@@ -360,6 +360,28 @@ int ape_vlf_pool(const void *v, const float *qa, const float *qc, void *workspac
                  int B, int S, int C, int NH, int stable_softmax_2d, int dtype, void *stream);
 
 /*
+ * VisionLanguageFusion for N >= 1 language tokens in the folded form (phrase / expression / fused-vocabulary prompts;
+ * csrc/vlf_fold.cu).  The language side is folded per head h and token n into 256-vectors of the vision space: keys
+ * qa [B, NH, N, 256] and values U [B, NH, N, 256] (16-bit, contiguous), per-key biases qc [B, NH, N] fp32.  v [B*S, 256] 16-bit
+ * with row pitch ldv (the LayerNormed vision tokens).  The reference's global-max shift and +-5e4 clamps are treated as
+ * softmax-invariant, as in ape_attn_cross_fwd.
+ *
+ * ape_vlf_fold_vision: out_s = v_s + gamma * (sum_h sum_n softmax_n(v_s . qa[h,n] + qc[h,n]) U[h,n] + bias), each head
+ * normalised exactly, fp32 accumulation, one rounding to the dtype of v.  gamma / bias fp32 [256]; out [B*S, 256] with row
+ * pitch ldo (may be v itself).  C must be 256.
+ *
+ * ape_vlf_fold_pool: pooled[b*N + n, h*256 + c] = sum_s softmax_s(v_s . qa[h,n]) v_s[c] (16-bit, row pitch ldp >= NH*256).
+ * The S tokens of an image are split into chunks across the SMs; the chunks' partials are combined in a fixed order, so the
+ * result is deterministic.  workspace: ape_vlf_fold_pool_workspace_bytes(B, S, N, NH) bytes, 16-byte aligned.
+ * Both: no allocation, no synchronisation, graph-capturable.
+ */
+int ape_vlf_fold_vision(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
+                        const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, int C, int dtype, void *stream);
+int64_t ape_vlf_fold_pool_workspace_bytes(int B, int S, int N, int NH);
+int ape_vlf_fold_pool(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B, int S, int N,
+                      int NH, int C, int dtype, void *stream);
+
+/*
  * Greedy hard NMS over boxes already sorted by descending score (torchvision.ops.nms semantics; replaces the
  * nms call inside batched_nms of deformable_transformer_vl.py:591-596 and fast_rcnn.py:192).
  * boxes_sorted [n,4] fp32 xyxy (16-byte aligned); keep [n] bytes (1 = survives); *count = survivors (device int).
