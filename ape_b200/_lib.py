@@ -184,6 +184,10 @@ def _declare(lib):
     lib.ape_pad_geometry.argtypes = [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i] + [ctypes.c_float] * 3 + [_i, _vp, _vp, _i] + [_vp] * 6
     lib.ape_zero_masked_rows.restype = _i
     lib.ape_zero_masked_rows.argtypes = [_vp, _i64, _vp, _i64, _i, _i, _vp]
+    lib.ape_region_prompt_empty.restype = _i
+    lib.ape_region_prompt_empty.argtypes = [_vp, _i64, _vp, _vp]
+    lib.ape_region_prompt.restype = _i
+    lib.ape_region_prompt.argtypes = [_vp, _i, _i, _i, _vp, _i] + [_vp] * 7
     lib.ape_mask_pack_dev.restype = _i
     lib.ape_mask_pack_dev.argtypes = [_vp, _vp, _vp, _i, _vp, _vp] + [_i] * 10 + [_vp]
     lib.ape_semseg_keys_init_dev.restype = _i
@@ -277,6 +281,8 @@ EXPORTS = (
     "ape_panoptic_pack",
     "ape_pad_geometry",
     "ape_zero_masked_rows",
+    "ape_region_prompt_empty",
+    "ape_region_prompt",
     "ape_mask_pack_dev",
     "ape_semseg_keys_init_dev",
     "ape_semseg_resample_dev",

@@ -150,6 +150,68 @@ __global__ void __launch_bounds__(kThreads) zero_masked_rows_kernel(T *__restric
   for (int c = threadIdx.x % 32; c < cols; c += 32) row[c] = T(0);
 }
 
+// Phase one of the region prompt: *empty is 1 on entry (set by the launcher); any CTA that finds a set byte of the map writes 0.
+// Every writer writes the same value, so the result does not depend on the order.
+__global__ void __launch_bounds__(kThreads) region_empty_kernel(const uint8_t *__restrict__ map, long long n, uint8_t *__restrict__ empty) {
+  ape::pdl_prologue();
+  const long long n16 = n / 16, stride = (long long)gridDim.x * kThreads;
+  bool set = false;
+  const uint4 *v = reinterpret_cast<const uint4 *>(map);
+  for (long long k = (long long)blockIdx.x * kThreads + threadIdx.x; k < n16; k += stride) {
+    const uint4 q = v[k];
+    set |= (q.x | q.y | q.z | q.w) != 0u;
+  }
+  for (long long k = n16 * 16 + (long long)blockIdx.x * kThreads + threadIdx.x; k < n; k += stride) set |= map[k] != 0;
+  if (__syncthreads_or(set) && threadIdx.x == 0) *empty = 0;
+}
+
+struct RegionLevels {
+  int h[kMaxLevels], w[kMaxLevels], start[kMaxLevels];
+  float sh[kMaxLevels], sw[kMaxLevels];  // (float)Hp / h_l and (float)Wp / w_l, divided on the host (IEEE, as torch's host code)
+  int L, S;
+};
+
+// The two source taps of destination index d along one axis of F.interpolate(mode="bilinear", align_corners=False), with the
+// fp32 operations of torch's CUDA kernel (upsample_bilinear2d_out_frame: FADD d + 0.5, FFMA by the scale minus 0.5, clamp at 0,
+// truncate, lambda = src - index): the first tap always has a nonzero weight (1 - lambda > 0); the second counts when lambda is
+// nonzero, and is the first again at the last source row or column.
+__device__ __forceinline__ void bilinear_taps(int d, float scale, int n_in, int &t0, int &t1) {
+  float src = __fmaf_rn((float)d + 0.5f, scale, -0.5f);
+  src = src < 0.f ? 0.f : src;
+  const int i = min((int)src, n_in - 1);
+  const float lambda = src - (float)i;
+  t0 = i;
+  t1 = lambda != 0.f && i < n_in - 1 ? i + 1 : i;
+}
+
+// One thread per token: region = the whole batch is empty, or a tap with nonzero weight reads a set byte of the image's map.
+__global__ void __launch_bounds__(kThreads) region_prompt_kernel(const uint8_t *__restrict__ map, int Hp, int Wp, RegionLevels lv,
+                                                                 const uint8_t *__restrict__ empty,
+                                                                 const float *__restrict__ output_proposals,
+                                                                 const uint8_t *__restrict__ proposal_invalid,
+                                                                 float *__restrict__ out_proposals, uint8_t *__restrict__ out_invalid,
+                                                                 uint8_t *__restrict__ region) {
+  ape::pdl_prologue();
+  const int s = blockIdx.x * kThreads + threadIdx.x, b = blockIdx.y;
+  if (s >= lv.S) return;
+  int l = 0;
+  while (l + 1 < lv.L && s >= lv.start[l + 1]) ++l;
+  const int i = (s - lv.start[l]) / lv.w[l], j = (s - lv.start[l]) % lv.w[l];
+  bool in = *empty != 0;
+  if (!in) {
+    int r0, r1, c0, c1;
+    bilinear_taps(i, lv.sh[l], Hp, r0, r1);
+    bilinear_taps(j, lv.sw[l], Wp, c0, c1);
+    const uint8_t *m = map + (long long)b * Hp * Wp;
+    in = (m[(long long)r0 * Wp + c0] | m[(long long)r0 * Wp + c1] | m[(long long)r1 * Wp + c0] | m[(long long)r1 * Wp + c1]) != 0;
+  }
+  const long long bs = (long long)b * lv.S + s;
+  const float4 p = reinterpret_cast<const float4 *>(output_proposals)[bs];
+  reinterpret_cast<float4 *>(out_proposals)[bs] = in ? p : make_float4(INFINITY, INFINITY, INFINITY, INFINITY);
+  out_invalid[bs] = proposal_invalid[bs] | !in;
+  if (region) region[bs] = in;
+}
+
 }  // namespace
 
 using namespace ape;
@@ -218,4 +280,53 @@ extern "C" int ape_zero_masked_rows(void *x, int64_t ld, const uint8_t *mask, in
   else
     return fail(APE_ERR_UNSUPPORTED, "zero_masked_rows: dtype %d (fp32 / fp16 / bf16 only)", dtype);
   return check_launch("zero_masked_rows_kernel");
+}
+
+extern "C" int ape_region_prompt_empty(const uint8_t *map, int64_t n, uint8_t *empty, void *stream) {
+  if (n < 0) return fail(APE_ERR_INVALID_ARG, "region_prompt_empty: n=%lld", (long long)n);
+  if (!empty || (n > 0 && !map)) return fail(APE_ERR_NULL_PTR, "region_prompt_empty: null pointer");
+  if (reinterpret_cast<uintptr_t>(map) & 15) return fail(APE_ERR_INVALID_ARG, "region_prompt_empty: map must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaMemsetAsync(empty, 1, 1, st);
+  if (e != cudaSuccess) return fail((int)e, "region_prompt_empty: %s", cudaGetErrorString(e));
+  if (n == 0) return APE_OK;
+  // 16 bytes per thread and pass; enough CTAs to fill the SMs a few times over, fewer for a small map
+  const long long per_cta = 16LL * kThreads * 4;
+  const long long ctas = (n + per_cta - 1) / per_cta;
+  const unsigned grid = (unsigned)(ctas < 1024 ? ctas : 1024);
+  APE_LAUNCH(region_empty_kernel, grid, kThreads, 0, st, map, (long long)n, empty);
+  return check_launch("region_empty_kernel");
+}
+
+extern "C" int ape_region_prompt(const uint8_t *map, int B, int Hp, int Wp, const int *level_hw, int L, const uint8_t *empty,
+                                 const float *output_proposals, const uint8_t *proposal_invalid, float *out_proposals,
+                                 uint8_t *out_invalid, uint8_t *region, void *stream) {
+  if (B <= 0 || B > 65535) return fail(APE_ERR_INVALID_ARG, "region_prompt: B=%d outside [1, 65535]", B);
+  if (L < 1 || L > kMaxLevels) return fail(APE_ERR_INVALID_ARG, "region_prompt: L=%d outside [1, %d]", L, kMaxLevels);
+  if (Hp <= 0 || Wp <= 0) return fail(APE_ERR_INVALID_ARG, "region_prompt: padded shape %dx%d", Hp, Wp);
+  if (!level_hw) return fail(APE_ERR_NULL_PTR, "region_prompt: null level shapes");
+  if (!map || !empty || !output_proposals || !proposal_invalid || !out_proposals || !out_invalid)
+    return fail(APE_ERR_NULL_PTR, "region_prompt: null pointer");
+  if ((reinterpret_cast<uintptr_t>(output_proposals) & 15) || (reinterpret_cast<uintptr_t>(out_proposals) & 15))
+    return fail(APE_ERR_INVALID_ARG, "region_prompt: output_proposals / out_proposals must be 16-byte aligned");
+  RegionLevels lv{};
+  lv.L = L;
+  long long S = 0;
+  for (int l = 0; l < L; ++l) {
+    const int h = level_hw[2 * l], w = level_hw[2 * l + 1];
+    if (h < 1 || h > Hp || w < 1 || w > Wp)
+      return fail(APE_ERR_INVALID_ARG, "region_prompt: level %d of %dx%d does not fit the %dx%d padded shape", l, h, w, Hp, Wp);
+    lv.h[l] = h;
+    lv.w[l] = w;
+    lv.start[l] = (int)S;
+    lv.sh[l] = (float)Hp / (float)h;
+    lv.sw[l] = (float)Wp / (float)w;
+    S += (long long)h * w;
+  }
+  if (S > INT32_MAX / 4) return fail(APE_ERR_INVALID_ARG, "region_prompt: %lld tokens", S);
+  lv.S = (int)S;
+  const dim3 grid((unsigned)((S + kThreads - 1) / kThreads), (unsigned)B);
+  APE_LAUNCH(region_prompt_kernel, grid, kThreads, 0, (cudaStream_t)stream, map, Hp, Wp, lv, empty, output_proposals,
+             proposal_invalid, out_proposals, out_invalid, region);
+  return check_launch("region_prompt_kernel");
 }

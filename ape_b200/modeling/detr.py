@@ -10,7 +10,8 @@ ape/modeling/ape_deta/ape_deta.py:20-40 (`SomeThing`).  Same constructor keyword
 `bbox_embed` aliases under `transformer.decoder`.
 
 Scope (SURVEY.md §8): inference (boxes, instance masks, semantic and panoptic maps) for "name", "phrase" / "text" and
-"expression" prompts.  Training and mask prompts raise NotImplementedError (next rows of §8f) — loudly, never silently."""
+"expression" prompts, with or without a region prompt (`mask_prompt`).  Training raises NotImplementedError — loudly, never
+silently."""
 import collections
 import copy
 import math
@@ -520,12 +521,15 @@ class DeformableDETRSegmVL(nn.Module):
         # at the start of the captured graph, which therefore serves every image size inside the padded shape
         sizes = self._sizes_tensor(image_sizes) if images.is_cuda else None
         geo = self._padded_geometry(images.shape) if images.is_cuda else self._geometry(images.shape, image_sizes, img_masks)
-        mask_prompt_flatten = self._mask_prompt(batched_inputs, images.shape, geo) if "mask_prompt" in batched_inputs[0] else None
-        graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion) and mask_prompt_flatten is None
+        # region prompt: CUDA, the padded uint8 map (a graph input like `images`, folded into the anchors by ops.region_prompt);
+        # host tensors, the flattened per-level bool mask of the torch restatement
+        region = self._mask_prompt(batched_inputs, images.shape, geo) if "mask_prompt" in batched_inputs[0] else None
+        has_region = region is not None
+        graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion)
         need_masks = self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)
         if graphs and fusion is not None and fusion.shape[1] > 1:
             graphs = self._graph_seen((prompt, tuple(images.shape), tuple(features_l.shape), self.engine_dtype, need_masks,
-                                       do_postprocess, self.profile_stages))
+                                       do_postprocess, self.profile_stages, has_region))
         with torch.autocast("cuda", dtype=self.engine_dtype, enabled=low):
             if graphs and not self.profile_stages:
                 # encode -> select -> decode in ONE graph: the selection is written with static shapes and no host
@@ -567,20 +571,21 @@ class DeformableDETRSegmVL(nn.Module):
                 # the image sizes are a graph input like the image: the key holds the padded shape, not the sizes
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
-                    ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel),
-                    self._stage_all, (images, fusion, features_l, sizes, dims), const)
+                    ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel, has_region),
+                    self._stage_all, (images, fusion, features_l, sizes, dims, region), const)
                 self.transformer.last_topk_proposals = topk
                 mark("encode")
                 mark("select")
             else:
                 if graphs:
                     memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features, geo = self._graphed(
-                        ("encode", tuple(images.shape), need_masks), self._stage_encode_sized, (images, fusion, sizes), (geo,))
+                        ("encode", tuple(images.shape), need_masks, has_region), self._stage_encode_sized, (images, fusion, sizes, region),
+                        (geo,))
                 else:
                     if images.is_cuda:
                         geo = self._geometry(images.shape, image_sizes, sizes=sizes)
                     memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = \
-                        self._stage_encode(images, fusion, geo, mask_prompt_flatten)
+                        self._stage_encode(images, fusion, geo, region)
                 mark("encode")
                 topk = self.transformer.stage_select(enc_cls, enc_coord, geo)
                 self.transformer.last_topk_proposals = topk
@@ -711,8 +716,18 @@ class DeformableDETRSegmVL(nn.Module):
     def _mask_prompt(self, batched_inputs, batch_shape, geo):
         """:394-412: region prompts.  Per-image masks padded like the image (ImageList.from_tensors), an all-zero batch means
         "everywhere" (set to 255), resized bilinearly to every level and thresholded by `.to(bool)`; flattened like the features
-        (deformable_transformer_vl.py:465-470).  Proposals outside the prompt are disabled in the two-stage selection."""
+        (deformable_transformer_vl.py:465-470).  Proposals outside the prompt are disabled in the two-stage selection.
+        CUDA: returns the padded map uint8 [B, H, W] (1 where the prompt, cast to the pixel dtype as the reference does, is
+        nonzero), written without a host synchronisation; `_stage_encode` folds it into the anchors with ops.region_prompt, which
+        decides the empty batch and resamples on the device.  Exact for prompts whose nonzero values share one sign (INTEGRATION.md).
+        Host tensors: the torch restatement below, the flattened bool [B, S]."""
         H, W = batch_shape[-2], batch_shape[-1]
+        if self.device.type == "cuda":
+            region = torch.zeros((len(batched_inputs), H, W), dtype=torch.uint8, device=self.device)
+            for i, x in enumerate(batched_inputs):
+                m = x["mask_prompt"].to(self.device, non_blocking=True).to(self.pixel_mean.dtype)
+                region[i, : m.shape[-2], : m.shape[-1]] = m != 0
+            return region
         mp = torch.zeros((len(batched_inputs), H, W), dtype=self.pixel_mean.dtype, device=self.device)
         for i, x in enumerate(batched_inputs):
             m = x["mask_prompt"].to(self.device).to(self.pixel_mean.dtype)
@@ -722,7 +737,14 @@ class DeformableDETRSegmVL(nn.Module):
         levels = [F.interpolate(mp[None], size=sh, mode="bilinear").to(torch.bool).squeeze(0) for sh in geo["shapes"]]
         return torch.cat([m.flatten(1) for m in levels], 1)
 
-    def _stage_encode(self, images, fusion, geo, mask_prompt_flatten=None):
+    def _stage_encode(self, images, fusion, geo, region=None):
+        """region: None, the padded uint8 map of `_mask_prompt` on CUDA (folded here into the anchors: ops.region_prompt), or
+        the flattened bool mask of its host restatement (applied by stage_encode's masked_fill)."""
+        proposals, mask_prompt_flatten = None, None
+        if region is not None and region.is_cuda:
+            proposals = ops.region_prompt(region, geo["shapes"], geo["output_proposals"], geo["proposal_invalid"])[:2]
+        else:
+            mask_prompt_flatten = region
         features = self.backbone(images.to(self.engine_dtype))
         if self.neck is not None:
             feats = self.neck({f: features[f] for f in self.neck.in_features})
@@ -731,7 +753,7 @@ class DeformableDETRSegmVL(nn.Module):
             feats = tuple(features.values())
             flat = getattr(self.backbone, "last_flat", None)
         memory, fusion_out, output_memory, enc_cls, enc_coord = self.transformer.stage_encode(
-            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=flat)
+            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=flat, proposals=proposals)
         mask_features = None
         if self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on):
             mask_features = self.maskdino_mask_features(memory, features, geo)
@@ -770,17 +792,19 @@ class DeformableDETRSegmVL(nn.Module):
             return features_l
         return 0.0 * features_l + 1.0 * fusion_out.float()  # (:448)
 
-    def _stage_encode_sized(self, images, fusion, sizes, padded):
+    def _stage_encode_sized(self, images, fusion, sizes, region, padded):
         """_stage_encode after the per-size geometry, for the encode graph of the profiling split; the geometry is returned too,
         because selection and the decode graph read it."""
         geo = self._size_geometry(padded, sizes, True)
-        return self._stage_encode(images, fusion, geo) + (geo,)
+        return self._stage_encode(images, fusion, geo, region) + (geo,)
 
-    def _stage_all(self, images, fusion, features_l, sizes, dims, padded, prompt, sel=None, size_columns=None):
+    def _stage_all(self, images, fusion, features_l, sizes, dims, region, padded, prompt, sel=None, size_columns=None):
         # inside a graph the padding mask is always passed: an all-false mask gives the values of None (masked_fill with no
-        # true entry changes nothing), so one graph serves padded and unpadded sizes alike
+        # true entry changes nothing), so one graph serves padded and unpadded sizes alike.  The region map (or None) is a graph
+        # input too: one graph with a region and one without per padded shape, whatever the prompt
         geo = self._size_geometry(padded, sizes, True)
-        memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._stage_encode(images, fusion, geo)
+        memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._stage_encode(
+            images, fusion, geo, region)
         topk = self.transformer.stage_select(enc_cls, enc_coord, geo)
         features_l = self._mix_text(prompt, features_l, fusion_out)
         box_cls, box_pred, inter_states, init_reference, inter_references, mask_logits = self._stage_decode(

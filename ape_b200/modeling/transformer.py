@@ -492,9 +492,11 @@ class DeformableDetrTransformerVL(nn.Module):
             host_shapes=geo["shapes"])
 
     def stage_encode(self, multi_level_feats, geo, query_l, attention_mask_l=None, mask_prompt_flatten=None,
-                     feat_flatten=None):
+                     feat_flatten=None, proposals=None):
         """feat_flatten: optional [B,S,C] tensor that already holds the flattened levels (the engine neck writes its
-        outputs straight into it; `multi_level_feats` are then views of its slices)."""
+        outputs straight into it; `multi_level_feats` are then views of its slices).  Region prompts: `proposals`, the pair
+        (output_proposals, proposal_invalid) with the region already folded in (ops.region_prompt, CUDA), replaces the
+        geometry's; `mask_prompt_flatten`, bool [B, S], is applied here with masked_fill (host tensors)."""
         if feat_flatten is None:
             feat_flatten = torch.cat([f.flatten(2).transpose(1, 2) for f in multi_level_feats], 1)
         engine_dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else torch.float32
@@ -510,8 +512,7 @@ class DeformableDetrTransformerVL(nn.Module):
             pos_flatten = cache[engine_dtype][1]
         memory, query_l = self._encode(feat_flatten, pos_flatten, geo, query_l, attention_mask_l)
         # gen_encoder_output_proposals (:354-369): zero the memory of invalid anchors, project, normalise
-        output_proposals = geo["output_proposals"]
-        invalid = geo["proposal_invalid"]
+        output_proposals, invalid = proposals if proposals is not None else (geo["output_proposals"], geo["proposal_invalid"])
         if mask_prompt_flatten is not None:
             output_proposals = output_proposals.masked_fill(~mask_prompt_flatten.unsqueeze(-1), float("inf"))
             invalid = invalid | ~mask_prompt_flatten.unsqueeze(-1)

@@ -1481,3 +1481,40 @@ def zero_masked_rows_(x, mask):
                                            _lib.dtype_code(x.dtype), _lib.current_stream_ptr())
     _lib.check(rc, "ape_zero_masked_rows")
     return x
+
+
+def region_prompt(region_map, shapes, output_proposals, proposal_invalid, empty=None, want_region=False):
+    """Region prompts folded into the two-stage anchors (ape_region_prompt): region_map uint8 [B, Hp, Wp] on the device, nonzero
+    where the prompt is set (padded like the images, 0 in the padding); the level shapes [L, 2] host ints; output_proposals fp32
+    [B, S, 4] and proposal_invalid bool [B, S, 1] (or [B, S]) of the geometry.  `empty`: a device byte, nonzero when the whole
+    batch's prompt is empty ("everywhere"); None computes it from the map on the device (ape_region_prompt_empty).
+    Returns (output_proposals with +inf outside the region, proposal_invalid | ~region as bool [B, S, 1], the region as bool
+    [B, S] with want_region, else None).  New tensors; no host synchronisation, capturable in a CUDA graph."""
+    _require(region_map.is_cuda and region_map.dtype == torch.uint8 and region_map.dim() == 3 and region_map.is_contiguous(),
+             "region_prompt: region_map must be a contiguous CUDA uint8 [B, Hp, Wp] tensor")
+    dev = region_map.device
+    B, Hp, Wp = (int(v) for v in region_map.shape)
+    L = len(shapes)
+    S = sum(int(h) * int(w) for h, w in shapes)
+    _require(output_proposals.device == dev and output_proposals.dtype == torch.float32 and tuple(output_proposals.shape) == (B, S, 4)
+             and output_proposals.is_contiguous(), f"region_prompt: output_proposals must be contiguous fp32 [{B}, {S}, 4] on {dev}")
+    _require(proposal_invalid.device == dev and proposal_invalid.dtype == torch.bool and proposal_invalid.numel() == B * S
+             and proposal_invalid.shape[:2] == (B, S) and proposal_invalid.is_contiguous(),
+             f"region_prompt: proposal_invalid must be contiguous bool [{B}, {S}(, 1)] on {dev}")
+    _require(empty is None or (empty.device == dev and empty.dtype in (torch.uint8, torch.bool) and empty.numel() == 1),
+             "region_prompt: empty must be one uint8 / bool element on the map's device")
+    hw = (ctypes.c_int * max(2 * L, 1))(*[int(v) for sh in shapes for v in sh])
+    out_p = torch.empty((B, S, 4), dtype=torch.float32, device=dev)
+    out_i = torch.empty((B, S, 1), dtype=torch.bool, device=dev)
+    region = torch.empty((B, S), dtype=torch.bool, device=dev) if want_region else None
+    with torch.cuda.device(dev), _timed(("region_prompt", B, Hp, Wp, S)):
+        stream = _lib.current_stream_ptr()
+        if empty is None:
+            empty = torch.empty((1,), dtype=torch.uint8, device=dev)
+            _lib.check(_lib.lib.ape_region_prompt_empty(region_map.data_ptr(), region_map.numel(), empty.data_ptr(), stream),
+                       "ape_region_prompt_empty")
+        rc = _lib.lib.ape_region_prompt(region_map.data_ptr(), B, Hp, Wp, hw, L, empty.data_ptr(), output_proposals.data_ptr(),
+                                        proposal_invalid.data_ptr(), out_p.data_ptr(), out_i.data_ptr(),
+                                        region.data_ptr() if region is not None else None, stream)
+        _lib.check(rc, "ape_region_prompt")
+    return out_p, out_i, region

@@ -653,6 +653,36 @@ int ape_pad_geometry(const int *sizes, int B, int Hp, int Wp, const int *level_h
  */
 int ape_zero_masked_rows(void *x, int64_t ld, const uint8_t *mask, int64_t rows, int cols, int dtype, void *stream);
 
+/*
+ * Region prompts (`mask_prompt`), folded into the two-stage anchors.  Replaces deformable_detr_segm_vl.py:394-412 (the prompts
+ * padded like the images, "an all-zero batch means everywhere" via `masks_prompt.sum() == 0` -> 255, F.interpolate(mode="bilinear")
+ * to every level, `.to(torch.bool)`) and the `masked_fill(~mask_prompt_flatten, inf)` / `| ~mask_prompt_flatten` of
+ * deformable_transformer_vl.py:356-365 and :465-470.
+ *
+ * ape_region_prompt_empty: *empty = 1 when every byte of map[0:n) is 0, else 0 (a memset of the flag, then one reduction
+ * kernel; map 16-byte aligned).
+ *
+ * ape_region_prompt, one thread per token:
+ *   map               uint8 [B, Hp, Wp], 1 <= B <= 65535: nonzero where the image's prompt is nonzero, 0 elsewhere and in the padding
+ *   level_hw          HOST int [L, 2], 1 <= L <= 8, each level inside Hp x Wp; S = sum h_l w_l tokens, levels flattened in order
+ *   empty             device byte: nonzero when the whole batch's prompt is empty (ape_region_prompt_empty)
+ *   output_proposals  fp32 [B, S, 4] and proposal_invalid bool [B, S]: the geometry's anchors (ape_pad_geometry), read only
+ * Token (i, j) of level (h, w) is inside the region when the batch is empty, or when a tap of nonzero weight of
+ * F.interpolate(mode="bilinear", align_corners=False) from (Hp, Wp) reads a set byte: source index
+ * max(fmaf(d + 0.5, (float)in / out, -0.5), 0) (the fp32 operations of torch's CUDA kernel, fused as it is compiled), its
+ * truncation t and lambda = src - t; tap t always, tap t + 1 when lambda != 0 and t < in - 1, rows and columns alike.  For
+ * prompts whose nonzero values share one sign (and do not underflow in the weighted sum) this is interpolate(...).to(bool).
+ * Outputs (written completely; new buffers, the geometry's are not touched):
+ *   out_proposals     fp32 [B, S, 4]   output_proposals inside the region, +inf outside
+ *   out_invalid       bool [B, S]      proposal_invalid | !region
+ *   region            bool [B, S] or NULL
+ * output_proposals / out_proposals 16-byte aligned.  No allocation, no synchronisation: both are capturable in a CUDA graph.
+ */
+int ape_region_prompt_empty(const uint8_t *map, int64_t n, uint8_t *empty, void *stream);
+int ape_region_prompt(const uint8_t *map, int B, int Hp, int Wp, const int *level_hw, int L, const uint8_t *empty,
+                      const float *output_proposals, const uint8_t *proposal_invalid, float *out_proposals, uint8_t *out_invalid,
+                      uint8_t *region, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
