@@ -120,6 +120,10 @@ def _declare(lib):
     lib.ape_vlf_fold_pool_workspace_bytes.argtypes = [_i, _i, _i, _i]
     lib.ape_vlf_fold_pool.restype = _i
     lib.ape_vlf_fold_pool.argtypes = [_vp, _i64, _vp, _vp, _vp, _i64] + [_i] * 6 + [_vp]
+    lib.ape_vlf_fold_vision_dev.restype = _i
+    lib.ape_vlf_fold_vision_dev.argtypes = [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64] + [_i] * 4 + [_vp, _i, _i, _vp]
+    lib.ape_vlf_fold_pool_dev.restype = _i
+    lib.ape_vlf_fold_pool_dev.argtypes = [_vp, _i64, _vp, _vp, _vp, _i64] + [_i] * 4 + [_vp, _i, _i, _vp]
     lib.ape_nms_workspace_bytes.restype = _i64
     lib.ape_nms_workspace_bytes.argtypes = [_i]
     lib.ape_nms_sorted.restype = _i
@@ -204,6 +208,8 @@ def _declare(lib):
     lib.ape_panoptic_winners_dev.argtypes = [_vp] * 5 + [_i] * 5 + [_vp, _i, ctypes.c_float, _i, _vp]
     lib.ape_panoptic_pack_dev.restype = _i
     lib.ape_panoptic_pack_dev.argtypes = [_vp] * 3 + [_i] * 4 + [ctypes.c_double, _vp, _i, _vp, _vp, _i, _vp]
+    lib.ape_gemm_tn_cols_dev.restype = _i
+    lib.ape_gemm_tn_cols_dev.argtypes = [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i, _i, _i, _vp, _i, _vp]
 
 
 
@@ -249,6 +255,8 @@ EXPORTS = (
     "ape_vlf_fold_vision",
     "ape_vlf_fold_pool_workspace_bytes",
     "ape_vlf_fold_pool",
+    "ape_vlf_fold_vision_dev",
+    "ape_vlf_fold_pool_dev",
     "ape_nms_workspace_bytes",
     "ape_nms_sorted",
     "ape_nms_sorted_dev",
@@ -291,6 +299,7 @@ EXPORTS = (
     "ape_label_rle_pack_dev",
     "ape_panoptic_winners_dev",
     "ape_panoptic_pack_dev",
+    "ape_gemm_tn_cols_dev",
 )
 
 

@@ -127,6 +127,14 @@ __device__ __forceinline__ size_t out_row_offset(const GemmParams &p, int m) {
   return (((size_t)img * p.conv_H + y) * p.conv_W + x) * p.ldc;
 }
 
+// The vision-language logits of a text padded to a capacity (ape_gemm_tn_cols_dev): the clamp + bias epilogue of
+// Epi<true, ACT_CLAMP, RES_NONE>, and the columns at or past the device count at `residual` (which no RES_NONE epilogue reads)
+// are written as -inf, so a padded class is never a candidate and never wins a maximum.  A type of its own, so that the
+// kernels of every other epilogue compile as before
+struct EpiClampCols : Epi<true, ACT_CLAMP, RES_NONE> {};
+template <class E>
+constexpr bool kDevCols = std::is_same<E, EpiClampCols>::value;
+
 template <typename TO>
 __device__ __forceinline__ void store_pair(TO *dst, float v0, float v1, bool ok1, bool vec) {
   if (vec && ok1) {
@@ -155,6 +163,8 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
   const int warp4 = (threadIdx.x >> 5) & 3, tq = lane & 3;
   const int c_base = n_blk * BN + 2 * tq;
   TO *C = reinterpret_cast<TO *>(p.C);
+  int n_cols = 0;  // kDevCols: the columns in use; a kernel before this one writes the count, read after pdl_wait()
+  if constexpr (kDevCols<E>) n_cols = *static_cast<const int *>(p.residual);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int m = m_blk * BM + wg * 64 + warp4 * 16 + (lane >> 2) + 8 * h;
@@ -230,6 +240,10 @@ __device__ __forceinline__ void epilogue(const GemmParams &p, const float *acc, 
         }
         v0 = act1<E::act>(v0);
         v1 = act1<E::act>(v1);
+        if constexpr (kDevCols<E>) {
+          if (n >= n_cols) v0 = -INFINITY;
+          if (n + 1 >= n_cols) v1 = -INFINITY;
+        }
         if constexpr (E::res != RES_NONE) {
           if (ok0) {
             const float2 r = E::res == RES_F32 ? ld_res_pair<FULL>(res32 + n, ok1) : ld_res_pair<FULL>(res16 + n, ok1);
@@ -1105,6 +1119,38 @@ extern "C" int ape_gemm_tn_argmax(const void *A, int64_t lda, const void *W, int
 extern "C" int ape_gemm_tn_argmax_dev(const void *A, int64_t lda, const void *W, int64_t ldw, uint64_t *keys, int M, const int *m_rows,
                                       int N, int K, int col_base, int in_dtype, void *stream) {
   return gemm_argmax<EpiArgmaxDev>(A, lda, W, ldw, keys, M, m_rows, N, K, col_base, in_dtype, stream);
+}
+
+// C = clamp(A W^T + bias, +-50000) in fp32 over the first *n_cols columns and -inf over the rest (EpiClampCols): the
+// VisionLanguageAlign logits of a vocabulary padded to N rows.  Single-CTA BN = 128 cooperative kernel, as ape_gemm_tn takes for
+// the classifier's shapes; every output element gets the same MMA sequence whatever N, so a column equals the exact-N GEMM's
+extern "C" int ape_gemm_tn_cols_dev(const void *A, int64_t lda, const void *W, int64_t ldw, float *C, int64_t ldc, const float *bias,
+                                    int M, int N, int K, const int *n_cols, int in_dtype, void *stream) {
+  if (in_dtype != APE_DTYPE_F16 && in_dtype != APE_DTYPE_BF16)
+    return fail(APE_ERR_INVALID_ARG, "gemm_cols_dev: operands must be fp16 or bf16 (got dtype %d)", in_dtype);
+  if (M < 0 || N <= 0 || K <= 0) return fail(APE_ERR_INVALID_ARG, "gemm_cols_dev: bad sizes M=%d N=%d K=%d", M, N, K);
+  if (!A || !W || !C || !n_cols) return fail(APE_ERR_NULL_PTR, "gemm_cols_dev: null pointer argument");
+  if ((lda * 2) % 16 || (ldw * 2) % 16 || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15))
+    return fail(APE_ERR_INVALID_ARG, "gemm_cols_dev: A/W base and row pitch must be 16-byte aligned (TMA)");
+  if (lda < K || ldw < K || ldc < N) return fail(APE_ERR_INVALID_ARG, "gemm_cols_dev: row pitch smaller than K or N");
+  if (reinterpret_cast<uintptr_t>(n_cols) & 3) return fail(APE_ERR_INVALID_ARG, "gemm_cols_dev: n_cols must be a 4-byte aligned int32");
+  if (M == 0) return APE_OK;
+  constexpr int bn = 128;
+  CUtensorMap ma, mb;
+  if (int rc = make_map(&ma, A, in_dtype, M, K, lda, BM)) return rc;
+  if (int rc = make_map(&mb, W, in_dtype, N, K, ldw, bn)) return rc;
+  GemmParams p{};
+  p.C = C; p.bias = bias; p.ldc = ldc;
+  p.M = M; p.N = N; p.K = K;
+  p.m_blocks = (M + BM - 1) / BM;
+  p.k_blocks = (K + BK - 1) / BK;
+  p.trace = g_gemm_trace;
+  p.residual = n_cols;  // EpiClampCols' column count
+  p.vec_out = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) % 8) == 0;
+  p.fast = p.vec_out && reinterpret_cast<uintptr_t>(bias) % 8 == 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (in_dtype == APE_DTYPE_BF16) return launch_gemm<bn, 6, 1, __nv_bfloat16, EpiClampCols>(ma, mb, p, st);
+  return launch_gemm<bn, 6, 1, __half, EpiClampCols>(ma, mb, p, st);
 }
 
 extern "C" int ape_gemm_tn_rope(const void *A, int64_t lda, const void *W, int64_t ldw, void *C, int64_t ldc,

@@ -46,12 +46,14 @@ struct alignas(1024) PoolSmem {
   uint64_t q_full, kv_full[2], kv_empty[2];
 };
 
-template <typename T>
-__global__ void __launch_bounds__(160, 1)
-vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_qa,
-                       const __grid_constant__ CUtensorMap map_u, const T *resid, long long ldv, const float *__restrict__ qc,
-                       const float *__restrict__ gamma, const float *__restrict__ bias, T *out, long long ldo, int S, int N,
-                       int NH) {
+// DEV (vlf_fold_vision_dev_kernel): the text is padded to N tokens per (b, h) block and only the first *n_dev (clamped to
+// [1, N]) are keys; the key blocks past them are not loaded, and whether the statistics pass runs is decided from N alone, so
+// the kernel's arithmetic follows the padded shape whatever the prompt.
+template <typename T, bool DEV>
+__device__ __forceinline__ void fold_vision(const CUtensorMap &map_v, const CUtensorMap &map_qa, const CUtensorMap &map_u,
+                                            const T *resid, long long ldv, const float *__restrict__ qc, const float *__restrict__ gamma,
+                                            const float *__restrict__ bias, T *out, long long ldo, int S, int N, int NH,
+                                            const int *n_dev) {
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
   VisionSmem &s = *reinterpret_cast<VisionSmem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -76,6 +78,11 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
   }
   __syncthreads();
   pdl_wait();
+  int n_live = N, nkb_live = nkb;  // keys in use and their blocks (a kernel before this one writes *n_dev)
+  if constexpr (DEV) {
+    n_live = min(max(*n_dev, 1), N);
+    nkb_live = (n_live + KB - 1) / KB;
+  }
 
   if (warp == 4) {
     // ===================== TMA producer: Q once, then per head [K blocks (statistics pass)] + (K, U) blocks =====================
@@ -95,8 +102,8 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
       for (int h = 0; h < NH; ++h) {
         const int row0 = (b * NH + h) * N;
         if (two_pass)
-          for (int j = 0; j < nkb; ++j) load_k(row0 + j * KB);
-        for (int j = 0; j < nkb; ++j) {
+          for (int j = 0; j < nkb_live; ++j) load_k(row0 + j * KB);
+        for (int j = 0; j < nkb_live; ++j) {
           load_k(row0 + j * KB);
           const int i = uj & 1, n = uj >> 1;
           tc::mbar_wait(&s.u_empty[i], (n & 1) ^ 1);
@@ -121,7 +128,7 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
   tc::mbar_wait(&s.q_full, 0);
   int kj = 0, uj = 0;
 
-  // scores of key block j of head h in the log2 domain: (v . qa + qc) * log2(e), keys >= N at -inf
+  // scores of key block j of head h in the log2 domain: (v . qa + qc) * log2(e), keys >= n_live at -inf
   auto scores = [&](float (&sc)[32], const float *qch, int j) {
     const int i = kj & 1, n = kj >> 1;
     tc::mbar_wait(&s.k_full[i], n & 1);
@@ -143,11 +150,11 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int key = j * KB + 8 * jj + 2 * tq + e;
-        const float bq = key < N ? __ldg(qch + key) : 0.f;
+        const float bq = key < n_live ? __ldg(qch + key) : 0.f;
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           float &x = sc[4 * jj + 2 * hh + e];
-          x = key < N ? (x + bq) * kLog2e : -INFINITY;
+          x = key < n_live ? (x + bq) * kLog2e : -INFINITY;
         }
       }
   };
@@ -166,7 +173,7 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
     float m[2] = {-INFINITY, -INFINITY}, inv[2] = {0.f, 0.f};
     if (two_pass) {  // statistics pass: exact row max and sum of the head's softmax
       float l[2] = {0.f, 0.f};
-      for (int j = 0; j < nkb; ++j) {
+      for (int j = 0; j < nkb_live; ++j) {
         float sc[32];
         scores(sc, qch, j);
 #pragma unroll
@@ -187,7 +194,7 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
         inv[hh] = 1.f / l[hh];
       }
     }
-    for (int j = 0; j < nkb; ++j) {
+    for (int j = 0; j < nkb_live; ++j) {
       float sc[32];
       scores(sc, qch, j);
       if (!two_pass) {
@@ -260,11 +267,30 @@ vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_c
   }
 }
 
-// grid (ceil(R / 64), nsplit, B), R = NH * N query rows per image; chunk c covers keys [c * chunk, min(S, (c + 1) * chunk)).
 template <typename T>
 __global__ void __launch_bounds__(160, 1)
-vlf_fold_pool_kernel(const __grid_constant__ CUtensorMap map_qa, const __grid_constant__ CUtensorMap map_v,
-                     float *__restrict__ part_o, float2 *__restrict__ part_ml, int S, int R, int chunk) {
+vlf_fold_vision_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_qa,
+                       const __grid_constant__ CUtensorMap map_u, const T *resid, long long ldv, const float *__restrict__ qc,
+                       const float *__restrict__ gamma, const float *__restrict__ bias, T *out, long long ldo, int S, int N,
+                       int NH) {
+  fold_vision<T, false>(map_v, map_qa, map_u, resid, ldv, qc, gamma, bias, out, ldo, S, N, NH, nullptr);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(160, 1)
+vlf_fold_vision_dev_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_qa,
+                           const __grid_constant__ CUtensorMap map_u, const T *resid, long long ldv, const float *__restrict__ qc,
+                           const float *__restrict__ gamma, const float *__restrict__ bias, T *out, long long ldo, int S, int N,
+                           int NH, const int *n_dev) {
+  fold_vision<T, true>(map_v, map_qa, map_u, resid, ldv, qc, gamma, bias, out, ldo, S, N, NH, n_dev);
+}
+
+// grid (ceil(R / 64), nsplit, B), R = NH * N query rows per image; chunk c covers keys [c * chunk, min(S, (c + 1) * chunk)).
+// DEV (vlf_fold_pool_dev_kernel): rows r of token r % N >= *n_dev (clamped to [1, N]) are padding; a tile of padding rows
+// alone returns at once, and the combine writes zeros for them without reading their partials.
+template <typename T, bool DEV>
+__device__ __forceinline__ void fold_pool(const CUtensorMap &map_qa, const CUtensorMap &map_v, float *__restrict__ part_o,
+                                          float2 *__restrict__ part_ml, int S, int R, int chunk, int N, const int *n_dev) {
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
   PoolSmem &s = *reinterpret_cast<PoolSmem *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -286,6 +312,12 @@ vlf_fold_pool_kernel(const __grid_constant__ CUtensorMap map_qa, const __grid_co
   }
   __syncthreads();
   pdl_wait();
+  if constexpr (DEV) {  // every row of the tile is a padding token: nothing of it is read
+    const int n_live = min(max(*n_dev, 1), N);
+    bool live = false;
+    for (int r = tile * 64; r < min(R, tile * 64 + 64) && !live; ++r) live = r % N < n_live;
+    if (!live) return;
+  }
 
   if (warp == 4) {
     if (lane == 0) {
@@ -398,6 +430,20 @@ vlf_fold_pool_kernel(const __grid_constant__ CUtensorMap map_qa, const __grid_co
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(160, 1)
+vlf_fold_pool_kernel(const __grid_constant__ CUtensorMap map_qa, const __grid_constant__ CUtensorMap map_v,
+                     float *__restrict__ part_o, float2 *__restrict__ part_ml, int S, int R, int chunk) {
+  fold_pool<T, false>(map_qa, map_v, part_o, part_ml, S, R, chunk, 1, nullptr);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(160, 1)
+vlf_fold_pool_dev_kernel(const __grid_constant__ CUtensorMap map_qa, const __grid_constant__ CUtensorMap map_v,
+                         float *__restrict__ part_o, float2 *__restrict__ part_ml, int S, int R, int chunk, int N, const int *n_dev) {
+  fold_pool<T, true>(map_qa, map_v, part_o, part_ml, S, R, chunk, N, n_dev);
+}
+
 // One CTA of 256 threads per query row (b, h, n): pooled[b * N + n, h * 256 + col] = sum_c w_c O_c / sum_c w_c l_c with
 // w_c = 2^(m_c - max_c m_c), chunks in ascending order.
 template <typename T>
@@ -418,6 +464,33 @@ vlf_fold_combine_kernel(const float *__restrict__ part_o, const float2 *__restri
   }
   const int h = r / N, n = r - h * N;
   pooled[((size_t)b * N + n) * ldp + h * C + col] = Elem<T>::from_f(acc / den);
+}
+
+// The combine of vlf_fold_pool_dev_kernel: padding rows (token >= *n_dev, clamped to [1, N]) are written as zeros, so every row
+// of the pooled output is finite whatever the prompt; the others as vlf_fold_combine_kernel.
+template <typename T>
+__global__ void __launch_bounds__(256)
+vlf_fold_combine_dev_kernel(const float *__restrict__ part_o, const float2 *__restrict__ part_ml, T *__restrict__ pooled,
+                            long long ldp, int R, int N, int nsplit, const int *__restrict__ n_dev) {
+  pdl_prologue();
+  const int b = blockIdx.y, r = blockIdx.x, col = threadIdx.x;
+  const int h = r / N, n = r - h * N;
+  T *dst = pooled + ((size_t)b * N + n) * ldp + h * C + col;
+  if (n >= min(max(*n_dev, 1), N)) {
+    *dst = Elem<T>::from_f(0.f);
+    return;
+  }
+  const size_t base = (size_t)b * nsplit * R + r;
+  float mx = -INFINITY;
+  for (int c = 0; c < nsplit; ++c) mx = fmaxf(mx, part_ml[base + (size_t)c * R].x);
+  float acc = 0.f, den = 0.f;
+  for (int c = 0; c < nsplit; ++c) {
+    const float2 ml = part_ml[base + (size_t)c * R];
+    const float w = ex2(ml.x - mx);
+    den = fmaf(w, ml.y, den);
+    acc = fmaf(w, part_o[(base + (size_t)c * R) * C + col], acc);
+  }
+  *dst = Elem<T>::from_f(acc / den);
 }
 
 // Key chunks of the pooling: enough CTAs for two per SM of an H100 SXM, at least 1024 keys each.
@@ -449,11 +522,20 @@ int set_smem(bool &set, K kernel, size_t bytes, const char *what) {
 
 template <typename T>
 int launch_vision(const CUtensorMap &mv, const CUtensorMap &mqa, const CUtensorMap &mu, const void *v, int64_t ldv, const float *qc,
-                  const float *gamma, const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, cudaStream_t st) {
+                  const float *gamma, const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, cudaStream_t st,
+                  const int *n_dev = nullptr) {
+  const dim3 grid((unsigned)((S + 63) / 64), (unsigned)B);
+  if (n_dev) {
+    auto k = vlf_fold_vision_dev_kernel<T>;
+    static bool set = false;
+    if (int rc = set_smem(set, k, sizeof(VisionSmem) + 1024, "vlf_fold_vision_dev")) return rc;
+    APE_LAUNCH(k, grid, 160, sizeof(VisionSmem) + 1024, st, mv, mqa, mu, (const T *)v, (long long)ldv, qc, gamma, bias, (T *)out,
+               (long long)ldo, S, N, NH, n_dev);
+    return check_launch("vlf_fold_vision_dev_kernel");
+  }
   auto k = vlf_fold_vision_kernel<T>;
   static bool set = false;
   if (int rc = set_smem(set, k, sizeof(VisionSmem) + 1024, "vlf_fold_vision")) return rc;
-  const dim3 grid((unsigned)((S + 63) / 64), (unsigned)B);
   APE_LAUNCH(k, grid, 160, sizeof(VisionSmem) + 1024, st, mv, mqa, mu, (const T *)v, (long long)ldv, qc, gamma, bias, (T *)out,
              (long long)ldo, S, N, NH);
   return check_launch("vlf_fold_vision_kernel");
@@ -461,7 +543,18 @@ int launch_vision(const CUtensorMap &mv, const CUtensorMap &mqa, const CUtensorM
 
 template <typename T>
 int launch_pool(const CUtensorMap &mqa, const CUtensorMap &mv, float *part_o, float2 *part_ml, void *pooled, int64_t ldp, int B,
-                int S, int N, int R, int nsplit, int chunk, cudaStream_t st) {
+                int S, int N, int R, int nsplit, int chunk, cudaStream_t st, const int *n_dev = nullptr) {
+  if (n_dev) {
+    auto k = vlf_fold_pool_dev_kernel<T>;
+    static bool set = false;
+    if (int rc = set_smem(set, k, sizeof(PoolSmem) + 1024, "vlf_fold_pool_dev")) return rc;
+    APE_LAUNCH(k, dim3((unsigned)((R + 63) / 64), (unsigned)nsplit, (unsigned)B), 160, sizeof(PoolSmem) + 1024, st, mqa, mv, part_o,
+               part_ml, S, R, chunk, N, n_dev);
+    if (int rc = check_launch("vlf_fold_pool_dev_kernel")) return rc;
+    APE_LAUNCH((vlf_fold_combine_dev_kernel<T>), dim3((unsigned)R, (unsigned)B), 256, 0, st, (const float *)part_o,
+               (const float2 *)part_ml, (T *)pooled, (long long)ldp, R, N, nsplit, n_dev);
+    return check_launch("vlf_fold_combine_dev_kernel");
+  }
   auto k = vlf_fold_pool_kernel<T>;  // T is not in the kernel's signature: the flag must live here, per T
   static bool set = false;
   if (int rc = set_smem(set, k, sizeof(PoolSmem) + 1024, "vlf_fold_pool")) return rc;
@@ -478,9 +571,9 @@ int launch_pool(const CUtensorMap &mqa, const CUtensorMap &mv, float *part_o, fl
 
 using namespace ape;
 
-extern "C" int ape_vlf_fold_vision(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
-                                   const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, int C_, int dtype,
-                                   void *stream) {
+static int fold_vision_impl(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
+                            const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, int C_, int dtype, void *stream,
+                            const int *n_dev) {
   if (int rc = check_common("vlf_fold_vision", B, S, N, NH, dtype)) return rc;
   if (C_ != C) return fail(APE_ERR_UNSUPPORTED, "vlf_fold_vision: %d channels (256 only)", C_);
   if (!v || !qa || !u || !qc || !gamma || !bias || !out) return fail(APE_ERR_NULL_PTR, "vlf_fold_vision: null pointer argument");
@@ -493,8 +586,22 @@ extern "C" int ape_vlf_fold_vision(const void *v, int64_t ldv, const void *qa, c
   if (int rc = attn::make_map(&mqa, qa, dtype, (long long)B * NH * N, C, C)) return rc;
   if (int rc = attn::make_map(&mu, u, dtype, (long long)B * NH * N, C, C)) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (dtype == APE_DTYPE_F16) return launch_vision<__half>(mv, mqa, mu, v, ldv, qc, gamma, bias, out, ldo, B, S, N, NH, st);
-  return launch_vision<__nv_bfloat16>(mv, mqa, mu, v, ldv, qc, gamma, bias, out, ldo, B, S, N, NH, st);
+  if (dtype == APE_DTYPE_F16) return launch_vision<__half>(mv, mqa, mu, v, ldv, qc, gamma, bias, out, ldo, B, S, N, NH, st, n_dev);
+  return launch_vision<__nv_bfloat16>(mv, mqa, mu, v, ldv, qc, gamma, bias, out, ldo, B, S, N, NH, st, n_dev);
+}
+
+extern "C" int ape_vlf_fold_vision(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
+                                   const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, int C_, int dtype,
+                                   void *stream) {
+  return fold_vision_impl(v, ldv, qa, u, qc, gamma, bias, out, ldo, B, S, N, NH, C_, dtype, stream, nullptr);
+}
+
+extern "C" int ape_vlf_fold_vision_dev(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
+                                       const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, const int *n_dev, int C_,
+                                       int dtype, void *stream) {
+  if (!n_dev) return fail(APE_ERR_NULL_PTR, "vlf_fold_vision_dev: null n_dev");
+  if (reinterpret_cast<uintptr_t>(n_dev) & 3) return fail(APE_ERR_INVALID_ARG, "vlf_fold_vision_dev: n_dev must be a 4-byte aligned int32");
+  return fold_vision_impl(v, ldv, qa, u, qc, gamma, bias, out, ldo, B, S, N, NH, C_, dtype, stream, n_dev);
 }
 
 extern "C" int64_t ape_vlf_fold_pool_workspace_bytes(int B, int S, int N, int NH) {
@@ -504,8 +611,8 @@ extern "C" int64_t ape_vlf_fold_pool_workspace_bytes(int B, int S, int N, int NH
   return (int64_t)B * nsplit * R * (C + 2) * 4;
 }
 
-extern "C" int ape_vlf_fold_pool(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B,
-                                 int S, int N, int NH, int C_, int dtype, void *stream) {
+static int fold_pool_impl(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B, int S, int N,
+                          int NH, int C_, int dtype, void *stream, const int *n_dev) {
   if (int rc = check_common("vlf_fold_pool", B, S, N, NH, dtype)) return rc;
   if (C_ != C) return fail(APE_ERR_UNSUPPORTED, "vlf_fold_pool: %d channels (256 only)", C_);
   if (!v || !qa || !workspace || !pooled) return fail(APE_ERR_NULL_PTR, "vlf_fold_pool: null pointer argument");
@@ -522,6 +629,19 @@ extern "C" int ape_vlf_fold_pool(const void *v, int64_t ldv, const void *qa, voi
   float *part_o = reinterpret_cast<float *>(workspace);
   float2 *part_ml = reinterpret_cast<float2 *>(part_o + (size_t)B * nsplit * R * C);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (dtype == APE_DTYPE_F16) return launch_pool<__half>(mqa, mv, part_o, part_ml, pooled, ldp, B, S, N, R, nsplit, chunk, st);
-  return launch_pool<__nv_bfloat16>(mqa, mv, part_o, part_ml, pooled, ldp, B, S, N, R, nsplit, chunk, st);
+  if (dtype == APE_DTYPE_F16) return launch_pool<__half>(mqa, mv, part_o, part_ml, pooled, ldp, B, S, N, R, nsplit, chunk, st, n_dev);
+  return launch_pool<__nv_bfloat16>(mqa, mv, part_o, part_ml, pooled, ldp, B, S, N, R, nsplit, chunk, st, n_dev);
+}
+
+extern "C" int ape_vlf_fold_pool(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B,
+                                 int S, int N, int NH, int C_, int dtype, void *stream) {
+  return fold_pool_impl(v, ldv, qa, workspace, pooled, ldp, B, S, N, NH, C_, dtype, stream, nullptr);
+}
+
+// The split over S and the combine order come from (B, S, N, NH): with N the padded token count they do not depend on *n_dev.
+extern "C" int ape_vlf_fold_pool_dev(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B,
+                                     int S, int N, int NH, const int *n_dev, int C_, int dtype, void *stream) {
+  if (!n_dev) return fail(APE_ERR_NULL_PTR, "vlf_fold_pool_dev: null n_dev");
+  if (reinterpret_cast<uintptr_t>(n_dev) & 3) return fail(APE_ERR_INVALID_ARG, "vlf_fold_pool_dev: n_dev must be a 4-byte aligned int32");
+  return fold_pool_impl(v, ldv, qa, workspace, pooled, ldp, B, S, N, NH, C_, dtype, stream, n_dev);
 }

@@ -45,10 +45,12 @@ class VisionLanguageAlign(nn.Module):
 
         return ops.cached(self, "_pk", dtype, (tuple(p._version for p in ps), lin.weight.data_ptr()), build)
 
-    def forward_engine(self, x, embedding):
+    def forward_engine(self, x, embedding, n_cols=None):
         """Engine path (x [B,Q,C] fp16 / bf16 CUDA): the text projection, the language bias and the query x text contraction
         are wgmma GEMMs (ape_gemm_tn); fp32 accumulation, fp32 logits, bias + clamp in the epilogue.  The reference's own
-        eval recipe runs this module in fp16 end to end (tools/train_net.py:641-642); here only the operands are 16-bit."""
+        eval recipe runs this module in fp16 end to end (tools/train_net.py:641-642); here only the operands are 16-bit.
+        n_cols (int32 [1] on the device, or None): the text is padded to embedding.shape[1] rows and only the first n_cols are
+        classes; the contraction (ape_gemm_tn_cols_dev) writes -inf into the other columns."""
         from .. import ops
 
         wt, bt, wl, bl = self._engine_weights(x.dtype)
@@ -56,13 +58,20 @@ class VisionLanguageAlign(nn.Module):
         tokens = ops.linear_tc(e, wt, bt)                                                # [B,N,C]: Linear(e / 2) / exp(log_scale)
         bias = ops.linear_tc(e, wl, bl, out_dtype=torch.float32)[..., 0].contiguous()    # [B,N]:   e . bias_lang + bias0
         act = "clamp" if self.clamp_dot_product else None
+        if n_cols is not None:
+            if act != "clamp":
+                raise NotImplementedError("ape_b200: a padded prompt needs clamp_dot_product (the kernel clamps)")
+            out = [ops.linear_cols_dev(x[b].contiguous(), tokens[b], bias[b], n_cols) for b in range(x.shape[0])]
+            return torch.stack(out) if len(out) > 1 else out[0][None]
         out = [ops.linear_tc(x[b].contiguous(), tokens[b], bias[b], act=act, out_dtype=torch.float32) for b in range(x.shape[0])]
         return torch.stack(out) if len(out) > 1 else out[0][None]
 
-    def forward(self, x, embedding):
+    def forward(self, x, embedding, n_cols=None):
         if x.is_cuda and x.dtype in (torch.float16, torch.bfloat16) and x.dim() == 3 and x.shape[-1] % 8 == 0 \
                 and embedding.shape[-1] % 8 == 0:
-            return self.forward_engine(x, embedding)
+            return self.forward_engine(x, embedding, n_cols)
+        if n_cols is not None:
+            raise NotImplementedError("ape_b200: padded prompts run on the engine path only (16-bit CUDA operands)")
         tokens, bias = self.project_text(embedding, x.dtype)
         logit = torch.matmul(x, tokens.transpose(-1, -2)) / self.log_scale.exp() + bias.unsqueeze(1)
         if self.clamp_dot_product:

@@ -130,7 +130,9 @@ class BiAttentionBlock(nn.Module):
         self.gamma_l = nn.Parameter(init_values * torch.ones(l_dim))
         self.fold_language_side = True  # one-token case: fold the small projection chains into two GEMVs (CUDA)
 
-    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None):
+    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None, n_tokens=None):
+        """n_tokens (int32 [1] on the device, or None): l is padded and only its first n_tokens tokens are real (a prompt padded
+        to a capacity); the folded path reads the count on the device, and no other path takes padded text."""
         # fuse_helper.py:221-232 — note the residual is added to the *normalised* v / l
         a = self.attn
         if v.is_cuda and v.dtype in (torch.float16, torch.bfloat16) and l.shape[1] > 1 and attention_mask_l is None and \
@@ -142,9 +144,13 @@ class BiAttentionBlock(nn.Module):
             with torch.autocast("cuda", enabled=False):
                 ln = self.layer_norm_l(l.float())
             if self.folds(vn.shape[-1], ln.shape[-1], ln.shape[1]):
-                return self.folded(vn, ln)
+                return self.folded(vn, ln, n_tokens)
+            if n_tokens is not None:
+                raise NotImplementedError("ape_b200: a padded prompt needs the folded fusion path")
             dv, dl = a.forward_engine(vn, ln)
             return vn + self.gamma_v.to(vn.dtype) * dv, ln + self.gamma_l.float() * dl
+        if n_tokens is not None:
+            raise NotImplementedError("ape_b200: a padded prompt needs the folded fusion path (16-bit CUDA)")
         v = self.layer_norm_v(v)
         l = self.layer_norm_l(l)
         if l.shape[1] == 1 and attention_mask_l is None and not (self.attn.use_attention_mask_v and attention_mask_v is not None):
@@ -167,7 +173,7 @@ class BiAttentionBlock(nn.Module):
         return a.head_dim in (64, 256) and v_dim == 256 and l_dim % 8 == 0 and n_tokens <= self.fold_max_tokens and \
             not (a.use_attention_mask_v and masked_v)
 
-    def folded(self, vn, ln):
+    def folded(self, vn, ln, n_tokens=None):
         """BiMultiHeadAttention.forward (fuse_helper.py:67-166) for N >= 1 unmasked language tokens, with the language side
         folded into the 256-dimensional vision space (fold_maps): per layer ONE GEMM maps the LayerNormed tokens to the
         per-head keys qa, biases qc and values U, and
@@ -176,7 +182,8 @@ class BiAttentionBlock(nn.Module):
                          delta_l = E pooled + e0.
         Nothing of width embed_dim is formed over the S vision tokens: no v_proj / values_v_proj / out_v_proj GEMMs.  The
         +-5e4 clamps and the global-max shift are treated as softmax-invariant translations, as in forward_engine.
-        vn [B,S,256] 16-bit (layer-normed), ln [B,N,l_dim] fp32.  Returns (query [B,S,256] in vn's dtype, l [B,N,l_dim] fp32)."""
+        vn [B,S,256] 16-bit (layer-normed), ln [B,N,l_dim] fp32.  Returns (query [B,S,256] in vn's dtype, l [B,N,l_dim] fp32).
+        n_tokens: see forward; the padding tokens are no keys of the vision side and their pooled rows are zeros."""
         from .. import ops
 
         a = self.attn
@@ -193,8 +200,8 @@ class BiAttentionBlock(nn.Module):
             qc = y[..., 2 * nh * C:].transpose(1, 2).contiguous()
             vn = vn.contiguous()
             _, bo = ops.packed(a.out_v_proj, dt)
-            out = ops.vlf_fold_vision(vn, qa, u, qc, self.gamma_v.detach().float().contiguous(), bo)
-            pooled = ops.vlf_fold_pool(vn, qa)
+            out = ops.vlf_fold_vision(vn, qa, u, qc, self.gamma_v.detach().float().contiguous(), bo, n_dev=n_tokens)
+            pooled = ops.vlf_fold_pool(vn, qa, n_dev=n_tokens)
             dl = ops.linear_tc(pooled, E, e0, out_dtype=torch.float32).view(B, N, L)
         return out, ln + self.gamma_l.float() * dl
 
@@ -345,5 +352,5 @@ class VisionLanguageFusion(nn.Module):
                                        stable_softmax_2d, clamp_min_for_underflow, clamp_max_for_overflow,
                                        use_attention_mask_v)
 
-    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None):
-        return self.b_attn(v, l, attention_mask_v, attention_mask_l)
+    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None, n_tokens=None):
+        return self.b_attn(v, l, attention_mask_v, attention_mask_l, n_tokens)

@@ -312,6 +312,12 @@ class DeformableDETRSegmVL(nn.Module):
         # panoptic stages on sizes held on the device (ops.*_dev), so `use_cuda_graphs` captures one graph per padded shape and
         # configuration for them instead of one per combination of sizes.  Larger outputs take the per-size path
         self.packed_output_capacity = None
+        # None, or an int C: a captured call whose text comes from the call itself (`text_prompt` names) and has n <= C classes
+        # runs with the text features zero-padded to C rows and n as an int32 graph input on the device, so `use_cuda_graphs`
+        # captures one graph per padded shape for every such prompt instead of one per n.  Columns n..C-1 of the logits are -inf
+        # and take no part in any selection or class reduction; what the caller sees is cut back to n.  Cached dataset
+        # vocabularies keep their exact-n graphs, and n > C takes today's per-n path
+        self.prompt_capacity = None
         self.semantic_post_nms = semantic_post_nms
         self.panoptic_post_nms = panoptic_post_nms
         self.panoptic_configs = panoptic_configs if panoptic_configs is not None else {
@@ -424,6 +430,8 @@ class DeformableDETRSegmVL(nn.Module):
 
     # -- text routing (:166-360) -------------------------------------------------------------------
     def _text_features(self, batched_inputs):
+        self._prompt_from_call = False  # set below when the class names come from the call (what prompt_capacity pads)
+        self._fusion_from_text = False  # set below when the fusion input is the text's own tokens (padded with it)
         dataset_id = self.eval_dataset_id
         if dataset_id >= 0:
             prompt = self.dataset_prompts[dataset_id]
@@ -453,6 +461,7 @@ class DeformableDETRSegmVL(nn.Module):
         if prompt == "name":
             if text_list:
                 cache = False
+                self._prompt_from_call = True
             elif dataset_id >= 0:
                 text_list, cache = list(self.vocabulary[self.dataset_names[dataset_id]]), True
             else:
@@ -474,6 +483,7 @@ class DeformableDETRSegmVL(nn.Module):
             features_l = features_l.to(self.device).unsqueeze(0).repeat(bs, 1, 1)
             if self.name_prompt_fusion_text is not None and self.name_prompt_fusion_text[dataset_id]:
                 fusion = features_l
+                self._fusion_from_text = True
             elif self.name_prompt_fusion_feature is not None:
                 fusion = self.name_prompt_fusion_feature.repeat(bs, 1, 1)
             else:
@@ -482,6 +492,7 @@ class DeformableDETRSegmVL(nn.Module):
         # phrase / expression (:284-337)
         if not text_list:
             raise NotImplementedError("ape_b200: phrase prompts need `text_prompt` (or `expressions`) at inference")
+        self._prompt_from_call = self._fusion_from_text = True
         # a text tower that packs its prompts by length reads out the end-of-text rows alone when told that nothing else is wanted
         kw = {"need_hidden": False} if getattr(self.model_language, "pack_prompts", False) else {}
         features_l = self.model_language.forward_text(text_list, **kw)["last_hidden_state_eot"].to(self.device)
@@ -527,7 +538,13 @@ class DeformableDETRSegmVL(nn.Module):
         has_region = region is not None
         graphs = low and self.use_cuda_graphs and self._graph_prompt(prompt, fusion)
         need_masks = self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on)
-        if graphs and fusion is not None and fusion.shape[1] > 1:
+        # prompt_capacity: the text (and a fusion input of the same tokens) padded to C rows, its length n a graph input (ncls),
+        # one graph per padded shape from the first call on; the logits are cut back to n below
+        n_text, ncls = features_l.shape[1], None
+        if low and self.use_cuda_graphs and not self.profile_stages:
+            features_l, fusion, ncls = self._pad_prompt(features_l, fusion)
+            graphs = graphs or ncls is not None
+        if graphs and ncls is None and fusion is not None and fusion.shape[1] > 1:
             graphs = self._graph_seen((prompt, tuple(images.shape), tuple(features_l.shape), self.engine_dtype, need_masks,
                                        do_postprocess, self.profile_stages, has_region))
         with torch.autocast("cuda", dtype=self.engine_dtype, enabled=low):
@@ -571,9 +588,12 @@ class DeformableDETRSegmVL(nn.Module):
                 # the image sizes are a graph input like the image: the key holds the padded shape, not the sizes
                 (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                  init_reference, inter_references, mask_logits, graph_pack) = self._graphed(
-                    ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel, has_region),
-                    self._stage_all, (images, fusion, features_l, sizes, dims, region), const)
+                    ("forward", prompt, tuple(images.shape), tuple(features_l.shape), need_masks, sel,
+                     None if ncls is None else (0 if fusion is None else fusion.shape[1]), has_region),
+                    self._stage_all, (images, fusion, features_l, sizes, dims, region, ncls), const)
                 self.transformer.last_topk_proposals = topk
+                if ncls is not None:  # the padded class columns are -inf: what follows sees the n columns of an exact-n run
+                    box_cls = box_cls[..., :n_text]
                 mark("encode")
                 mark("select")
             else:
@@ -737,7 +757,7 @@ class DeformableDETRSegmVL(nn.Module):
         levels = [F.interpolate(mp[None], size=sh, mode="bilinear").to(torch.bool).squeeze(0) for sh in geo["shapes"]]
         return torch.cat([m.flatten(1) for m in levels], 1)
 
-    def _stage_encode(self, images, fusion, geo, region=None):
+    def _stage_encode(self, images, fusion, geo, region=None, n_tokens=None):
         """region: None, the padded uint8 map of `_mask_prompt` on CUDA (folded here into the anchors: ops.region_prompt), or
         the flattened bool mask of its host restatement (applied by stage_encode's masked_fill)."""
         proposals, mask_prompt_flatten = None, None
@@ -753,7 +773,7 @@ class DeformableDETRSegmVL(nn.Module):
             feats = tuple(features.values())
             flat = getattr(self.backbone, "last_flat", None)
         memory, fusion_out, output_memory, enc_cls, enc_coord = self.transformer.stage_encode(
-            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=flat, proposals=proposals)
+            feats, geo, fusion, mask_prompt_flatten=mask_prompt_flatten, feat_flatten=flat, proposals=proposals, n_tokens=n_tokens)
         mask_features = None
         if self.semantic_on or self.panoptic_on or (self.instance_on and self.test_mask_on):
             mask_features = self.maskdino_mask_features(memory, features, geo)
@@ -770,6 +790,51 @@ class DeformableDETRSegmVL(nn.Module):
             return True
         enc = self.transformer.encoder
         return all(vl is None or vl.b_attn.folds(enc.embed_dim, fusion.shape[-1], fusion.shape[1]) for vl in enc.vl_layers)
+
+    def _pad_prompt(self, features_l, fusion):
+        """(features_l, fusion, ncls) of a captured call.  With `prompt_capacity` C set, a text from the call (names, phrases or
+        expressions: not a cached vocabulary) of n <= C rows, and a fusion input that is one token, none, or the same n tokens
+        with every fusion layer on the folded path at C tokens (BiAttentionBlock.folds): the text features, and such a fusion
+        input, zero-padded to C rows, and n as int32 [1] on the device.  Otherwise the inputs and None.  n is the reference's
+        own length (for phrases with the text-feature bank, max(len(text_list), num_classes))."""
+        cap = self.prompt_capacity
+        if cap is None:
+            return features_l, fusion, None
+        if isinstance(cap, bool) or not isinstance(cap, int) or cap < 1:
+            raise ValueError(f"ape_b200: prompt_capacity must be None or an int >= 1 (got {cap!r})")
+        B, n, D = features_l.shape
+        if not getattr(self, "_prompt_from_call", False) or n > cap:
+            return features_l, fusion, None
+        # the text's own tokens as the fusion input (phrases, expressions, fused-vocabulary names), one token included
+        multi = fusion is not None and (fusion.shape[1] != 1 or getattr(self, "_fusion_from_text", False))
+        if multi:
+            enc = self.transformer.encoder
+            if fusion.shape[1] != n or cap < 2 or not all(
+                    vl is None or vl.b_attn.folds(enc.embed_dim, fusion.shape[-1], cap) for vl in enc.vl_layers):
+                return features_l, fusion, None
+            same = fusion is features_l
+            padded_f = fusion.new_zeros((B, cap, fusion.shape[-1]))
+            padded_f[:, :n] = fusion
+        padded = features_l.new_zeros((B, cap, D))
+        padded[:, :n] = features_l
+        if multi:
+            fusion = padded if same else padded_f
+        cache = self.__dict__.setdefault("_ncls_dev", {})
+        key = (n, str(self.device))
+        ncls = cache.get(key)
+        if ncls is None:  # read-only, cached per n: a repeated length costs no upload, a new one no host synchronisation
+            if len(cache) > 256:
+                cache.clear()
+            ncls = cache[key] = torch.tensor([n], dtype=torch.int32, pin_memory=True).to(self.device, non_blocking=True)
+        return padded, fusion, ncls
+
+    @staticmethod
+    def _class_ok(logits, ncls, shift=0):
+        """bool [N] over the class columns of logits: True for the first ncls - shift (ncls: int32 [1] on the device, the length of
+        a padded prompt; `shift` columns of the padded width were merged away before the padding), or None when ncls is None."""
+        if ncls is None:
+            return None
+        return torch.arange(logits.shape[-1], device=logits.device, dtype=torch.int32) < (ncls - shift)
 
     def _graph_seen(self, key):
         """Multi-token prompts: True the second time `key` is seen.  A new token count costs two eager warm-ups and a capture,
@@ -798,32 +863,33 @@ class DeformableDETRSegmVL(nn.Module):
         geo = self._size_geometry(padded, sizes, True)
         return self._stage_encode(images, fusion, geo, region) + (geo,)
 
-    def _stage_all(self, images, fusion, features_l, sizes, dims, region, padded, prompt, sel=None, size_columns=None):
+    def _stage_all(self, images, fusion, features_l, sizes, dims, region, ncls, padded, prompt, sel=None, size_columns=None):
         # inside a graph the padding mask is always passed: an all-false mask gives the values of None (masked_fill with no
         # true entry changes nothing), so one graph serves padded and unpadded sizes alike.  The region map (or None) is a graph
         # input too: one graph with a region and one without per padded shape, whatever the prompt
         geo = self._size_geometry(padded, sizes, True)
+        n_tokens = ncls if ncls is not None and fusion is not None and fusion.shape[1] == features_l.shape[1] > 1 else None  # padded fusion
         memory, fusion_out, output_memory, enc_cls, enc_coord, features, feats, mask_features = self._stage_encode(
-            images, fusion, geo, region)
+            images, fusion, geo, region, n_tokens)
         topk = self.transformer.stage_select(enc_cls, enc_coord, geo)
         features_l = self._mix_text(prompt, features_l, fusion_out)
         box_cls, box_pred, inter_states, init_reference, inter_references, mask_logits = self._stage_decode(
-            topk, features_l, memory, output_memory, enc_coord, geo, mask_features)
+            topk, features_l, memory, output_memory, enc_coord, geo, mask_features, ncls)
         pack = None
         if sel is not None:  # (class-wise path?, thresholds ..., instance branch on?) — see forward()
             det_cls = self._detector_box_cls(box_cls) if sel[6] else box_cls
-            pack = self._select_device(det_cls, box_pred, sizes, sel[0])
+            pack = self._select_device(det_cls, box_pred, sizes, sel[0], ncls)
             if len(sel) > 7:  # sel[7] = (image sizes, output sizes, mask slot bytes or None, semantic / panoptic configuration[, C])
                 image_sizes, out_sizes, mask_slot, sem, pan = sel[7][:5]
                 cap = sel[7][5] if len(sel[7]) > 5 else None
                 if cap is not None:  # capacity mode: the size columns come from the device sizes (exact in fp32)
                     size_columns = dims.to(torch.float32)
                 pack = self._pack_rows(pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, tuple(images.shape[-2:]),
-                                       sel[0], out_sizes, mask_slot, sem, pan, dims=dims, cap=cap)
+                                       sel[0], out_sizes, mask_slot, sem, pan, dims=dims, cap=cap, ncls=ncls)
         return (memory, output_memory, enc_cls, enc_coord, features, feats, topk, box_cls, box_pred, inter_states,
                 init_reference, inter_references, mask_logits, pack)
 
-    def _stage_decode(self, topk, features_l, memory, output_memory, enc_coord, geo, mask_features=None):
+    def _stage_decode(self, topk, features_l, memory, output_memory, enc_coord, geo, mask_features=None, ncls=None):
         inter_states, init_reference, inter_references = self.transformer.stage_decode(
             memory, output_memory, enc_coord, topk, geo)
         states16 = inter_states  # decoder outputs are LayerNorm outputs in the engine dtype
@@ -834,10 +900,10 @@ class DeformableDETRSegmVL(nn.Module):
         with torch.autocast("cuda", enabled=False):
             if states16.dtype in (torch.float16, torch.bfloat16):
                 # engine: query x text logits and the box MLP on the tensor cores (fp32 accumulation, fp32 outputs)
-                box_cls = self.class_embed[lvl](states16[lvl], features_l.float())
+                box_cls = self.class_embed[lvl](states16[lvl], features_l.float(), ncls)
                 box_pred = (self.bbox_embed[lvl](states16[lvl], out_dtype=torch.float32) + inverse_sigmoid(reference)).sigmoid()
             else:
-                box_cls = self.class_embed[lvl](inter_states[lvl], features_l.float())
+                box_cls = self.class_embed[lvl](inter_states[lvl], features_l.float(), ncls)
                 box_pred = (self.bbox_embed[lvl](inter_states[lvl]) + inverse_sigmoid(reference)).sigmoid()
         mask_logits = None
         if mask_features is not None:
@@ -1065,9 +1131,11 @@ class DeformableDETRSegmVL(nn.Module):
                                      pred_classes=p[:, 5].to(torch.int64), query_index=p[:, 6].to(torch.int64)))
         return results
 
-    def _select_device(self, box_cls, box_pred, sizes, classwise):
+    def _select_device(self, box_cls, box_pred, sizes, classwise, ncls=None, shift=0):
         """Device half of `_inference_static`: [B, topk, 9] fp32 = (x1, y1, x2, y2, score, class, query index, number of
-        candidates, number kept) per detection slot; static shapes, no host synchronisation (CUDA-graph / NCCL friendly)."""
+        candidates, number kept) per detection slot; static shapes, no host synchronisation (CUDA-graph / NCCL friendly).
+        ncls / shift: the class columns of a padded prompt (`_class_ok`); the others are never candidates."""
+        col_ok = self._class_ok(box_cls, ncls, shift)
         cap, topk = int(self.static_inference_cap), int(self.test_topk_per_image)
         # sizes: int32 [B, 2] (h, w) on the device (a graph input), so the fp32 scaling and clamp below read them from device memory
         hw = sizes.to(device=box_cls.device, dtype=torch.float32)
@@ -1083,11 +1151,14 @@ class DeformableDETRSegmVL(nn.Module):
             boxes = torch.stack((boxes[:, 0].clamp(min=zero, max=w), boxes[:, 1].clamp(min=zero, max=h),
                                  boxes[:, 2].clamp(min=zero, max=w), boxes[:, 3].clamp(min=zero, max=h)), dim=-1).contiguous()
             mask = (scores > self.test_score_thresh) & valid[:, None]
+            if col_ok is not None:  # row-major order of the real pairs is kept, so the compacted list is the exact-n run's
+                mask = mask & col_ok
             n = mask.sum().to(torch.int32).reshape(1)
             Q, N = scores.shape
             if classwise:
                 k = min(topk, Q * N)
-                surv = ops.nms_classwise(boxes, scores, self.test_score_thresh, self.test_nms_thresh,
+                cw_scores = scores if col_ok is None else scores.masked_fill(~col_ok, float("-inf"))
+                surv = ops.nms_classwise(boxes, cw_scores, self.test_score_thresh, self.test_nms_thresh,
                                          row_valid=valid.to(torch.uint8))                   # [N, Q], -inf = gone
                 topv, topi = torch.topk(surv.flatten(), k)                                  # descending score
                 c, q = topi // Q, topi % Q
@@ -1261,12 +1332,13 @@ class DeformableDETRSegmVL(nn.Module):
                                  f"model.panoptic_slot_bytes is {slot}")
 
     def _pack_rows(self, pack, size_columns, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes,
-                   mask_slot, sem, pan=None, dims=None, cap=None):
+                   mask_slot, sem, pan=None, dims=None, cap=None, ncls=None):
         """Selection rows [B, topk, 9] + size columns -> what forward_packed returns: fp32 [B, topk, 13] rows, or uint8
         [B, topk, 60 + mask_slot] with the kept masks' run-length codes (mask_slot not None); with a semantic configuration
         (`_packed_semantic_config`) or a panoptic one (`_packed_panoptic_config`) each image's header, those rows as bytes, its
         semantic slot (empty without one) and its panoptic slot (none without one).  No host synchronisation.  With a capacity cap,
-        the stages read the sizes from dims (int32 [B, 4] on the device) and image_sizes / out_sizes are not used."""
+        the stages read the sizes from dims (int32 [B, 4] on the device) and image_sizes / out_sizes are not used.  ncls: the class
+        count of a padded prompt (`_pad_prompt`), or None."""
         rows = torch.cat([pack, size_columns[:, None, :].expand(-1, pack.shape[1], -1)], dim=2)
         if mask_slot is not None:
             if cap is not None:
@@ -1285,10 +1357,10 @@ class DeformableDETRSegmVL(nn.Module):
         info = torch.zeros((B, 3), dtype=torch.int32, device=rows.device)  # kind, bytes used, labels present
         if sem is not None:
             self._pack_semantic(sem, out[:, ops.SEM_PACK_HEAD + det.shape[1]:ops.SEM_PACK_HEAD + det.shape[1] + sem_bytes], info, pack,
-                                box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes, dims, cap)
+                                box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes, dims, cap, ncls)
         if pan is not None:
             self._pack_panoptic(pan, out[:, out.shape[1] - pan_bytes:], pack, box_cls, box_pred, mask_logits, sizes, image_sizes,
-                                padded_hw, classwise, out_sizes, dims, cap)
+                                padded_hw, classwise, out_sizes, dims, cap, ncls)
         hdr = torch.zeros((B, 8), dtype=torch.int32, device=rows.device)
         hdr[:, 0], hdr[:, 1] = topk, R
         hdr[:, 2:4] = info[:, 0:2]
@@ -1299,32 +1371,34 @@ class DeformableDETRSegmVL(nn.Module):
         return out
 
     def _pack_semantic(self, sem, slots, info, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise,
-                       out_sizes, dims=None, cap=None):
+                       out_sizes, dims=None, cap=None, ncls=None):
         """The semantic slots [B, slot] of `_pack_rows` and their (kind, bytes used, labels present) in info [B, 3]."""
         slot, on, post_nms, class0, things, stuff, entity = sem
         B = slots.shape[0]
         if on:
             sem_cls = get_stuff_score(box_cls, list(things), list(stuff), entity)
+            shift = box_cls.shape[-1] - sem_cls.shape[-1]  # the thing columns merged into one by get_stuff_score
+            col_ok = self._class_ok(sem_cls, ncls, shift)
             if post_nms and self.instance_on and not (self.eval_dataset_entity and "thing" not in self.eval_dataset_entity) and \
                     self._detector_box_cls(box_cls) is box_cls and sem_cls.shape == box_cls.shape:
                 keep = pack  # _semantic reuses the instance branch's kept queries in this case
             elif post_nms:
-                keep = self._select_device(sem_cls, box_pred, sizes, classwise)
+                keep = self._select_device(sem_cls, box_pred, sizes, classwise, ncls, shift)
             else:
                 keep = None
             if cap is not None:
                 labels = torch.stack([self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw,
-                                                                  None, None, class0, dims[b], cap) for b in range(B)])
+                                                                  None, None, class0, dims[b], cap, col_ok) for b in range(B)])
                 ops.semseg_pack_dev(labels, dims, cap, sem_cls.shape[-1], slots, info)
                 return
             labels = [self._semantic_label_static(sem_cls[b], mask_logits[b], None if keep is None else keep[b], padded_hw, image_sizes[b],
-                                                  out_sizes[b], class0) for b in range(B)]
+                                                  out_sizes[b], class0, col_ok=col_ok) for b in range(B)]
             ops.semseg_pack(labels, sem_cls.shape[-1], slots, info)
         else:
             slots.zero_()
 
     def _pack_panoptic(self, pan, slots, pack, box_cls, box_pred, mask_logits, sizes, image_sizes, padded_hw, classwise, out_sizes,
-                       dims=None, cap=None):
+                       dims=None, cap=None, ncls=None):
         """The panoptic slots [B, slot] of `_pack_rows`: `_panoptic`'s merge with K = topk queries whatever the kept count (every
         query without panoptic_post_nms), no host synchronisation.  The rows of the selection at or past the kept count and the
         queries under object_mask_threshold get the score -inf, so they take no part (ops.panoptic_winners)."""
@@ -1339,9 +1413,10 @@ class DeformableDETRSegmVL(nn.Module):
         if post_nms and self.instance_on and not (ent and "thing" not in ent) and self._detector_box_cls(box_cls) is box_cls:
             keep = pack  # _panoptic reuses the instance branch's kept queries in this case
         elif post_nms:
-            keep = self._select_device(box_cls, box_pred, sizes, classwise)
+            keep = self._select_device(box_cls, box_pred, sizes, classwise, ncls)
         else:
             keep = None
+        col_ok = self._class_ok(box_cls, ncls)
         B, Q = box_cls.shape[0], box_cls.shape[1]
         stuff_first = bool(stuff) and stuff[0] == "things"
         for b in range(B):
@@ -1350,7 +1425,7 @@ class DeformableDETRSegmVL(nn.Module):
             else:
                 qi = keep[b, :, 6].to(torch.int64).clamp(0, Q - 1)
                 live = torch.arange(keep.shape[1], device=keep.device) < keep[b, :, 8].to(torch.int64)
-            scores, labels, kept = _query_scores(box_cls[b, qi].float(), cfg)
+            scores, labels, kept = _query_scores(box_cls[b, qi].float(), cfg, col_ok)
             if live is not None:
                 kept = kept & live
             scores = torch.where(kept, scores, float("-inf"))
@@ -1363,18 +1438,23 @@ class DeformableDETRSegmVL(nn.Module):
             ops.panoptic_pack(ids, counts, labels.to(torch.int32), box_cls.shape[-1], len(things), stuff_first, overlap_threshold,
                               slots[b])
 
-    def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0, dims=None, cap=None):
+    def _semantic_label_static(self, sem_cls, mask_logits, keep, padded_hw, size, out_hw, class0, dims=None, cap=None, col_ok=None):
         """`_semantic`'s label map of one image with K = topk queries whatever the kept count (no host synchronisation): the
         rows of `keep` ([topk, 9] selection rows, None = every query) at or past the kept count get zero class weights, so the
         class GEMM adds exact zeros for them.  With a capacity cap the sizes are dims ([4] on the device) and the map is
-        ops.semseg_label_dev's [cap * cap] buffer."""
+        ops.semseg_label_dev's [cap * cap] buffer.  col_ok: the class columns of a padded prompt (`_class_ok`); the others take no
+        part in the softmax and get zero weight, so they never win the label GEMM's first argmax (the real columns come first and
+        their weighted sums are never negative)."""
         Q = sem_cls.shape[0]
         if keep is None:
             qi, live = torch.arange(Q, device=sem_cls.device), None
         else:
             qi = keep[:, 6].to(torch.int64).clamp(0, Q - 1)
             live = torch.arange(keep.shape[0], device=keep.device) < keep[:, 8].to(torch.int64)
-        cls = F.softmax(sem_cls[qi].float().sigmoid() / 0.06, dim=-1)
+        logits = sem_cls[qi].float().sigmoid() / 0.06
+        if col_ok is not None:
+            logits = logits.masked_fill(~col_ok, float("-inf"))
+        cls = F.softmax(logits, dim=-1)
         if live is not None:
             cls = torch.where(live[:, None], cls, cls.new_zeros(()))
         if cap is not None:

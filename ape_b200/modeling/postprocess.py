@@ -14,13 +14,17 @@ import torch
 import torch.nn.functional as F
 
 
-def _query_scores(mask_cls: torch.Tensor, cfg: Dict) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+def _query_scores(mask_cls: torch.Tensor, cfg: Dict, col_ok=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """(scores, labels, keep) of all K queries: the class scores and labels the merge ranks them by, and the queries above
-    object_mask_threshold (on the sigmoid scores, before the transform_eval softmax)."""
-    scores, labels = mask_cls.sigmoid().max(-1)
+    object_mask_threshold (on the sigmoid scores, before the transform_eval softmax).  col_ok: bool [N], the class columns of a
+    padded prompt; the others never win the maximum and take no part in the softmax."""
+    sig = mask_cls.sigmoid()
+    if col_ok is not None:
+        sig = sig.masked_fill(~col_ok, float("-inf"))
+    scores, labels = sig.max(-1)
     keep = scores > cfg["object_mask_threshold"]
     if cfg["transform_eval"]:
-        scores, labels = F.softmax(mask_cls.sigmoid() / cfg["pano_temp"], dim=-1).max(-1)
+        scores, labels = F.softmax(sig / cfg["pano_temp"], dim=-1).max(-1)
     return scores, labels, keep
 
 

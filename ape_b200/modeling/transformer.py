@@ -173,11 +173,11 @@ class DeformableDetrTransformerEncoderVL(nn.Module):
         self.record_taps = False  # tests: keep per-layer outputs ("vlf{i}.v" after the fusion, "enc{i}" after the layer) in self.taps
 
     def forward(self, query, key, value, query_l, attention_mask_l, query_pos=None, key_pos=None, attn_masks=None,
-                query_key_padding_mask=None, key_padding_mask=None, **kwargs):
+                query_key_padding_mask=None, key_padding_mask=None, n_tokens=None, **kwargs):
         engine_dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else None
         if engine_dtype is not None:
             query, query_pos = query.to(engine_dtype), query_pos.to(engine_dtype)
-            if query_l is not None and query_l.shape[1] == 1 and attention_mask_l is None and query.shape[-1] % 8 == 0 \
+            if query_l is not None and query_l.shape[1] == 1 and n_tokens is None and attention_mask_l is None and query.shape[-1] % 8 == 0 \
                     and all(v is not None and not v.b_attn.attn.use_attention_mask_v for v in self.vl_layers):
                 return self._engine_single_token(query.contiguous(), query_pos.contiguous(), query_l,
                                                  query_key_padding_mask, kwargs)
@@ -186,7 +186,7 @@ class DeformableDetrTransformerEncoderVL(nn.Module):
         for i, (vl_layer, layer) in enumerate(zip(self.vl_layers, self.layers)):
             if vl_layer is not None and query_l is not None:
                 query, query_l = vl_layer(query, query_l, attention_mask_v=query_key_padding_mask,
-                                          attention_mask_l=attention_mask_l)
+                                          attention_mask_l=attention_mask_l, n_tokens=n_tokens)
                 if engine_dtype is not None:
                     query = query.to(engine_dtype)
                 if self.record_taps:
@@ -482,17 +482,18 @@ class DeformableDetrTransformerVL(nn.Module):
         del g["pos_flatten"]
         return dict(padded, **g, has_padding=has_padding)
 
-    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l):
-        """The encoder call of stage_encode -> (memory, language features after the fusion layers)."""
+    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l, n_tokens=None):
+        """The encoder call of stage_encode -> (memory, language features after the fusion layers).  n_tokens: the length of a
+        padded text (int32 [1] on the device), or None."""
         return self.encoder(
-            query=feat_flatten, key=None, value=None, query_l=query_l, attention_mask_l=attention_mask_l,
+            query=feat_flatten, key=None, value=None, query_l=query_l, attention_mask_l=attention_mask_l, n_tokens=n_tokens,
             query_pos=pos_flatten, query_key_padding_mask=geo["mask_flatten"] if geo["has_padding"] else None,
             spatial_shapes=geo["spatial_shapes"], reference_points=geo["reference_points"],
             level_start_index=geo["level_start_index"], valid_ratios=geo["valid_ratios"],
             host_shapes=geo["shapes"])
 
     def stage_encode(self, multi_level_feats, geo, query_l, attention_mask_l=None, mask_prompt_flatten=None,
-                     feat_flatten=None, proposals=None):
+                     feat_flatten=None, proposals=None, n_tokens=None):
         """feat_flatten: optional [B,S,C] tensor that already holds the flattened levels (the engine neck writes its
         outputs straight into it; `multi_level_feats` are then views of its slices).  Region prompts: `proposals`, the pair
         (output_proposals, proposal_invalid) with the region already folded in (ops.region_prompt, CUDA), replaces the
@@ -510,7 +511,7 @@ class DeformableDetrTransformerVL(nn.Module):
                                            for i, (h, w) in enumerate(geo["shapes"])], 1)
                     cache[engine_dtype] = (ck, (geo["pos_flatten"] + lvl_embed.float()).to(engine_dtype).contiguous())
             pos_flatten = cache[engine_dtype][1]
-        memory, query_l = self._encode(feat_flatten, pos_flatten, geo, query_l, attention_mask_l)
+        memory, query_l = self._encode(feat_flatten, pos_flatten, geo, query_l, attention_mask_l, n_tokens)
         # gen_encoder_output_proposals (:354-369): zero the memory of invalid anchors, project, normalise
         output_proposals, invalid = proposals if proposals is not None else (geo["output_proposals"], geo["proposal_invalid"])
         if mask_prompt_flatten is not None:
@@ -700,8 +701,8 @@ class DeformableDetrTransformer(DeformableDetrTransformerVL):
     def gen_encoder_output_proposals(self, memory, memory_padding_mask, spatial_shapes):
         return super().gen_encoder_output_proposals(memory, memory_padding_mask, spatial_shapes)
 
-    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l):
-        if query_l is not None or attention_mask_l is not None:
+    def _encode(self, feat_flatten, pos_flatten, geo, query_l, attention_mask_l, n_tokens=None):
+        if query_l is not None or attention_mask_l is not None or n_tokens is not None:
             raise ValueError("ape_b200.DeformableDetrTransformer has no fusion layers: language features go to the classifier")
         memory = self.encoder(
             query=feat_flatten, key=None, value=None, query_pos=pos_flatten,

@@ -256,6 +256,32 @@ def linear_tc(x, weight, bias=None, act=None, out_dtype=None, residual=None, til
     return (res, stats) if stats_out else res
 
 
+def linear_cols_dev(x, weight, bias, n_cols):
+    """linear_tc(x, weight, bias, act="clamp", out_dtype=torch.float32) over the first n_cols rows of weight, -inf in the columns
+    past them (ape_gemm_tn_cols_dev): the vision-language logits of a vocabulary padded to weight.shape[0] rows, whose true length
+    n_cols (int32 [1] on the device) is read by the kernel, so one CUDA graph serves every length.  x [M, K] and weight [N, K]
+    fp16 / bf16 with 16-byte aligned rows, bias fp32 [N] or None.  Returns fp32 [M, N]."""
+    _require(x.is_cuda and weight.is_cuda and n_cols.is_cuda, "linear_cols_dev: CUDA tensors only")
+    _require(x.dtype == weight.dtype and x.dtype in (torch.float16, torch.bfloat16), "linear_cols_dev: fp16/bf16 operands")
+    _require(x.dim() == 2 and weight.dim() == 2 and x.shape[1] == weight.shape[1] and x.stride(1) == 1 and weight.stride(1) == 1,
+             "linear_cols_dev: x [M, K] and weight [N, K] with unit inner stride")
+    _require(n_cols.dtype == torch.int32 and n_cols.numel() == 1, "linear_cols_dev: n_cols must be int32 [1]")
+    if bias is not None:
+        _require(bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == weight.shape[0],
+                 "linear_cols_dev: bias must be fp32 [N]")
+    if x.stride(0) % 8 or x.data_ptr() % 16:
+        x = x.contiguous()
+    M, K = x.shape
+    N = weight.shape[0]
+    out = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device), _timed(("gemm_tn_cols_dev", M, N, K)):
+        rc = _lib.lib.ape_gemm_tn_cols_dev(x.data_ptr(), x.stride(0), weight.data_ptr(), weight.stride(0), out.data_ptr(), N,
+                                           bias.data_ptr() if bias is not None else None, M, N, K, n_cols.data_ptr(),
+                                           _lib.dtype_code(x.dtype), _lib.current_stream_ptr())
+    _lib.check(rc, "ape_gemm_tn_cols_dev")
+    return out
+
+
 def quantize_rows_e4m3(w):
     """(q, scale): per-row e4m3 quantisation of a 2-D tensor, computed in fp32 on its device: scale = max|row| / 448 (1 for
     an all-zero row), q = e4m3(row / scale) rounded to nearest even.  Weight preparation for linear_fp8, done once."""
@@ -662,10 +688,16 @@ def _check_fold_operands(v, qa, name):
     return B, v.shape[1], qa.shape[2], qa.shape[1]
 
 
-def vlf_fold_vision(v, qa, u, qc, gamma, bias, out=None):
+def _check_n_dev(n_dev, what):
+    _require(n_dev is None or (n_dev.is_cuda and n_dev.dtype == torch.int32 and n_dev.numel() == 1),
+             f"{what}: n_dev must be an int32 [1] CUDA tensor")
+
+
+def vlf_fold_vision(v, qa, u, qc, gamma, bias, out=None, n_dev=None):
     """v + gamma * (sum_h sum_n softmax_n(v . qa[:,h,n] + qc[:,h,n]) u[:,h,n] + bias) over all S rows (ape_vlf_fold_vision).
     v [B,S,256] fp16/bf16; qa / u [B,NH,N,256] contiguous, dtype of v; qc fp32 [B,NH,N]; gamma / bias fp32 [256].
-    Returns [B,S,256] in the dtype of v (`out` may be given, v itself included)."""
+    Returns [B,S,256] in the dtype of v (`out` may be given, v itself included).  n_dev (int32 [1] on the device, or None): the
+    text is padded to N tokens and only the first n_dev are keys (ape_vlf_fold_vision_dev)."""
     B, S, N, NH = _check_fold_operands(v, qa, "vlf_fold_vision")
     _require(u.shape == qa.shape and u.dtype == v.dtype and u.is_contiguous(), "vlf_fold_vision: u must be like qa")
     _require(qc.dtype == torch.float32 and qc.is_contiguous() and tuple(qc.shape) == (B, NH, N), "vlf_fold_vision: qc fp32 [B,NH,N]")
@@ -675,24 +707,37 @@ def vlf_fold_vision(v, qa, u, qc, gamma, bias, out=None):
         out = torch.empty((B, S, 256), dtype=v.dtype, device=v.device)
     _require(out.shape == v.shape and out.dtype == v.dtype and out.stride(2) == 1 and out.stride(0) == S * out.stride(1),
              "vlf_fold_vision: bad `out`")
+    _check_n_dev(n_dev, "vlf_fold_vision")
     with torch.cuda.device(v.device), _timed(("vlf_fold_vision", B, S, N, NH)):
-        rc = _lib.lib.ape_vlf_fold_vision(v.data_ptr(), v.stride(1), qa.data_ptr(), u.data_ptr(), qc.data_ptr(), gamma.data_ptr(),
-                                          bias.data_ptr(), out.data_ptr(), out.stride(1), B, S, N, NH, 256, _lib.dtype_code(v.dtype),
-                                          _lib.current_stream_ptr())
+        if n_dev is None:
+            rc = _lib.lib.ape_vlf_fold_vision(v.data_ptr(), v.stride(1), qa.data_ptr(), u.data_ptr(), qc.data_ptr(), gamma.data_ptr(),
+                                              bias.data_ptr(), out.data_ptr(), out.stride(1), B, S, N, NH, 256, _lib.dtype_code(v.dtype),
+                                              _lib.current_stream_ptr())
+        else:
+            rc = _lib.lib.ape_vlf_fold_vision_dev(v.data_ptr(), v.stride(1), qa.data_ptr(), u.data_ptr(), qc.data_ptr(),
+                                                  gamma.data_ptr(), bias.data_ptr(), out.data_ptr(), out.stride(1), B, S, N, NH,
+                                                  n_dev.data_ptr(), 256, _lib.dtype_code(v.dtype), _lib.current_stream_ptr())
     _lib.check(rc, "ape_vlf_fold_vision")
     return out
 
 
-def vlf_fold_pool(v, qa):
+def vlf_fold_pool(v, qa, n_dev=None):
     """sum_s softmax_s(v_s . qa[:,h,n]) v_s for every head h and token n (ape_vlf_fold_pool: S split across the SMs, the chunks
     combined in a fixed order).  v [B,S,256] fp16/bf16, qa [B,NH,N,256] contiguous in the dtype of v.
-    Returns [B*N, NH*256] in the dtype of v (row b*N + n, head h at columns h*256)."""
+    Returns [B*N, NH*256] in the dtype of v (row b*N + n, head h at columns h*256).  n_dev (int32 [1] on the device, or None):
+    tokens n >= n_dev are padding and their rows are zeros (ape_vlf_fold_pool_dev; the split is chosen from N)."""
     B, S, N, NH = _check_fold_operands(v, qa, "vlf_fold_pool")
     pooled = torch.empty((B * N, NH * 256), dtype=v.dtype, device=v.device)
     ws = torch.empty((int(_lib.lib.ape_vlf_fold_pool_workspace_bytes(B, S, N, NH)) // 4,), dtype=torch.float32, device=v.device)
+    _check_n_dev(n_dev, "vlf_fold_pool")
     with torch.cuda.device(v.device), _timed(("vlf_fold_pool", B, S, N, NH)):
-        rc = _lib.lib.ape_vlf_fold_pool(v.data_ptr(), v.stride(1), qa.data_ptr(), ws.data_ptr(), pooled.data_ptr(), pooled.stride(0),
-                                        B, S, N, NH, 256, _lib.dtype_code(v.dtype), _lib.current_stream_ptr())
+        if n_dev is None:
+            rc = _lib.lib.ape_vlf_fold_pool(v.data_ptr(), v.stride(1), qa.data_ptr(), ws.data_ptr(), pooled.data_ptr(),
+                                            pooled.stride(0), B, S, N, NH, 256, _lib.dtype_code(v.dtype), _lib.current_stream_ptr())
+        else:
+            rc = _lib.lib.ape_vlf_fold_pool_dev(v.data_ptr(), v.stride(1), qa.data_ptr(), ws.data_ptr(), pooled.data_ptr(),
+                                                pooled.stride(0), B, S, N, NH, n_dev.data_ptr(), 256, _lib.dtype_code(v.dtype),
+                                                _lib.current_stream_ptr())
     _lib.check(rc, "ape_vlf_fold_pool")
     return pooled
 

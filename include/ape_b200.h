@@ -382,6 +382,22 @@ int ape_vlf_fold_pool(const void *v, int64_t ldv, const void *qa, void *workspac
                       int NH, int C, int dtype, void *stream);
 
 /*
+ * The same for a text padded to N tokens per (b, h) block, of which the first *n_dev (device int32, clamped to [1, N]) are real,
+ * so that one CUDA graph serves every prompt length up to N.  Launches, workspaces and the pooling's split over S are sized from
+ * N; the arithmetic follows the padded shape, never *n_dev, so a replay is deterministic whatever the prompt.
+ *   ape_vlf_fold_vision_dev  ape_vlf_fold_vision with the keys >= *n_dev at -inf (their key blocks are not loaded).
+ *   ape_vlf_fold_pool_dev    ape_vlf_fold_pool for the rows of tokens < *n_dev; the rows of padding tokens are written as zeros.
+ *                            workspace: ape_vlf_fold_pool_workspace_bytes(B, S, N, NH).
+ * Both: no allocation, no synchronisation, capturable; bad arguments are reported (APE_ERR_*) before any launch.  Separate kernel
+ * instantiations: the kernels of the two entry points above are unchanged.
+ */
+int ape_vlf_fold_vision_dev(const void *v, int64_t ldv, const void *qa, const void *u, const float *qc, const float *gamma,
+                            const float *bias, void *out, int64_t ldo, int B, int S, int N, int NH, const int *n_dev, int C, int dtype,
+                            void *stream);
+int ape_vlf_fold_pool_dev(const void *v, int64_t ldv, const void *qa, void *workspace, void *pooled, int64_t ldp, int B, int S, int N,
+                          int NH, const int *n_dev, int C, int dtype, void *stream);
+
+/*
  * Greedy hard NMS over boxes already sorted by descending score (torchvision.ops.nms semantics; replaces the
  * nms call inside batched_nms of deformable_transformer_vl.py:591-596 and fast_rcnn.py:192).
  * boxes_sorted [n,4] fp32 xyxy (16-byte aligned); keep [n] bytes (1 = survives); *count = survivors (device int).
@@ -614,6 +630,18 @@ int ape_panoptic_winners_dev(const void *logits, const int64_t *index, const flo
 int ape_panoptic_pack_dev(const int *ids, const int *counts, const int *classes, int K, int num_classes, int num_things, int stuff_first,
                           double overlap_threshold, const int *sizes, int cap, void *workspace, uint8_t *slot, int slot_bytes,
                           void *stream);
+
+/*
+ * Vision-language logits of a text padded to a capacity: one CUDA graph serves every prompt length up to N.
+ *   ape_gemm_tn_cols_dev  C [M, N] fp32 (pitch ldc) = clamp(A W^T + bias, -50000, 50000) over columns [0, *n_cols) and -inf over
+ *                         [*n_cols, N) (n_cols: device int32; a count outside [0, N] changes values, never addresses).  A [M, K] and
+ *                         W [N, K] fp16 / bf16 as ape_gemm_tn; bias fp32 [N] or NULL.  A column in use equals the one
+ *                         ape_gemm_tn(act clamp, fp32 out) gives with W cut to its first *n_cols rows.  No allocation, no
+ *                         synchronisation, capturable; bad arguments return APE_ERR_INVALID_ARG (NULL pointers
+ *                         APE_ERR_NULL_PTR) before any launch.  A separate instantiation: the other GEMM kernels are unchanged.
+ */
+int ape_gemm_tn_cols_dev(const void *A, int64_t lda, const void *W, int64_t ldw, float *C, int64_t ldc, const float *bias, int M, int N,
+                         int K, const int *n_cols, int in_dtype, void *stream);
 
 /*
  * Per-image-size geometry of the deformable transformer for a padded batch (DeformableDetrTransformerVL.geometry and the sine
