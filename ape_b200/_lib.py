@@ -158,6 +158,12 @@ def _declare(lib):
     lib.ape_resample_coeffs_u8.argtypes = [_i, _i, _vp, _vp]
     lib.ape_resample_u8.restype = _i
     lib.ape_resample_u8.argtypes = [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _vp, _vp, _i] + [_i] * 6 + [_vp]
+    lib.ape_jpeg_workspace_bytes.restype = _i64
+    lib.ape_jpeg_workspace_bytes.argtypes = [_i, _vp] + [_i] * 4
+    lib.ape_jpeg_decode.restype = _i
+    lib.ape_jpeg_decode.argtypes = [_vp, _i, _vp, _i, _vp, _vp] + [_i] * 4 + [_vp, _i, _i, _vp, _i64, _vp, _vp, _vp]
+    lib.ape_jpeg_status_error.restype = _i
+    lib.ape_jpeg_status_error.argtypes = [_i]
     lib.ape_semseg_resample.restype = _i
     lib.ape_semseg_resample.argtypes = [_vp, _vp, _vp, _i64] + [_i] * 13 + [_vp]
     lib.ape_semseg_keys_init.restype = _i
@@ -274,6 +280,9 @@ EXPORTS = (
     "ape_resample_ksize",
     "ape_resample_coeffs_u8",
     "ape_resample_u8",
+    "ape_jpeg_workspace_bytes",
+    "ape_jpeg_decode",
+    "ape_jpeg_status_error",
     "ape_semseg_resample",
     "ape_semseg_keys_init",
     "ape_gemm_tn_argmax",

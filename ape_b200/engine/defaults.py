@@ -146,12 +146,7 @@ class DefaultPredictor:
         if not (isinstance(image, np.ndarray) and image.dtype == np.uint8):
             return image
         n = int(image.size)
-        ent = self._staging[slot]
-        if ent is None or ent[0].numel() < n:
-            buf = torch.empty((max(n, 1 << 22),), dtype=torch.uint8, pin_memory=True)
-            ent = self._staging[slot] = (buf, buf.numpy())  # the numpy view shares the pinned pages
-        if self._staged[slot] is not None:
-            self._staged[slot].synchronize()  # the previous upload out of this buffer has finished
+        ent = self._stage(slot, n)
         np.copyto(ent[1][:n].reshape(image.shape), image)  # one plain memcpy (a torch CPU copy_ spins up the intra-op pool)
         dev = ent[0][:n].view(image.shape).to(self.device, non_blocking=True)
         if self._staged[slot] is None:
@@ -159,11 +154,56 @@ class DefaultPredictor:
         self._staged[slot].record(torch.cuda.current_stream(self.device))
         return dev
 
+    def _stage(self, slot, n):
+        """The pinned staging buffer of `slot` with room for n bytes, once the previous upload out of it has finished."""
+        ent = self._staging[slot]
+        if ent is None or ent[0].numel() < n:
+            buf = torch.empty((max(n, 1 << 22),), dtype=torch.uint8, pin_memory=True)
+            ent = self._staging[slot] = (buf, buf.numpy())  # the numpy view shares the pinned pages
+        if self._staged[slot] is not None:
+            self._staged[slot].synchronize()  # the previous upload out of this buffer has finished
+        return ent
+
+    def _decode(self, source, slot):
+        """A JPEG path or file bytes -> the device uint8 HWC image in the model's channel order (ape_b200.engine.read_image).
+        The compressed bytes go through the slot's pinned staging buffer and the decode runs on a side stream: the host waits
+        for the decode alone (to read its status), not for the forward already queued on the current stream, which then
+        waits for the image."""
+        from .read import decode, file_bytes
+
+        data = file_bytes(source)
+        main = torch.cuda.current_stream(self.device)
+        if self._side is None:
+            self._side = torch.cuda.Stream(self.device)
+        ent = self._stage(slot, 3 * len(data) + (1 << 16))  # scan + decoder tables + restart offsets (4 bytes per 2-byte marker)
+        done = torch.cuda.Event()
+        with torch.cuda.stream(self._side):
+            image, status, _ = decode(data, self.input_format, self.device, host=ent[0])
+            if self._staged[slot] is None:
+                self._staged[slot] = torch.cuda.Event()
+            self._staged[slot].record(self._side)
+            done.record(self._side)
+            if status is not None:
+                ops.jpeg_check(status)  # reads the status word on the side stream: waits for the decode only
+        main.wait_event(done)
+        image.record_stream(main)
+        return image
+
     def preprocess(self, original_image, text_prompt=None, mask_prompt=None, slot=0):
-        """defaults.py:216-229 up to the model call: the input dict, with `image` resized on the device."""
-        height, width = original_image.shape[:2]
-        tfm = self.aug.get_transform(original_image)
-        image = tfm.apply_image(self._upload(original_image, slot), device=self.device, flip_channels=self.input_format == "RGB")
+        """defaults.py:216-229 up to the model call: the input dict, with `image` resized on the device.  original_image: the
+        BGR uint8 array of the reference, or a JPEG file (path or bytes), decoded on the device as read_image(path, format)
+        would on the host; height / width are then those of the EXIF-oriented image."""
+        from .read import is_encoded
+
+        if is_encoded(original_image):
+            decoded = self._decode(original_image, slot)  # already in the model's channel order
+            height, width = decoded.shape[:2]
+            tfm = self.aug.get_transform(decoded)
+            image = tfm.apply_image(decoded, device=self.device, flip_channels=False)
+        else:
+            height, width = original_image.shape[:2]
+            tfm = self.aug.get_transform(original_image)
+            image = tfm.apply_image(self._upload(original_image, slot), device=self.device, flip_channels=self.input_format == "RGB")
         inputs = {"image": image, "height": height, "width": width}
         if text_prompt is not None:
             inputs["prompt"] = "text"
@@ -173,7 +213,8 @@ class DefaultPredictor:
         return inputs
 
     def __call__(self, original_image, text_prompt=None, mask_prompt=None):
-        """original_image: np.ndarray (H, W, C) in BGR order.  Returns the model's output dict for this one image."""
+        """original_image: np.ndarray (H, W, C) in BGR order, or a JPEG file as a path or bytes (decoded on the device,
+        ape_b200.engine.read_image).  Returns the model's output dict for this one image."""
         with torch.no_grad():
             return self.model([self.preprocess(original_image, text_prompt, mask_prompt)])[0]
 
@@ -182,7 +223,9 @@ class DefaultPredictor:
         pipelined: while the device runs the forward of image i, the host stages, uploads and resizes image i+1 and unpacks the
         detections of image i-1 — the device never waits for the host between images.  Boxes-only configurations go through
         `model.forward_packed` (results stay on the device until one small pinned copy); configurations with masks / semantic /
-        panoptic outputs run one by one (their post-processing synchronises).  Returns the list of output dicts."""
+        panoptic outputs run one by one (their post-processing synchronises).  `images` may mix arrays and JPEG files (paths
+        or bytes); the device decode of image i+1 runs on a side stream under the forward of image i.  Returns the list of
+        output dicts."""
         from ..parallel import unpack_packed
 
         m = getattr(self.model, "model_vision", self.model)

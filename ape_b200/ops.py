@@ -1416,6 +1416,57 @@ def resize_u8_bilinear(img, new_h, new_w, flip_channels=False, out=None):
     return out[:, :new_h, :new_w]
 
 
+def jpeg_decode(info, data, format="BGR", device="cuda", host=None):
+    """Device decode of a JPEG file the header walk routed to the device (`ape_b200.jpeg.parse(data).device`): the uint8
+    [H, W, 3] tensor of detectron2's `read_image(file, format)` (EXIF orientation applied), bit for bit with Pillow.
+    One host-to-device copy carries the decoder tables and the compressed scan (ape_jpeg_decode, csrc/jpeg.cu); `host` is an
+    optional pinned uint8 tensor to stage it in (a fresh block of the pinned caching allocator otherwise).
+    Returns (image, status): status is a device int32 [1] that the stream sets to 0, or to the error bits of a corrupt scan;
+    `jpeg_check(status)` raises for the latter (it waits for the decode)."""
+    import numpy as np
+
+    from . import jpeg as J
+
+    _require(info.device, f"jpeg_decode: file not supported on the device ({info.reason})")
+    _require(format in ("BGR", "RGB"), f"jpeg_decode: format {format!r} (BGR or RGB)")
+    device = torch.device(device)
+    huff, comp, quant, rst = J.device_tables(info)
+    scan = np.frombuffer(data, np.uint8, info.scan_end - info.scan_start, info.scan_start)
+    words = np.concatenate([huff.ravel(), quant.ravel(), rst.ravel()]).astype(np.int32).view(np.uint8)
+    off = (words.size + 255) // 256 * 256
+    n = off + scan.size
+    if host is None or host.numel() < n:
+        host = torch.empty((n,), dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    hv[:words.size] = words
+    hv[off:n] = scan
+    dev = host[:n].to(device, non_blocking=True)
+    base = dev.data_ptr()
+    comp = np.ascontiguousarray(comp[:info.ncomp])
+    args = (scan.size, comp.ctypes.data, info.ncomp, info.height, info.width, info.restart_interval)
+    wsb = int(_lib.lib.ape_jpeg_workspace_bytes(*args))
+    _require(wsb > 0, "jpeg_decode: bad geometry")
+    ws = torch.empty((wsb,), dtype=torch.uint8, device=device)
+    status = torch.empty((1,), dtype=torch.int32, device=device)
+    oh, ow = info.oriented_hw
+    out = torch.empty((oh, ow, 3), dtype=torch.uint8, device=device)
+    with torch.cuda.device(device), _timed(("jpeg", info.height, info.width, info.ncomp)):
+        rc = _lib.lib.ape_jpeg_decode(base + off, scan.size, base, huff.shape[0], base + huff.nbytes, comp.ctypes.data, info.ncomp,
+                                      info.height, info.width, info.restart_interval,
+                                      base + huff.nbytes + quant.nbytes if rst.size else None, info.orientation,
+                                      1 if format == "BGR" else 0, ws.data_ptr(), wsb, status.data_ptr(), out.data_ptr(),
+                                      _lib.current_stream_ptr())
+    _lib.check(rc, "ape_jpeg_decode")
+    return out, status
+
+
+def jpeg_check(status):
+    """Raise RuntimeError (with ape_last_error()'s description) when a device decode found a corrupt scan."""
+    code = int(status.item())
+    if code:
+        _lib.check(_lib.lib.ape_jpeg_status_error(code), "ape_jpeg_decode")
+
+
 def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=64):
     """[grad_value, grad_sampling_loc, grad_attn_weight] (ape_msda_bwd; ms_deform_attn_cuda.cu:84-160).  grad_value is
     accumulated in fp32 by vector atomics and cast to value's dtype at the end."""

@@ -441,6 +441,29 @@ int ape_resample_u8(const uint8_t *src, int64_t src_pitch, uint8_t *tmp, float *
                     const int *bounds_h, const int *kk_h, int ksize_h, const int *bounds_v, const int *kk_v, int ksize_v, int H,
                     int W, int C, int new_h, int new_w, int flip_channels, void *stream);
 
+/*
+ * JPEG decode on the device (DESIGN.md 4.16): detectron2 read_image(file, format) of a sequential-Huffman JPEG, bit for bit
+ * with Pillow (libjpeg defaults: JDCT_ISLOW, fancy upsampling), for the files ape_b200/jpeg.py routes here (8-bit, 1 or 3
+ * components, YCbCr 4:4:4 / 4:2:2 / 4:2:0, one interleaved scan, with or without restart markers).
+ *   scan             device bytes of the entropy-coded segment (SOS payload end .. the marker after it), scan_bytes > 0
+ *   huff             device int32 [n_tables, 1024] decoder tables (jpeg.py huffman_lut), 1 <= n_tables <= 6
+ *   quant            device int32 [n_q, 64] quantisation tables, natural order
+ *   comp             HOST int32 [ncomp, 4]: (DC table, AC table, quant table, h << 4 | v) per component
+ *   restart_offsets  device int32: byte offset (from the scan start) of restart intervals 1.. (two bytes past each RSTn);
+ *                    read only when restart_interval > 0 and the scan has more than one interval
+ *   orientation      EXIF orientation 1..8 (other values: none); bgr: channel order of out
+ *   workspace        ape_jpeg_workspace_bytes(...) bytes; status: device int, written (0 = ok) by the call
+ *   out              uint8 [H', W', 3], (H', W') = (width, height) for orientations 5..8, else (height, width)
+ * No allocation, no synchronisation.  Corrupt data (an invalid Huffman code, data ending inside a needed codeword, fewer blocks
+ * than the frame holds) is reported through *status after the stream reaches it; ape_jpeg_status_error(status) turns a
+ * non-zero word into an APE_ERR_INVALID_ARG with its description in ape_last_error().  Every read stays inside the scan.
+ */
+int64_t ape_jpeg_workspace_bytes(int scan_bytes, const int *comp, int ncomp, int height, int width, int restart_interval);
+int ape_jpeg_decode(const uint8_t *scan, int scan_bytes, const int *huff, int n_tables, const int *quant, const int *comp,
+                    int ncomp, int height, int width, int restart_interval, const int *restart_offsets, int orientation, int bgr,
+                    void *workspace, int64_t workspace_bytes, int *status, uint8_t *out, void *stream);
+int ape_jpeg_status_error(int status);
+
 /* Decoder reference-point update (deformable_transformer_vl.py:268-300, 4-d reference points): new_ref [B,Q,4] =
  * sigmoid(delta + inverse_sigmoid(ref, eps)) and ref_in [B,Q,L,4] = new_ref[:,:,None] * cat(valid_ratios, valid_ratios)[:,None]
  * (valid_ratios [B,L,2]); all fp32, same operation order as the PyTorch sequence. */
